@@ -1,4 +1,4 @@
-"""Build libb200rl.so in-tree with nvcc for sm_100a (no torch dependency in the library)."""
+"""Build libb200rl.so in-tree with nvcc for sm_90a (no torch dependency in the library)."""
 import os
 import shutil
 import subprocess
@@ -7,8 +7,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200rl.so")
-SOURCES = ["api.cu", "gemm_tcgen05.cu", "conv_shift.cu", "gae.cu", "conv_lowering.cu", "policy_heads.cu", "optim.cu", "replay.cu", "obs_encode.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["api.cu", "gemm_wgmma.cu", "conv_shift.cu", "gae.cu", "conv_lowering.cu", "policy_heads.cu", "optim.cu", "replay.cu", "obs_encode.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -63,7 +63,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed building libb200rl")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-lcudart"]
+    cmd = [nvcc] + NVCC_FLAGS[:2] + ["-shared", "-o", LIB] + objs + ["-lcudart"]
     subprocess.check_call(cmd)
     with open(STAMP, "w") as f:
         f.write(_source_hash() + "\n")

@@ -1,4 +1,4 @@
-"""Policy / value network for the PPO2 learner on the B200 kernels.
+"""Policy / value network for the PPO2 learner on the H100 kernels.
 
 Behavioural mirror of the reference's common/policies.py (build_policy :121-179, PolicyWithValue
 :13-119), common/distributions.py (CategoricalPd :153-204, DiagGaussianPd :227-251) and
@@ -299,7 +299,7 @@ class PolicyNet:
         bn = 256 if N2 == 256 else (128 if N2 > 64 else 64)
         tiles = -(-a.K // 128) * -(-N2 // bn)
         kb = -(-B // 64)
-        split = max(1, min(kb // 2 if kb >= 2 else 1, -(-296 // tiles)))
+        split = max(1, min(kb // 2 if kb >= 2 else 1, -(-2 * ops.num_sms() // tiles)))
         self.g0cat.zero_()
         for xs in ((x, x[:, a.Kp:]) if a.split_in else (x,)):
             ops.gemm(xs, self.dz0cat, self.g0cat, M=a.K, N=N2, K=B, lda=ldx, ldb=N2, ldc=N2, mn_major=True,

@@ -228,7 +228,7 @@ class VecFrameStack(VecEnvWrapper):
     cleared when its episode ends.
 
     reset()/step_wait() are the reference's host implementation (np.roll on a [N, H, W, nstack*c] array).  The
-    B200 Runner does not call them: it sees `frame_stack_device`, pulls the UNSTACKED frames with step_frames()
+    device Runner does not call them: it sees `frame_stack_device`, pulls the UNSTACKED frames with step_frames()
     (1/nstack of the bytes over PCIe) and applies the same update to the HBM-resident rollout buffer with
     b200rl_frame_stack -- the previous stacked observation is already there as rollout.obs[t-1]."""
     frame_stack_device = True

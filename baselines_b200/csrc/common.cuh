@@ -1,4 +1,4 @@
-// Shared device/host helpers for libb200rl (sm_100a only).
+// Shared device/host helpers for libb200rl (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -35,8 +35,18 @@ inline int check_launch(const char* what) {
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline long long ceil_div_ll(long long a, long long b) { return (a + b - 1) / b; }
 
+// Deterministic cross-CTA reductions: instead of float atomics (whose order, and so whose rounding, changes from run
+// to run) every CTA stores its partial result into a device workspace and sum_partials() adds the parts in index order.
+// det_workspace() returns a per-device buffer of at least `floats` floats; it only grows outside stream capture, and a
+// buffer is never freed, so captured graphs keep valid pointers.  Its users must be ordered on the device: every
+// reduction of the training path is issued on the caller's current stream.
+float* det_workspace(size_t floats, cudaStream_t stream);
+// out[r * ldo + c] += sum_{p < parts} ws[(p * rows + r) * cols + c], parts summed in order
+int sum_partials(const float* ws, int parts, long long rows, int cols, float* out, long long ldo, cudaStream_t stream);
+int device_num_sms();   // streaming multiprocessors of the current device (grid sizing)
+
 #ifdef __CUDACC__
-// ------------------------------------------------------------------ mbarrier / TMA / tcgen05 PTX
+// ------------------------------------------------------------------ mbarrier / TMA / wgmma PTX
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
@@ -58,8 +68,8 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 // try_wait suspends the warp until the phase completes or the hint expires; without a hint the default time limit is
-// short and the polling loop (YIELD / TRYWAIT / BRA) of the ~20 waiting warps took 21 % of all issued instructions in
-// the conv kernels (profiles/r2_ncu_conv_fwd.md) -- issue slots the producer and epilogue warps need.
+// short and the polling loop (YIELD / TRYWAIT / BRA) of the waiting warps takes issue slots the producer and
+// consumer warps need.
 static constexpr uint32_t MBAR_SUSPEND_NS = 20000;
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -103,77 +113,12 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, u
                : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem], fp16 operands, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// The same MMA with each 64-bit shared-memory descriptor passed as (low word, high word).  These kernels issue many
-// SMALL MMAs (N = 32..128: 16-64 tensor-core clocks each), so the single issuing thread's own instruction stream is
-// the bound (tools/conv_roles.py): inside an unrolled loop only the 14-bit start-address field of the low word
-// changes, and this form costs one uniform add per operand and MMA instead of rebuilding two 64-bit values.
-// ACC is the compile-time accumulate flag (false: overwrite D).
-template <bool ACC>
-__device__ __forceinline__ void umma_f16_lh(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                            uint32_t idesc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "n"(ACC ? 1 : 0)
-      : "memory");
-}
-// ... and with a run-time accumulate flag
-__device__ __forceinline__ void umma_f16_lhp(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 16 consecutive fp32 columns: thread i <- lane (base+i), columns [col, col+16)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// wgmma.mma_async ordering: fence before the first MMA that touches accumulator registers written by ordinary
+// instructions; MMAs issued since the last commit form a group; wait until at most N groups are pending.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------------------------------ small reductions
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,4 +1,4 @@
-// Lowering of NHWC convolutions (tf.nn.conv2d, a2c/utils.py:56 of the reference) onto the tcgen05 GEMM:
+// Lowering of NHWC convolutions (tf.nn.conv2d, a2c/utils.py:56 of the reference) onto the wgmma GEMM:
 //   im2col  : patches -> cols[B*OH*OW, rf*rf*C] fp16, K ordered (ky, kx, c) = HWIO weight flatten order
 //             - uint8 source: the uint8->fp16 cast of models.py:19 is fused into this first load (the /255
 //               is folded into the fp16 copy of the c1 weights), and the minibatch gather of
@@ -184,9 +184,9 @@ s2d_gather_kernel(const uint8_t* __restrict__ x, const long long* __restrict__ s
   }
 }
 
-// db[c] += alpha * sum_rows dz[row, c]
+// part[block, c] = alpha * sum over the block's rows of dz[row, c]  (colsum_impl adds the blocks' parts in order)
 __global__ void __launch_bounds__(256)
-colsum_kernel(const __half* __restrict__ dz, float* __restrict__ db, long long rows, int C, long long ld, float alpha,
+colsum_kernel(const __half* __restrict__ dz, float* __restrict__ part, long long rows, int C, long long ld, float alpha,
               int rows_per_block) {
   __shared__ float red[256];
   const int cw = C < 256 ? C : 256;
@@ -207,7 +207,7 @@ colsum_kernel(const __half* __restrict__ dz, float* __restrict__ db, long long r
     if (tid < cw && cbase + tid < C) {
       float s = 0.0f;
       for (int gI = 0; gI < groups; ++gI) s += red[gI * cw + tid];
-      atomicAdd(db + cbase + tid, s * alpha);
+      part[(long long)blockIdx.x * C + cbase + tid] = s * alpha;
     }
     __syncthreads();
   }
@@ -215,7 +215,7 @@ colsum_kernel(const __half* __restrict__ dz, float* __restrict__ db, long long r
 
 // same sum with 16-byte loads: thread = (row group, 8-column slice); C and ld multiples of 8, 16-byte aligned base
 __global__ void __launch_bounds__(256)
-colsum_vec_kernel(const __half* __restrict__ dz, float* __restrict__ db, long long rows, int C, long long ld, float alpha,
+colsum_vec_kernel(const __half* __restrict__ dz, float* __restrict__ part, long long rows, int C, long long ld, float alpha,
                   int rows_per_block) {
   __shared__ float red[256][9];
   const int slices = C >> 3;                         // 8-column slices per row (<= 32)
@@ -244,13 +244,13 @@ colsum_vec_kernel(const __half* __restrict__ dz, float* __restrict__ db, long lo
     const int s2 = tid >> 3, i = tid & 7;
     float s = 0.0f;
     for (int gI = 0; gI < groups; ++gI) s += red[gI * slices + s2][i];
-    atomicAdd(db + tid, s * alpha);
+    part[(long long)blockIdx.x * C + tid] = s * alpha;
   }
 }
 
 static int grid_for(long long total, int threads) {
   long long blocks = (total + threads - 1) / threads;
-  const long long cap = 148LL * 32;
+  const long long cap = (long long)device_num_sms() * 32;
   return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
 }
 
@@ -343,7 +343,7 @@ int frame_stack_impl(const void* prev, const void* frame, const void* news, void
                     (reinterpret_cast<uintptr_t>(frame) & 3) == 0;
   if (K == 4 && c == 1) {
     if (al16 && pixels % 4 == 0) {
-      const int grid = (int)std::min<long long>((total / 4 + 255) / 256, 148LL * 16);
+      const int grid = (int)std::min<long long>((total / 4 + 255) / 256, (long long)device_num_sms() * 16);
       frame_stack_k4_kernel<4><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint32_t*>(prev),
                                                         reinterpret_cast<const uint8_t*>(frame),
                                                         reinterpret_cast<const uint8_t*>(news),
@@ -351,14 +351,14 @@ int frame_stack_impl(const void* prev, const void* frame, const void* news, void
     } else {
       B200RL_REQUIRE(((reinterpret_cast<uintptr_t>(prev) | reinterpret_cast<uintptr_t>(out)) & 3) == 0,
                      "frame_stack: stacked buffers must be 4-byte aligned");
-      const int grid = (int)std::min<long long>((total + 255) / 256, 148LL * 16);
+      const int grid = (int)std::min<long long>((total + 255) / 256, (long long)device_num_sms() * 16);
       frame_stack_k4_kernel<1><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint32_t*>(prev),
                                                         reinterpret_cast<const uint8_t*>(frame),
                                                         reinterpret_cast<const uint8_t*>(news),
                                                         reinterpret_cast<uint32_t*>(out), pixels, total);
     }
   } else {
-    const int grid = (int)std::min<long long>((total + 255) / 256, 148LL * 16);
+    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)device_num_sms() * 16);
     frame_stack_generic_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(prev),
                                                         reinterpret_cast<const uint8_t*>(frame),
                                                         reinterpret_cast<const uint8_t*>(news),
@@ -400,15 +400,21 @@ int col2im_impl(const void* dcols, const void* saved, void* dx, long long B, int
 
 int colsum_impl(const void* dz, float* db, long long rows, int C, long long ld, float alpha, cudaStream_t stream) {
   B200RL_REQUIRE(dz && db && rows > 0 && C > 0, "colsum: bad args");
-  long long rpb = (rows + 148LL * 8 - 1) / (148LL * 8);
+  long long rpb = (rows + (long long)device_num_sms() * 8 - 1) / ((long long)device_num_sms() * 8);
   if (rpb < 64) rpb = 64;
   const int grid = (int)((rows + rpb - 1) / rpb);
+  float* part = det_workspace((size_t)grid * C, stream);
+  if (!part) return B200RL_ERR_CUDA;
+  int rc;
   if ((C & 7) == 0 && C <= 256 && (ld & 7) == 0 && (reinterpret_cast<uintptr_t>(dz) & 15) == 0) {
-    colsum_vec_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(dz), db, rows, C, ld, alpha, (int)rpb);
-    return check_launch("colsum_vec_kernel");
+    colsum_vec_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(dz), part, rows, C, ld, alpha, (int)rpb);
+    rc = check_launch("colsum_vec_kernel");
+  } else {
+    colsum_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(dz), part, rows, C, ld, alpha, (int)rpb);
+    rc = check_launch("colsum_kernel");
   }
-  colsum_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(dz), db, rows, C, ld, alpha, (int)rpb);
-  return check_launch("colsum_kernel");
+  if (rc == B200RL_OK) rc = sum_partials(part, grid, 1, C, db, C, stream);
+  return rc;
 }
 
 }  // namespace b200rl

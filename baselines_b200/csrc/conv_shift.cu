@@ -1,8 +1,8 @@
-// "Shift-GEMM" convolutions for sm_100a: stride-1 convolutions over an NHWC fp16 activation viewed as a plain
+// "Shift-GEMM" convolutions for sm_90a: stride-1 convolutions over an NHWC fp16 activation viewed as a plain
 // 2-D matrix X[rows = (n, y, x) grid positions, C] (strided convs are brought to this form by space-to-depth).
 //
 // Every input row is loaded into shared memory ONCE per tile by a tiled 2-D TMA; each filter tap (r, s) is then
-// just the same smem buffer read through a UMMA descriptor whose start address is shifted by (r*Wg + s) rows
+// just the same smem buffer read through a wgmma descriptor whose start address is shifted by (r*Wg + s) rows
 // (a SWIZZLE_128B descriptor may start at any 128-byte row: the swizzle is a function of the smem address).
 // This removes the R*S-fold duplication of an im2col operand on the L2->SM path.
 //
@@ -10,15 +10,14 @@
 //                                       and, with negative shifts over a zero-bordered dY, the data gradient
 //                                       dX[m, :] = ( sum_t dY[m - sh_t, :] * W_t ) * act'(saved)
 //   conv_shift_wgrad_kernel (MN-major): G[t, c, n] += alpha * sum_m X[m + sh_t, c] * dY[m, n]         wgrad
-//                                       (all taps' accumulators live in TMEM at once; X and dY are read once)
+//                                       (a CTA keeps the accumulators of up to 2*QW taps x 64 channels in registers;
+//                                        X and dY are read once per such group of taps)
 //
-// Warp roles (forward, 384 threads; uint8-fed first layer 896): 0 TMA loads (weights once, A tile per tile) | 1 and 3
-// MMA issue (elect.sync) for the even / odd tiles | 2 TMEM alloc | 4-7 / 8-11 epilogue sets for the even / odd tiles
-// (4 TMEM accumulator stages; first layer: four sets, warps 4-19) | first layer only: the last 8 warps are uint8
-// producers that cast raw frames into a rolling A ring instead of the TMA.  wgrad (256 threads [+256]): 0 TMA | 1 and 3 MMA issue for the even / odd k-blocks (own accumulators each, when two
-// sets fit in TMEM) | 2 TMEM | 4-7 fused bias-gradient sums during the main loop, then the epilogue | 8-15 uint8 producers.
-// The forward epilogue can also write 1 bit per output element (act > 0); the dgrad of the next layer reads that
-// instead of the fp16 activation.
+// Warp roles: warps 0-7 are two consumer warpgroups (rows [64g, 64g+64) of every 128-row tile; they issue the
+// wgmma.mma_async chains, and run the epilogue -- or, in the wgrad, the fused bias-gradient sums -- from their own
+// registers) | warp 8 TMA loads | uint8-fed first layer only: warps 9-16 are uint8 producers that cast raw frames
+// into a rolling A ring instead of the TMA.  The forward epilogue can also write 1 bit per output element (act > 0);
+// the dgrad of the next layer reads that instead of the fp16 activation.
 //
 // Outputs at grid positions that are not valid conv outputs are computed from wrapped rows and discarded (fwd),
 // or multiply a zero of the zero-bordered dY (wgrad / dgrad) -- so dY tensors live on the conv's INPUT grid.
@@ -31,21 +30,12 @@
 namespace b200rl {
 
 static constexpr int SH_BM = 128;
-static constexpr int SH_THREADS = 256;             // wgrad: TMA, MMA, TMEM alloc, MMA, 4 bias-sum / epilogue warps
-// forward: epilogue sets x SH_CG column groups x 4 lane quadrants of epilogue warps.  A second column group was
-// measured 3-6 % slower on all three layers (profiles/r2_ncu_conv_fwd_xfold_cg2.md: per-warp overhead, more waiting warps).
-static constexpr int SH_CG = 1;
-// Epilogue warp sets of the forward kernel (4 warps x SH_CG each; set e takes the tiles i = e mod sets).  The uint8-fed
-// layer has four: its epilogue's tcgen05.ld queues behind the other tile's MMAs, and with two sets that wait was on
-// the critical path (tools/conv_roles.py: MMA + epilogue alone took the sum of their times).
-__host__ __device__ constexpr int sh_epi_sets(bool u8) { return u8 ? 4 : 2; }
-__host__ __device__ constexpr int sh_epi_warps(bool u8) { return sh_epi_sets(u8) * SH_CG * 4; }
-__host__ __device__ constexpr int sh_fwd_threads(bool u8) { return 128 + sh_epi_warps(u8) * 32 + (u8 ? 256 : 0); }
+static constexpr int SH_CONSUMER_WARPS = 8;        // two warpgroups, 64 tile rows each
+static constexpr int SH_TMA_WARP = SH_CONSUMER_WARPS;
+__host__ __device__ constexpr int sh_threads(bool u8) { return (SH_CONSUMER_WARPS + 1) * 32 + (u8 ? 256 : 0); }
 static constexpr int SH_MAX_TAPS = 16;
 // rows of one TMA-fed A stage: 128 + the largest shift span.  64-channel inputs: span <= 32.  128-channel inputs (two
-// halves per stage): span <= 16, so that FOUR stages fit beside the weights -- the stage count must be even, because
-// the two MMA-issuing warps alternate over the tiles and each must own its stages' barriers (a warp that met only
-// every other phase of an mbarrier could mistake an old phase of that parity for the one it waits for).
+// halves per stage): span <= 16, so that four stages fit beside the weights.
 __host__ __device__ constexpr int sh_arows(int KH) { return KH == 1 ? 160 : 144; }
 __host__ __device__ constexpr int sh_stages(int KH) { return KH == 1 ? 6 : 4; }
 __host__ __device__ constexpr int sh_wgrad_krows(bool u8) { return u8 ? 128 : 64; }   // wgrad: reduction rows per stage
@@ -53,6 +43,8 @@ __host__ __device__ constexpr int sh_wgrad_krows(bool u8) { return u8 ? 128 : 64
 __host__ __device__ constexpr int sh_wres_bytes(int KH) { return KH == 1 ? 80 * 1024 : 64 * 1024; }
 static constexpr int SH_WROWS_K = 96;                // wgrad: 64 + max shift span (<= 32)
 static constexpr int SH_WABYTES = SH_WROWS_K * 128;
+// wgrad: 64-channel accumulator chunks per consumer warpgroup (2 * QW * N/2 registers per thread)
+__host__ __device__ constexpr int sh_wgrad_qw(int BN, bool u8) { return u8 ? 2 : (BN == 64 ? 2 : 4); }
 
 // address map of an output / saved tensor: grid position (n, y, x) + column -> element offset
 struct AddrMap {
@@ -113,7 +105,6 @@ struct U8Src {
 };
 
 static constexpr int U8_WARPS = 8;
-static constexpr int U8_THREADS = U8_WARPS * 32;
 
 // 16 uint8 -> 16 fp16 (exact): bytes are spliced into 0x64xx (= 1024 + b) and 1024 is subtracted
 __device__ __forceinline__ void u8x16_to_f16(const uint4& q, uint4& lo, uint4& hi) {
@@ -140,14 +131,13 @@ __device__ __forceinline__ void u8x16_to_f16(const uint4& q, uint4& lo, uint4& h
 // unit that mirrors the first unit of stage 0, so the tile in the last stage can read past the end.
 //
 // The raw bytes go global -> registers -> cast -> one swizzled store: no staging copy in shared memory (the port is
-// shared with the tensor core's SS operand fetch, which wins the arbitration), and no 25-50 % of halo rows cast twice.
-// What bounds the producers is measured in profiles/r2_conv_roles.md (not load latency: depth 2, 3, 4 time the same).
+// shared with the tensor core's operand fetch), and no 25-50 % of halo rows cast twice.
 //
 // Work unit = 32 consecutive grid rows (one warp, lane = row); unit u of the CTA covers rows row_start + 32u ...,
 // belongs to tile u / UPT, and the units are dealt round-robin to the U8_WARPS producer warps.  Each warp keeps
 // D units of loads in flight in registers (the sample index of the gather is looked up one round earlier).
 // Barriers per stage: full (UPT unit arrivals [+ the TMA of the other operand]), head (the first unit alone: the
-// tile in the PREVIOUS stage waits for it), empty (tcgen05.commit of the tile's MMAs).
+// tile in the PREVIOUS stage waits for it), empty (every consumer warp, once the tile's MMAs retired).
 
 __device__ __forceinline__ uint4 ldg_stream_v4(const void* p) {
   uint4 v;
@@ -195,11 +185,10 @@ __device__ __forceinline__ void u8_load(const U8Src& u, long long row_start, int
 template <int TR, int STAGES, int D>
 __device__ __forceinline__ void u8_ring_producer(const U8Src& u, long long M, long long row_start, int ntiles,
                                                  uint8_t* ring, uint64_t* full_bar, uint64_t* head_bar,
-                                                 uint64_t* empty_bar, int pw, int lane, bool dry = false) {
+                                                 uint64_t* empty_bar, int pw, int lane) {
   using R = U8Ring<TR, STAGES>;
   constexpr int UPT = R::UPT, RND = U8_WARPS * D;
   if (ntiles <= 0) return;
-  if (dry) M = 0;                                        // diagnostics: every row "outside the matrix": no loads
   const int total = ntiles * UPT + 1;                    // + the head unit the last tile reads into
   // row_sw = address of this lane's row of unit 0 of stage 0, + ((lane & 7) << 4): chunk c of a row lives at row_sw ^ (c << 4)
   const uint32_t ring0 = smem_u32(ring) + lane * 128 + ((lane & 7) << 4);
@@ -224,7 +213,7 @@ __device__ __forceinline__ void u8_ring_producer(const U8Src& u, long long M, lo
         const uint32_t dst = ring0 + (uint32_t)(s * TR + ub * 32) * 128u;
         const bool mirror = (s == 0) && (ub == 0);
 #pragma unroll
-        for (int dy = 0; dy < 4 && !dry; ++dy) {
+        for (int dy = 0; dy < 4; ++dy) {
           uint4 lo, hi;
           u8x16_to_f16(q[d][dy], lo, hi);
           st_shared_v4(dst ^ (uint32_t)((2 * dy) << 4), lo);
@@ -234,7 +223,7 @@ __device__ __forceinline__ void u8_ring_producer(const U8Src& u, long long M, lo
             st_shared_v4((dst + (uint32_t)(STAGES * TR) * 128u) ^ (uint32_t)((2 * dy + 1) << 4), hi);
           }
         }
-        fence_proxy_async_smem();                        // generic-proxy writes -> visible to the tensor core
+        fence_proxy_async_smem();                        // generic-proxy writes -> visible to wgmma
         __syncwarp();
         if (lane == 0) {
           if (tile < ntiles) mbar_arrive(&full_bar[s]);
@@ -247,27 +236,14 @@ __device__ __forceinline__ void u8_ring_producer(const U8Src& u, long long M, lo
   }
 }
 
-// bit k of the result = (fp16 element k of the 16 packed values > 0): one packed compare (0xffff per true half) and
-// one LOP3 per pair instead of two compares, two selects and two ORs
-__device__ __forceinline__ uint16_t relu_bits16(const uint32_t (&packed)[8]) {
-  const __half2 z = __floats2half2_rn(0.0f, 0.0f);
-  uint32_t acc = 0;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const uint32_t m = __hgt2_mask(*reinterpret_cast<const __half2*>(&packed[i]), z);
-    acc |= m & ((1u << (2 * i)) | (0x20000u << (2 * i)));
-  }
-  return (uint16_t)((acc & 0xffffu) | (acc >> 16));
-}
-
 struct ShiftParams {
   U8Src u8;
   FastDiv fwg, fhg;        // epilogue row -> (n, y, x)
   long long M;             // grid rows = B*Hg*Wg
   int Hg, Wg;              // grid
-  int N;                   // output channels of the conv (the MMA's N is KX * N when the x-taps are folded)
-  int taps;                // taps the MMA loop accumulates over (KX > 1: the ky row-taps only)
-  int tstep;               // output rows per tile: 128 - (KX - 1)
+  int N;                   // output channels of the conv
+  int taps;                // filter rows (kx > 1) or taps (kx == 1)
+  int kx;                  // taps per filter row: tap (a, b) reads rows shifted by shift[a] + b
   int shift[SH_MAX_TAPS];  // row shift of tap t, relative to min_shift (>= 0)
   int min_shift;           // smallest absolute shift (negative for dgrad)
   int vy, vx;              // rows with y < vy && x < vx produce an output
@@ -281,83 +257,47 @@ struct ShiftParams {
   int act, dact;           // dact = 1: multiply by act'(saved) instead of applying act
   float alpha;
   int num_tiles;
-  int debug;               // diagnostics (B200RL_CONV_DEBUG): 1 producers / TMA move no data, 2 no MMAs, 4 no epilogue work
 };
 
 // ------------------------------------------------------------------------------------------------ forward / dgrad
-// KX > 1 ("x-fold"): the KX horizontally adjacent filter taps of one filter row are folded into the MMA's N
-// dimension -- D[m, (b, n)] = sum_{a, c} X[m + a*Wg, c] * W[(a, b), c, n] -- so every A slab is fetched from shared
-// memory once per filter ROW instead of once per tap (tcgen05 SS operand fetch is 128 B/clk and is the bound of
-// these N <= 64 kernels, profiles/r2_mma_probe.jsonl).  The epilogue finishes the sum across lanes:
-// out[m, n] = sum_b D[m + b, b*N + n] (warp shuffle by b lanes; the last b lanes of a warp take the rows from the next
-// warp through a tiny smem exchange; tiles overlap by KX - 1 rows so nothing crosses a tile).
-template <int BN, int KH, bool DACT, bool U8, int KX>
-__global__ void __launch_bounds__(sh_fwd_threads(U8), 1)
+// Weights: [kx*BN rows (b, n), taps*KH*64 columns (a, h, c)], all resident in shared memory as (a, h) sub-tiles of
+// kx*BN rows x 128 B; tap (a, b) uses rows [b*BN, b*BN + BN) of them.
+template <int BN, int KH, bool DACT, bool U8>
+__global__ void __launch_bounds__(sh_threads(U8), 1)
 conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                       const __grid_constant__ ShiftParams p) {
-  static_assert(KX == 1 || !DACT, "the data gradient keeps one MMA group per tap");
-  static_assert(!(U8 && KX > 1), "the rolling A ring needs tiles that start a whole tile apart");
-  constexpr int NO = BN / KX;                        // output channels
-  constexpr int TSTEP = SH_BM - (KX - 1);
   constexpr int SH_ABYTES = sh_arows(KH) * 128;      // one 64-channel half of an A stage
   constexpr int STAGE_BYTES = KH * SH_ABYTES;
   constexpr int STAGES = sh_stages(KH);
-  static_assert(STAGES % 2 == 0, "each MMA-issuing warp owns alternate stages");
   using Ring = U8Ring<SH_BM, STAGES>;                // uint8-fed first layer: rolling ring instead of per-tile stages
   constexpr int A_PITCH = U8 ? SH_BM * 128 : STAGE_BYTES;
   constexpr int A_TOTAL = U8 ? Ring::BYTES : STAGES * STAGE_BYTES;
-  constexpr int W_SUB = BN * 128;                    // one (tap, half) weight sub-tile
-  // Accumulator stages.  The hand-off of a TMEM stage (tcgen05.commit -> mbarrier -> epilogue warps wake, read, arrive
-  // -> MMA warp wakes) costs on the order of a whole tile of these small MMAs (tools/conv_roles.py: a tile loop with all
-  // data movement and math removed still runs at ~40 % of the full kernel's time), so two stages leave the tensor core
-  // idle; four hide it.  Two epilogue warp sets still alternate over the tiles.
-  constexpr int NACC = (BN <= 128) ? 4 : 2;
-  constexpr int NSETS = sh_epi_sets(U8), EPI_WARPS = sh_epi_warps(U8);
-  static_assert(NACC % NSETS == 0, "each epilogue set owns its accumulator stages' barriers");
-  constexpr int TMEM_COLS = (NACC * BN <= 64) ? 64 : (NACC * BN <= 128) ? 128 : (NACC * BN <= 256) ? 256 : 512;
-  static_assert(NACC * BN <= 512, "accumulator stages exceed TMEM");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* wres = smem + A_TOTAL;                    // resident weights: taps*KH sub-tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(wres + sh_wres_bytes(KH));
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + NACC;
-  uint64_t* w_bar = bars + 2 * STAGES + 2 * NACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * NACC + 1);
-  uint64_t* head_bar = bars + 2 * STAGES + 2 * NACC + 2;   // U8: first unit of the stage's tile is in place
-  static_assert((3 * STAGES + 2 * NACC + 2) * 8 <= 256, "barrier block");
+  uint64_t* w_bar = bars + 2 * STAGES;
+  uint64_t* head_bar = bars + 2 * STAGES + 1;        // U8: first unit of the stage's tile is in place
+  static_assert((3 * STAGES + 1) * 8 <= 256, "barrier block");
 
-  __shared__ float s_bias[NO];
-  // x-fold halo exchange: [accumulator stage][parity][warp][halo row slot][column of the current chunk]
-  constexpr int NCG = NO / SH_CG;                                     // output columns per epilogue column group
-  static_assert(NCG % 16 == 0, "column groups are whole 16-column chunks");
-  constexpr int XG = (KX == 2 && NCG >= 32) ? 2 : 1;                  // 16-column chunks combined per exchange round
-  constexpr int XROWS = (KX * (KX - 1)) / 2;                          // sum_b b halo rows per warp
-  __shared__ float s_xch[(KX > 1) ? NSETS * SH_CG : 1][2][4][(KX > 1) ? XROWS : 1][16 * XG];
+  __shared__ float s_bias[BN];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x < NO) s_bias[threadIdx.x] = (p.bias && (int)threadIdx.x < p.N) ? p.bias[threadIdx.x] : 0.0f;
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmX);
-    tma_prefetch_desc(&tmW);
-  }
-  if (warp == 1 && lane == 0) {
+  const int w_sub = p.kx * BN * 128;                 // one (a, h) weight sub-tile
+  if (threadIdx.x < BN) s_bias[threadIdx.x] = (p.bias && (int)threadIdx.x < p.N) ? p.bias[threadIdx.x] : 0.0f;
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], U8 ? Ring::UPT : 1);
-      mbar_init(&empty_bar[s], U8 ? 2 : 1);                // ring: the stage's own tile and the tile before it (see the MMA warps)
+      // ring: a tile also reads the first unit of the next stage; the consumers finish tiles in order, so the next
+      // stage's own tile releasing it implies this one is done too
+      mbar_init(&empty_bar[s], SH_CONSUMER_WARPS);
       if (U8) mbar_init(&head_bar[s], 1);
     }
-    for (int s = 0; s < NACC; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], 128 * SH_CG); }
     mbar_init(w_bar, 1);
     fence_barrier_init();
-    if (U8) mbar_arrive(&empty_bar[0]);                    // stands in for "the tile before" the CTA's first tile
   }
-  if (warp == 2) tmem_alloc<TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // Tiles of this CTA: tile(i) = tile_first + i * tile_stride, i < tile_count.  TMA-fed layers interleave the CTAs
   // (neighbouring CTAs share L2 lines of the halo rows); the uint8-fed layer gives every CTA one consecutive run.
@@ -373,13 +313,12 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
     tile_count = tile_first < p.num_tiles ? (p.num_tiles - tile_first + tile_stride - 1) / tile_stride : 0;
   }
 
-  // Role loops are warp-uniform; only the issue of the uniform-datapath instructions (TMA, tcgen05.mma,
-  // tcgen05.commit) is gated by elect.sync -- a data-dependent `if (lane == 0)` makes the compiler wrap every
-  // such instruction in an ELECT / BRA.U.ANY loop (~300 instructions per tile on the issuing thread).
-  if (warp == 0) {
+  if (warp == SH_TMA_WARP) {
     if (elect_one()) {
-      mbar_arrive_expect_tx(w_bar, (uint32_t)(p.taps * KH) * W_SUB);
-      for (int q = 0; q < p.taps * KH; ++q) tma_load_2d(wres + q * W_SUB, &tmW, w_bar, q * 64, 0);
+      tma_prefetch_desc(&tmX);
+      tma_prefetch_desc(&tmW);
+      mbar_arrive_expect_tx(w_bar, (uint32_t)(p.taps * KH) * w_sub);
+      for (int q = 0; q < p.taps * KH; ++q) tma_load_2d(wres + q * w_sub, &tmW, w_bar, q * 64, 0);
     }
     __syncwarp();
     int s = 0;
@@ -391,7 +330,7 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
         if (elect_one()) {
           uint8_t* sa = smem + s * STAGE_BYTES;
           mbar_arrive_expect_tx(&full_bar[s], (uint32_t)STAGE_BYTES);
-          const int row0 = tile * TSTEP + p.min_shift;                  // may be negative: TMA zero-fills
+          const int row0 = tile * SH_BM + p.min_shift;                  // may be negative: TMA zero-fills
 #pragma unroll
           for (int h = 0; h < KH; ++h) tma_load_2d(sa + h * SH_ABYTES, &tmX, &full_bar[s], h * 64, row0);
         }
@@ -399,259 +338,98 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (U8 && warp >= 4 + EPI_WARPS) {
-    // uint8 producer warps (2 units of loads in flight each: 896 threads leave 72 registers)
+  } else if (U8 && warp > SH_TMA_WARP) {
+    // uint8 producer warps (2 units of loads in flight each)
     u8_ring_producer<SH_BM, STAGES, 2>(p.u8, p.M, (long long)tile_first * SH_BM + p.min_shift, tile_count, smem,
-                                       full_bar, head_bar, empty_bar, warp - (4 + EPI_WARPS), lane, (p.debug & 1) != 0);
-  } else if (warp == 1 || warp == 3) {
-    // TWO MMA-issuing warps, even / odd tiles.  tcgen05.mma issue is not fire-and-forget at this size: the issuing thread
-    // stalls on the (shallow) MMA queue, so with one issuer the per-tile barrier waits + commits (~430 clocks, measured
-    // with tools/conv_roles.py) ADD to the 16..36 small MMAs instead of hiding under them.  With two issuers one warp
-    // does its waits while the other feeds the tensor core; the two tiles use different TMEM stages (NACC even).
-    static_assert(NACC % 2 == 0, "issuers own alternate accumulator stages");
-    constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(SH_BM >> 4) << 24);
-    const int iss = warp >> 1;
-    int s = iss % STAGES, as = iss;
-    uint32_t ph = 0, aph = 0;
+                                       full_bar, head_bar, empty_bar, warp - (SH_TMA_WARP + 1), lane);
+  } else {
+    // consumer warpgroup wg: tile rows [64*wg, 64*wg + 64); thread t holds rows r0 and r0 + 8 of its accumulator
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const int r0 = wg * 64 + acc_row(t, 0);
+    const uint32_t w_base = smem_u32(wres);
+    const float lo = (p.act == ACT_RELU) ? 0.0f : -INFINITY;
+    const __half2 lo2 = __floats2half2_rn(lo, lo);
+    const __half2 zero2 = __floats2half2_rn(0.0f, 0.0f);
+    float acc[BN / 2];
+    int s = 0;
+    uint32_t ph = 0;
     mbar_wait(w_bar, 0);
-    // descriptors differ only in the 14-bit start-address field of their low word: the rest is built once, and
-    // every MMA adds (byte offset >> 4) to a low word (shared memory ends below 256 KB, so the field never carries)
-    constexpr uint64_t DESC0 = (1ull << 46) | (2ull << 61) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)(16 >> 4) << 16);
-    constexpr uint32_t D_HI = (uint32_t)(DESC0 >> 32), D_LO = (uint32_t)DESC0;
-    const uint32_t w_lo = D_LO + ((smem_u32(wres) & 0x3FFFFu) >> 4);
-    for (int i = iss; i < tile_count; i += 2) {
+    for (int i = 0; i < tile_count; ++i) {
+      const int tile = tile_first + i * tile_stride;
       const int s1 = (s + 1 == STAGES) ? 0 : s + 1;
-      mbar_wait(&tempty_bar[as], aph ^ 1);
       mbar_wait(&full_bar[s], ph);
       if (U8) mbar_wait(&head_bar[s1], s1 == 0 ? ph ^ 1 : ph);   // the shifted taps read into the next tile's first unit
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t a_lo = D_LO + ((smem_u32(smem + s * A_PITCH) & 0x3FFFFu) >> 4);
-        const uint32_t tmem_d = tmem_base + (uint32_t)(as * BN);
-        if (!(p.debug & 2)) {
-          // tap 0 overwrites the accumulator with its first MMA; the others accumulate
-          {
-            const uint32_t at = a_lo + (uint32_t)p.shift[0] * 8u;        // 128 B per row = 8 x 16 B
-#pragma unroll
-            for (int h = 0; h < KH; ++h) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                if (h == 0 && k == 0)
-                  umma_f16_lh<false>(tmem_d, at, D_HI, w_lo, D_HI, IDESC);
-                else
-                  umma_f16_lh<true>(tmem_d, at + h * (SH_ABYTES >> 4) + 2 * k, D_HI, w_lo + h * (W_SUB >> 4) + 2 * k,
-                                    D_HI, IDESC);
-              }
-            }
-          }
-          // not unrolled: an unrolled tap loop keeps dozens of descriptor pairs live and spills the uniform registers;
-          // the next tap's shift is fetched (constant bank) while this tap's MMAs are issued
-          uint32_t wt = w_lo;
-          uint32_t sh_next = (uint32_t)p.shift[1];
+      const uint32_t a_base = smem_u32(smem + s * A_PITCH) + (uint32_t)(wg * 64 * 128);
+      wgmma_fence();
+      // tap 0 overwrites the accumulator with its first MMA; the others accumulate
 #pragma unroll 1
-          for (int t = 1; t < p.taps; ++t) {
-            const uint32_t at = a_lo + sh_next * 8u;
-            sh_next = (uint32_t)p.shift[(t + 1) & (SH_MAX_TAPS - 1)];
-            wt += (uint32_t)KH * (W_SUB >> 4);
+      for (int a = 0; a < p.taps; ++a) {
+#pragma unroll 1
+        for (int b = 0; b < p.kx; ++b) {
+          const uint32_t at = a_base + (uint32_t)(p.shift[a] + b) * 128u;
+          const uint32_t wt = w_base + (uint32_t)(a * KH * w_sub + b * BN * 128);
 #pragma unroll
-            for (int h = 0; h < KH; ++h) {
+          for (int h = 0; h < KH; ++h) {
 #pragma unroll
-              for (int k = 0; k < 4; ++k)
-                umma_f16_lh<true>(tmem_d, at + h * (SH_ABYTES >> 4) + 2 * k, D_HI, wt + h * (W_SUB >> 4) + 2 * k, D_HI,
-                                  IDESC);
+            for (int k = 0; k < 4; ++k) {
+              const uint64_t adesc = make_sdesc(at + h * SH_ABYTES + k * 32, 16, 1024, 1);
+              const uint64_t bdesc = make_sdesc(wt + h * w_sub + k * 32, 16, 1024, 1);
+              wgmma_f16<BN, 0, 0>(acc, adesc, bdesc, (a | b | h | k) ? 1u : 0u);
             }
           }
         }
-        umma_commit(&empty_bar[s]);
-        // ring: this tile also read the head of the next stage, whose own tile belongs to the OTHER issuer -- that
-        // stage is free only when both tiles are done (barrier count 2)
-        if (U8) umma_commit(&empty_bar[s1]);
-        umma_commit(&tfull_bar[as]);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
-      s += 2;
-      if (s >= STAGES) { s -= STAGES; ph ^= 1; }
-      as += 2;
-      if (as >= NACC) { as -= NACC; aph ^= 1; }
-    }
-  } else if (warp >= 4 && warp < 4 + EPI_WARPS) {
-    // epilogue warp e = warp - 4: warp set eset = e / (4*SH_CG) (even / odd tiles; tile i sits in accumulator stage
-    // i % NACC, use number i / NACC), column group
-    // cg = (e / 4) % SH_CG, TMEM lane quadrant ew = warp % 4 (a warp reaches only that quadrant)
-    const int ew = warp & 3;
-    const int eset = (warp - 4) / (4 * SH_CG);
-    const int cg = ((warp - 4) >> 2) % SH_CG;
-    if constexpr (KX > 1) {
-      uint32_t par = 0;
-      for (int i = eset; i < tile_count; i += NSETS) {
-        const int tile = tile_first + i * tile_stride;
-        const int as = i % NACC;
-        const uint32_t aph = (uint32_t)(i / NACC) & 1u;
-        const int ml = ew * 32 + lane;
-        const uint32_t m = (uint32_t)tile * TSTEP + ml;
-        const uint32_t t2 = p.fwg.div(m);
-        const int x = (int)(m - t2 * (uint32_t)p.Wg);
-        const int n = (int)p.fhg.div(t2);
-        const int y = (int)(t2 - (uint32_t)n * (uint32_t)p.Hg);
-        const bool ok = (ml < TSTEP) && ((long long)m < p.M) && (y < p.vy) && (x < p.vx);
-        const long long obase = map_rowbase(p.omap, n, y, x);
-        const float lo = (p.act == ACT_RELU) ? 0.0f : -INFINITY;
-        mbar_wait(&tfull_bar[as], aph);
-        tc_fence_after();
-        const uint32_t taddr0 = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(as * BN);
-#pragma unroll 1
-        for (int c0 = cg * NCG; c0 < (cg + 1) * NCG; c0 += 16 * XG) {
-          uint32_t r[KX][XG][16];
+      if (lane == 0) mbar_arrive(&empty_bar[s]);
+
 #pragma unroll
-          for (int b = 0; b < KX; ++b)
-#pragma unroll
-            for (int j = 0; j < XG; ++j) tmem_ld16(taddr0 + b * NO + c0 + 16 * j, r[b][j]);
-          tmem_ld_wait();
-          // rows this warp's first lanes hold are the halo of the previous warp: publish them
-#pragma unroll
-          for (int b = 1; b < KX; ++b) {
-            if (lane < b) {
-              float* dst = s_xch[eset * SH_CG + cg][par][ew][(b * (b - 1)) / 2 + lane];
-#pragma unroll
-              for (int j = 0; j < XG; ++j)
-#pragma unroll
-                for (int i = 0; i < 16; ++i) dst[16 * j + i] = __uint_as_float(r[b][j][i]);
-            }
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + eset * SH_CG + cg) : "memory");
-#pragma unroll
-          for (int b = 1; b < KX; ++b) {
-            const bool halo = lane >= 32 - b;
-            const float* src = s_xch[eset * SH_CG + cg][par][(ew + 1) & 3][(b * (b - 1)) / 2 + (halo ? lane - (32 - b) : 0)];
-#pragma unroll
-            for (int j = 0; j < XG; ++j)
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                float v = __shfl_down_sync(0xffffffffu, __uint_as_float(r[b][j][i]), b);
-                if (halo) v = (ew < 3) ? src[16 * j + i] : 0.0f;
-                r[0][j][i] = __float_as_uint(__uint_as_float(r[0][j][i]) + v);
-              }
-          }
-          par ^= 1;
-          if (ok) {
-#pragma unroll
-            for (int j = 0; j < XG; ++j) {
-              const int c = c0 + 16 * j;
-              uint32_t packed[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float a = fmaxf(fmaf(__uint_as_float(r[0][j][2 * i]), p.alpha, s_bias[c + 2 * i]), lo);
-                const float b2 = fmaxf(fmaf(__uint_as_float(r[0][j][2 * i + 1]), p.alpha, s_bias[c + 2 * i + 1]), lo);
-                const __half2 o = __floats2half2_rn(a, b2);
-                packed[i] = *reinterpret_cast<const uint32_t*>(&o);
-              }
-              const long long eo = obase + map_coloff(p.omap, c);
-              stg256(p.out + eo, packed);
-              if (p.bits_out != nullptr) {
-                p.bits_out[eo >> 4] = relu_bits16(packed);
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(&tempty_bar[as]);
-      }
-    } else {
-      // 16-column chunks handled together (loads in flight); the masked data gradient also holds the mask words
-      constexpr int G = (DACT && SH_CG > 1) ? ((NCG >= 32) ? 2 : 1) : ((NCG >= 64) ? 4 : NCG / 16);
-      for (int i = eset; i < tile_count; i += NSETS) {
-        const int tile = tile_first + i * tile_stride;
-        const int as = i % NACC;
-        const uint32_t aph = (uint32_t)(i / NACC) & 1u;
-        const uint32_t m = (uint32_t)tile * SH_BM + ew * 32 + lane;       // M < 2^31 (checked on the host)
+      for (int hr = 0; hr < 2; ++hr) {
+        const uint32_t m = (uint32_t)tile * SH_BM + r0 + 8 * hr;         // M < 2^31 (checked on the host)
         const uint32_t t2 = p.fwg.div(m);
         const int x = (int)(m - t2 * (uint32_t)p.Wg);
         const int n = (int)p.fhg.div(t2);
         const int y = (int)(t2 - (uint32_t)n * (uint32_t)p.Hg);
         const bool ok = ((long long)m < p.M) && (y < p.vy) && (x < p.vx);
         const long long obase = map_rowbase(p.omap, n, y, x);
-        const long long sbase = p.saved ? map_rowbase(p.smap, n, y, x) : 0;
-        const bool masked = DACT && p.saved != nullptr;
-        // branch-free activation: relu(x) = max(x, 0), identity = max(x, -inf); relu'(h) = (h > 0), 1 = (h > -inf).
-        // (The epilogue is instruction-FETCH bound when its unrolled body outgrows the L0 / L1.5 I-caches, so it is
-        // kept small: no tanh here, no per-element mode switches.)
-        const float lo = (p.act == ACT_RELU) ? 0.0f : -INFINITY;
-        const __half2 lo2 = __floats2half2_rn(lo, lo);
-        mbar_wait(&tfull_bar[as], aph);
-        tc_fence_after();
-        const uint32_t taddr0 = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(as * BN);
-  #pragma unroll 1
-        for (int c0 = cg * NCG; c0 < ((p.debug & 4) ? 0 : (cg + 1) * NCG); c0 += 16 * G) {
-          // activation-derivative mask of this lane's 16-column chunks as 1 bit per element (bit k <-> column c + k):
-          // read as such (saved_bits: 2 B instead of 32 B of HBM traffic per chunk), or derived from the fp16 activation
-          uint32_t mw[G];
-          if (DACT) {
-  #pragma unroll
-            for (int j = 0; j < G; ++j) mw[j] = 0xffffu;
-            if (masked && ok && p.saved_bits != nullptr) {
-  #pragma unroll
-              for (int j = 0; j < G; ++j)
-                mw[j] = __ldg(p.saved_bits + ((sbase + map_coloff(p.smap, c0 + 16 * j)) >> 4));
-            } else if (masked && ok) {
-  #pragma unroll
-              for (int j = 0; j < G; ++j) {
-                uint32_t sv[8];
-                ldg256(p.saved + sbase + map_coloff(p.smap, c0 + 16 * j), sv);
-                uint32_t m = 0;
-  #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&sv[i]));
-                  m |= (h.x > lo ? 1u : 0u) << (2 * i);
-                  m |= (h.y > lo ? 2u : 0u) << (2 * i);
-                }
-                mw[j] = m;
+        const long long sbase = DACT && p.saved ? map_rowbase(p.smap, n, y, x) : 0;
+        const bool masked = DACT && p.saved != nullptr && ok;
+#pragma unroll
+        for (int j = 0; j < BN / 16; ++j) {                  // 16-column chunks: two 8-column accumulator blocks
+          uint32_t mw = 0xffffu;                              // activation-derivative bits of the chunk (DACT)
+          if (masked && p.saved_bits != nullptr) mw = __ldg(p.saved_bits + ((sbase + map_coloff(p.smap, 16 * j)) >> 4));
+          uint32_t bits = 0;
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const int e = 4 * (2 * j + jj) + 2 * hr;
+            const int cc = 8 * jj + 2 * (t & 3);              // column within the chunk
+            const int c = 16 * j + cc;
+            __half2 o;
+            if (DACT) {
+              uint32_t mb = mw >> cc;
+              if (masked && p.saved_bits == nullptr) {
+                const float2 h = __half22float2(*reinterpret_cast<const __half2*>(p.saved + sbase + map_coloff(p.smap, c)));
+                mb = (h.x > lo ? 1u : 0u) | (h.y > lo ? 2u : 0u);
               }
+              o = __floats2half2_rn((mb & 1u) ? acc[e] * p.alpha : 0.0f, (mb & 2u) ? acc[e + 1] * p.alpha : 0.0f);
+            } else {                                          // relu after the rounding: same result, one packed max
+              o = __hmax2(__floats2half2_rn(fmaf(acc[e], p.alpha, s_bias[c]), fmaf(acc[e + 1], p.alpha, s_bias[c + 1])),
+                          lo2);
+              const uint32_t gt = __hgt2_mask(o, zero2);
+              bits |= ((gt & 1u) | ((gt >> 15) & 2u)) << cc;
             }
+            if (ok) *reinterpret_cast<__half2*>(p.out + obase + map_coloff(p.omap, c)) = o;
           }
-          uint32_t r[G][16];
-  #pragma unroll
-          for (int j = 0; j < G; ++j) tmem_ld16(taddr0 + c0 + 16 * j, r[j]);
-          tmem_ld_wait();
-          if (ok) {
-  #pragma unroll
-            for (int j = 0; j < G; ++j) {
-              const int c = c0 + 16 * j;
-              uint32_t packed[8];
-              if (DACT) {
-  #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const float a = (mw[j] & (1u << (2 * i))) ? __uint_as_float(r[j][2 * i]) * p.alpha : 0.0f;
-                  const float b = (mw[j] & (2u << (2 * i))) ? __uint_as_float(r[j][2 * i + 1]) * p.alpha : 0.0f;
-                  const __half2 o = __floats2half2_rn(a, b);
-                  packed[i] = *reinterpret_cast<const uint32_t*>(&o);
-                }
-              } else {
-  #pragma unroll
-                for (int i = 0; i < 8; ++i) {               // relu after the rounding: same result, one packed max
-                  const float a = fmaf(__uint_as_float(r[j][2 * i]), p.alpha, s_bias[c + 2 * i]);
-                  const float b = fmaf(__uint_as_float(r[j][2 * i + 1]), p.alpha, s_bias[c + 2 * i + 1]);
-                  const __half2 o = __hmax2(__floats2half2_rn(a, b), lo2);
-                  packed[i] = *reinterpret_cast<const uint32_t*>(&o);
-                }
-              }
-              const long long eo = obase + map_coloff(p.omap, c);
-              stg256(p.out + eo, packed);
-              if (!DACT && p.bits_out != nullptr) {
-                p.bits_out[eo >> 4] = relu_bits16(packed);
-              }
-            }
+          if (!DACT && p.bits_out != nullptr) {               // the four lanes of a row assemble the chunk's 16 bits
+            bits |= __shfl_xor_sync(0xffffffffu, bits, 1);
+            bits |= __shfl_xor_sync(0xffffffffu, bits, 2);
+            if (ok && (t & 3) == 0) p.bits_out[(obase + map_coloff(p.omap, 16 * j)) >> 4] = (uint16_t)bits;
           }
         }
-        tc_fence_before();
-        mbar_arrive(&tempty_bar[as]);
       }
+      if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
   }
 }
 
@@ -662,85 +440,68 @@ struct ShiftWgradParams {
   float alpha_b;
   long long M;             // reduction rows = B*Hg*Wg
   int N;                   // dY channels
-  int taps;
+  int taps;                // filter rows (kx > 1) or taps (kx == 1)
+  int kx;                  // taps per filter row: tap (a, b) reads X shifted by shift[a] + b
   int shift[SH_MAX_TAPS];  // >= 0
-  float* G;                // [taps*KH*64, N] fp32, row pitch ldg
+  float* G;                // [taps*kx*KH*64, N] fp32, row pitch ldg; row ((a*kx + b)*KH + h)*64 + c
   long long ldg;
   float alpha;
   int kb_total, kb_per_cta;
-  int debug;               // diagnostics (B200RL_CONV_DEBUG): 1 producers move no data, 2 no MMAs, 4 no bias sums
+  // CTA x stores its partial G at ws_g + x*grows*N and its partial bias gradient at ws_b + x*N (summed in x order
+  // afterwards, so the result does not depend on which CTA finishes first)
+  float* ws_g;
+  float* ws_b;
+  long long grows;         // rows of G = taps*kx*KH*64
 };
 
-// KX > 1 ("x-fold", see the forward kernel): the accumulator holds G for one filter row a and all KX taps b of it,
-//   D[(a, h, c), (j, n)] = sum_m' X[m' + a*Wg, h*64 + c] * dY[m' - (KX-1-j), n]         (b = KX - 1 - j)
-// i.e. the MMA's N dimension is KX copies of the dY tile, each starting ONE ROW earlier (descriptor LBO = one row of
-// the tile), so the X slab is fetched once per filter row instead of once per tap.  BN stays the number of dY channels.
-template <int BN, int KH, bool U8, int KX>
-__global__ void __launch_bounds__(SH_THREADS + (U8 ? U8_THREADS : 0), 1)
+// blockIdx.x: a run of k-blocks (reduction rows); blockIdx.y: a group of 2*QW 64-row accumulator chunks
+// q = (tap, h) of G.  Both operands are MN-major: X[rows, 64 channels] (shifted per tap) and dY[rows, N].
+template <int BN, int KH, bool U8>
+__global__ void __launch_bounds__(sh_threads(U8), 1)
 conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmD,
                         const __grid_constant__ ShiftWgradParams p) {
   constexpr int BROWB = (BN >= 64) ? 128 : BN * 2;            // dY row bytes in smem
-  constexpr uint32_t LAYOUT_B = (BROWB == 64) ? 4u : 2u;
-  // reduction rows per pipeline stage ("k-block").  uint8-fed: 128 -- with 64 the single TMA-issuing thread's
-  // wait / expect_tx / issue sequence per stage (~300 clocks, tools/conv_roles.py) was the kernel's floor
-  constexpr int KR = sh_wgrad_krows(U8);
-  constexpr int BROWS = KR + (KX - 1);                        // dY rows per stage (halo of KX - 1 rows in front)
-  constexpr int B_BYTES = BROWS * BROWB;
+  constexpr uint32_t LAYOUT_B = sdesc_layout(BROWB);
+  constexpr int KR = sh_wgrad_krows(U8);                      // reduction rows per pipeline stage ("k-block")
+  constexpr int B_BYTES = KR * BROWB;
   constexpr int B_REGION = (B_BYTES + 1023) & ~1023;
   constexpr int STAGES = (KH == 1) ? 8 : 6;
+  constexpr int QW = sh_wgrad_qw(BN, U8);
   static_assert(!U8 || KH == 1, "the uint8-fed layer has 64 space-to-depth channels");
-  static_assert(STAGES % 2 == 0, "each MMA-issuing warp owns alternate stages");
-  // TMA-fed: stage = [A halves | B], 1024 B aligned.  uint8-fed: [rolling A ring (64-row tiles) | B stages]
+  // TMA-fed: stage = [A halves | B], 1024 B aligned.  uint8-fed: [rolling A ring (KR-row blocks) | B stages]
   using Ring = U8Ring<KR, STAGES>;
   constexpr int A_PITCH = U8 ? KR * 128 : KH * SH_WABYTES + B_REGION;
   constexpr int B_PITCH = U8 ? B_REGION : KH * SH_WABYTES + B_REGION;
   constexpr int B_BASE = U8 ? Ring::BYTES : KH * SH_WABYTES;
   constexpr int SMEM_TILES = U8 ? Ring::BYTES + STAGES * B_REGION : STAGES * (KH * SH_WABYTES + B_REGION);
-  constexpr int NW = KX * BN;                                 // MMA N
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SMEM_TILES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* done_bar = bars + 2 * STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
-  uint64_t* head_bar = bars + 2 * STAGES + 2;                 // U8: first unit of the stage's k-block is in place
+  uint64_t* head_bar = bars + 2 * STAGES;                     // U8: first unit of the stage's k-block is in place
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kb0 = blockIdx.x * p.kb_per_cta;
   const int kb1 = min(kb0 + p.kb_per_cta, p.kb_total);
-  const int nchunks = p.taps * KH;                  // 64-row chunks of the accumulator rows
-  const int n_mt = (nchunks + 1) / 2;               // 128-row accumulator tiles
-  // Two MMA-issuing warps (1 and 3) take the even / odd k-blocks when a second set of accumulators fits in TMEM (see the
-  // forward kernel: the issuing thread stalls on the MMA queue, so one issuer's barrier waits add to its MMAs).  Each
-  // accumulates into its own TMEM columns; the epilogue adds the two.
-  const int acc_cols = n_mt * NW;
-  const bool two = (2 * acc_cols <= 512) && (kb1 - kb0 >= 2);
-  const int nissue = two ? 2 : 1;
+  const int nchunks = p.taps * p.kx * KH;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmX);
-    tma_prefetch_desc(&tmD);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], U8 ? 1 + Ring::UPT : 1);
-      // ring with two issuers: a stage is free when its own k-block AND the one before it (which read this stage's head
-      // rows and belongs to the other issuer) are done
-      mbar_init(&empty_bar[s], (p.gbias ? 2 : 1) + ((U8 && two) ? 1 : 0));
+      mbar_init(&empty_bar[s], SH_CONSUMER_WARPS);   // ring: see the forward kernel
       if (U8) mbar_init(&head_bar[s], 1);
     }
-    mbar_init(done_bar, nissue);
     fence_barrier_init();
-    if (U8 && two) mbar_arrive(&empty_bar[0]);               // stands in for "the k-block before" the CTA's first one
   }
-  if (warp == 2) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == SH_TMA_WARP) {
+    if (elect_one()) {
+      tma_prefetch_desc(&tmX);
+      tma_prefetch_desc(&tmD);
+    }
+    __syncwarp();
     int s = 0;
     uint32_t ph = 0;
     for (int kb = kb0; kb < kb1; ++kb) {
@@ -752,154 +513,118 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
 #pragma unroll
           for (int h = 0; h < KH; ++h) tma_load_2d(sa + h * SH_WABYTES, &tmX, &full_bar[s], h * 64, kb * KR);
         }
-        tma_load_2d(smem + B_BASE + s * B_PITCH, &tmD, &full_bar[s], 0, kb * KR - (KX - 1));   // negative rows: zero fill
+        tma_load_2d(smem + B_BASE + s * B_PITCH, &tmD, &full_bar[s], 0, kb * KR);
       }
       __syncwarp();
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-  } else if (U8 && warp >= 8) {
+  } else if (U8 && warp > SH_TMA_WARP) {
     u8_ring_producer<KR, STAGES, 3>(p.u8, p.M, (long long)kb0 * KR, kb1 - kb0, smem, full_bar, head_bar, empty_bar,
-                                 warp - 8, lane, (p.debug & 1) != 0);
-  } else if (warp == 1 || warp == 3) {
-    constexpr uint32_t IDESC = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(NW >> 3) << 17) |
-                               ((uint32_t)(SH_BM >> 4) << 24);
-    const int iss = warp >> 1;
-    if (iss < nissue) {
-      // Descriptor words relative to the stage base, built once (see the forward kernel): A chunk pair j = accumulator
-      // rows of taps/halves (2j, 2j+1): start = shift of the first, LBO = distance to the second.  B (dY): KX == 1 one
-      // chunk (LBO unused); KX > 1: N-chunk j of the dY operand starts j rows further into the tile.
-      constexpr uint32_t HI_A = (uint32_t)(((1ull << 46) | (2ull << 61) | ((uint64_t)(1024 >> 4) << 32)) >> 32);
-      constexpr uint32_t HI_B = (uint32_t)(((1ull << 46) | ((uint64_t)LAYOUT_B << 61) | ((uint64_t)((8 * BROWB) >> 4) << 32)) >> 32);
-      constexpr uint32_t B_REL = (uint32_t)(((KX == 1 ? KR * BROWB : BROWB) >> 4) & 0x3FFF) << 16;
-      auto a_rel_of = [&](int j) {
-        const int q0 = 2 * j, q1 = 2 * j + 1;
-        const uint32_t st0 = (uint32_t)((q0 % KH) * SH_WABYTES + p.shift[q0 / KH] * 128);
-        uint32_t lbo = 128;
-        if (q1 < nchunks) lbo = (uint32_t)((q1 % KH) * SH_WABYTES + p.shift[q1 / KH] * 128) - st0;
-        return (st0 >> 4) + (((lbo >> 4) & 0x3FFFu) << 16);
-      };
-      const uint32_t a_rel0 = a_rel_of(0), a_rel1 = n_mt > 1 ? a_rel_of(1) : 0u;   // the x-folded layers have n_mt <= 2
-      int s = iss;
-      uint32_t ph = 0;
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(iss * acc_cols);
-      for (int kb = kb0 + iss; kb < kb1; kb += nissue) {
-        const int s1 = (s + 1 == STAGES) ? 0 : s + 1;
-        mbar_wait(&full_bar[s], ph);
-        if (U8) mbar_wait(&head_bar[s1], s1 == 0 ? ph ^ 1 : ph);   // the shifted taps read into the next block's first unit
-        tc_fence_after();
-        if (elect_one()) {
-        const uint32_t a_base = (smem_u32(smem + s * A_PITCH) & 0x3FFFFu) >> 4;
-        const uint32_t b_lo = B_REL + ((smem_u32(smem + B_BASE + s * B_PITCH) & 0x3FFFFu) >> 4);
-        if (!(p.debug & 2)) {
-          const uint32_t accum = (kb > kb0 + iss) ? 1u : 0u;   // the issuer's first k-block overwrites its accumulators
-#pragma unroll 1
-          for (int j = 0; j < n_mt; ++j) {
-            const uint32_t a_lo = a_base + (j == 0 ? a_rel0 : (j == 1 ? a_rel1 : a_rel_of(j)));
-            const uint32_t td = tmem_acc + (uint32_t)(j * NW);
-            umma_f16_lhp(td, a_lo, HI_A, b_lo, HI_B, IDESC, accum);
+                                    warp - (SH_TMA_WARP + 1), lane);
+  } else {
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const int q0 = (int)blockIdx.y * 2 * QW + wg * QW;         // this warpgroup's first accumulator chunk
+    // A descriptor start of chunk q relative to the stage: half h, rows shifted by the tap's shift
+    int a_rel[QW];
 #pragma unroll
-            for (int k = 1; k < KR / 16; ++k)
-              umma_f16_lh<true>(td, a_lo + k * (16 * 128 / 16), HI_A, b_lo + k * (16 * BROWB / 16), HI_B, IDESC);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-        if (U8 && two) umma_commit(&empty_bar[s1]);
-        if (kb + nissue >= kb1) umma_commit(done_bar);
-        }
-        __syncwarp();
-        s += nissue;
-        if (s >= STAGES) { s -= STAGES; ph ^= 1; }
-      }
+    for (int i = 0; i < QW; ++i) {
+      const int q = min(q0 + i, nchunks - 1);
+      const int tap = q / KH, h = q - tap * KH;
+      a_rel[i] = h * SH_WABYTES + (p.shift[tap / p.kx] + tap % p.kx) * 128;
     }
-  } else if (warp >= 4 && warp < 8) {
-    const int ew = warp - 4;
-    // fused bias gradient: column sums of the dY tile while it sits in shared memory (swizzle undone by hand)
-    if (p.gbias != nullptr) {
-      // lanes cover one 64-wide row with 8-byte loads (4 columns per lane); the remaining lanes take other rows
-      constexpr int LPR = BROWB / 8;                           // lanes per row: 16 (128 B rows) or 8 (64 B rows)
-      constexpr int RG = 32 / LPR;                             // row groups handled in parallel
-      const int cq = lane % LPR, rg = lane / LPR;              // column quad, row group
-      const int chunk = (cq * 8) >> 4, within = (cq * 8) & 15;
-      float a[4] = {0.f, 0.f, 0.f, 0.f};
-      // pipeline stage s is always summed by warp s % 4: a warp then sees every fill of its stages in order, so the
-      // parity wait cannot alias (a k-block round-robin would let a warp run a whole phase ahead of a stage)
-      int s = 0;
-      uint32_t ph = 0;
-      for (int kb = kb0; kb < kb1; ++kb, s = (s + 1 == STAGES) ? 0 : s + 1, ph ^= (s == 0)) {
-        if ((s & 3) != ew) continue;
-        mbar_wait(&full_bar[s], ph);
+    // fused bias gradient (first chunk group only): column sums of the dY tile while it sits in shared memory
+    // (swizzle undone by hand); LPR lanes cover one row with 8-byte loads (4 columns per lane)
+    const bool do_bias = p.gbias != nullptr && blockIdx.y == 0;
+    constexpr int LPR = BROWB / 8;
+    constexpr int RG = 32 / LPR;                               // row groups per warp
+    const int cq = lane % LPR, rg = lane / LPR;
+    const int chunk = (cq * 8) >> 4, within = (cq * 8) & 15;
+    float bsum[4] = {0.f, 0.f, 0.f, 0.f};
+    // Each k-block's MMAs start a fresh accumulator (part) that is then added to acc in fp32 registers: a CTA reduces
+    // ~10^4 rows, and one chain of that many tensor-core accumulations loses ~1e-5 relative against an fp32 sum.
+    float acc[QW][BN / 2], part[QW][BN / 2];
+#pragma unroll
+    for (int i = 0; i < QW; ++i)
+#pragma unroll
+      for (int e = 0; e < BN / 2; ++e) acc[i][e] = 0.0f;
+    int s = 0;
+    uint32_t ph = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      const int s1 = (s + 1 == STAGES) ? 0 : s + 1;
+      mbar_wait(&full_bar[s], ph);
+      if (U8) mbar_wait(&head_bar[s1], s1 == 0 ? ph ^ 1 : ph);   // the shifted taps read into the next block's first unit
+      const uint32_t a_base = smem_u32(smem + s * A_PITCH);
+      const uint32_t b_base = smem_u32(smem + B_BASE + s * B_PITCH);
+      wgmma_fence();
+#pragma unroll
+      for (int i = 0; i < QW; ++i) {
+        // chunks past the last one repeat it (a_rel is clamped) and are dropped by the epilogue: a wgmma under a
+        // thread-dependent branch would make the compiler serialise every wgmma of the kernel
+#pragma unroll
+        for (int k = 0; k < KR / 16; ++k) {
+          const uint64_t adesc = make_sdesc(a_base + a_rel[i] + k * 16 * 128, 8 * 1024, 1024, 1);
+          const uint64_t bdesc = make_sdesc(b_base + k * 16 * BROWB, 8 * 8 * BROWB, 8 * BROWB, LAYOUT_B);
+          wgmma_f16<BN, 1, 1>(part[i], adesc, bdesc, k > 0 ? 1u : 0u);
+        }
+      }
+      wgmma_commit();
+      if (do_bias) {
         const uint8_t* sb = smem + B_BASE + s * B_PITCH;
-#pragma unroll 8
-        for (int r = rg + (KX - 1); r < ((p.debug & 4) ? 0 : KR + (KX - 1)); r += RG) {   // the halo rows belong to the previous block
+#pragma unroll 4
+        for (int r = warp * RG + rg; r < KR; r += SH_CONSUMER_WARPS * RG) {
           const int sw = (BROWB == 128) ? (r & 7) : ((r >> 1) & 3);
           const uint2 w = *reinterpret_cast<const uint2*>(sb + r * BROWB + ((chunk ^ sw) << 4) + within);
-          a[0] += __half2float(__ushort_as_half((unsigned short)(w.x & 0xffffu)));
-          a[1] += __half2float(__ushort_as_half((unsigned short)(w.x >> 16)));
-          a[2] += __half2float(__ushort_as_half((unsigned short)(w.y & 0xffffu)));
-          a[3] += __half2float(__ushort_as_half((unsigned short)(w.y >> 16)));
+          bsum[0] += __half2float(__ushort_as_half((unsigned short)(w.x & 0xffffu)));
+          bsum[1] += __half2float(__ushort_as_half((unsigned short)(w.x >> 16)));
+          bsum[2] += __half2float(__ushort_as_half((unsigned short)(w.y & 0xffffu)));
+          bsum[3] += __half2float(__ushort_as_half((unsigned short)(w.y >> 16)));
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[s]);
       }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+      for (int i = 0; i < QW; ++i)
+#pragma unroll
+        for (int e = 0; e < BN / 2; ++e) acc[i][e] += part[i][e];
+      s = s1;
+      if (s == 0) ph ^= 1;
+    }
+    if (do_bias) {
+      __shared__ float s_bsum[SH_CONSUMER_WARPS][64];
 #pragma unroll
       for (int o = LPR; o < 32; o <<= 1)                       // fold the row groups together
 #pragma unroll
-        for (int i = 0; i < 4; ++i) a[i] += __shfl_xor_sync(0xffffffffu, a[i], o);
-      if (rg == 0 && kb1 > kb0) {
+        for (int i = 0; i < 4; ++i) bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], o);
+      if (rg == 0) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-          if (4 * cq + i < p.N) atomicAdd(p.gbias + 4 * cq + i, a[i] * p.alpha_b);
+        for (int i = 0; i < 4; ++i) s_bsum[warp][4 * cq + i] = bsum[i];
+      }
+      asm volatile("bar.sync 1, %0;" ::"n"(SH_CONSUMER_WARPS * 32) : "memory");   // consumer warps only
+      if ((int)threadIdx.x < p.N) {
+        float b = 0.0f;
+#pragma unroll
+        for (int w = 0; w < SH_CONSUMER_WARPS; ++w) b += s_bsum[w][threadIdx.x];
+        p.ws_b[(long long)blockIdx.x * p.N + threadIdx.x] = b * p.alpha_b;
       }
     }
     if (kb1 > kb0) {
-      mbar_wait(done_bar, 0);
-      tc_fence_after();
-      const int mrows = nchunks * 64;
-      for (int j = 0; j < n_mt; ++j) {
-        const int row = j * 128 + ew * 32 + lane;               // accumulator row = (a, h, c): chunk q = row / 64
-        // G row of accumulator row (q, c) and N-chunk jb: tap (a, b = KX-1-jb) -> ((a*KX + b)*KH + h)*64 + c
-        const int q = row >> 6, cc = row & 63;
-        const int ta = q / KH, th = q - ta * KH;
-#pragma unroll 1
-        for (int c = 0; c < NW; c += 16) {
-          uint32_t r[16];
-          tmem_ld16(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(j * NW + c), r);
-          if (two) {
-            uint32_t r2[16];
-            tmem_ld16(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc_cols + j * NW + c), r2);
-            tmem_ld_wait();
 #pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r2[i]));
-          }
-          tmem_ld_wait();
-          const int jb = c / BN, cn = c - jb * BN;
-          if (row < mrows && cn < p.N) {
-            const long long grow = (long long)((ta * KX + (KX - 1 - jb)) * KH + th) * 64 + cc;
-            float* out = p.G + grow * p.ldg + cn;
+      for (int i = 0; i < QW; ++i) {
+        if (q0 + i < nchunks) {
 #pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (cn + i < p.N) atomicAdd(out + i, __uint_as_float(r[i]) * p.alpha);
+          for (int e = 0; e < BN / 2; ++e) {
+            const int cn = acc_col(t, e);
+            const long long grow = (long long)(q0 + i) * 64 + acc_row(t, e);
+            if (cn < p.N) p.ws_g[((long long)blockIdx.x * p.grows + grow) * p.N + cn] = acc[i][e] * p.alpha;
           }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ host
-// Role-isolation diagnostics for tools/conv_roles.py: results are garbage when the mask is non-zero.  Read per call
-// (getenv is ~100 ns) so one process can time every mask.
-static int conv_debug_mask() {
-  const char* e = getenv("B200RL_CONV_DEBUG");
-  return e ? atoi(e) : 0;
-}
-
 static U8Src make_u8src(const void* x, const long long* idx, int H, int W, int C, int s) {
   U8Src u{};
   u.x = reinterpret_cast<const uint8_t*>(x);
@@ -914,13 +639,13 @@ static U8Src make_u8src(const void* x, const long long* idx, int H, int W, int C
   return u;
 }
 
-template <int BN, int KH, bool DACT, bool U8 = false, int KX = 1>
+template <int BN, int KH, bool DACT, bool U8 = false>
 static int launch_fwd(const CUtensorMap& tmX, const CUtensorMap& tmW, const ShiftParams& p, cudaStream_t st) {
   constexpr int STAGES = sh_stages(KH);
   constexpr int SMEM = (U8 ? U8Ring<SH_BM, STAGES>::BYTES : STAGES * KH * sh_arows(KH) * 128) + sh_wres_bytes(KH) + 1024 + 256;
-  static_assert(SMEM + 4096 <= 227 * 1024, "conv_shift_fwd: shared memory budget (+ static bias / exchange arrays)");
+  static_assert(SMEM + 1024 <= 227 * 1024, "conv_shift_fwd: shared memory budget (+ static bias array)");
   static bool attr = false;
-  auto kern = conv_shift_fwd_kernel<BN, KH, DACT, U8, KX>;
+  auto kern = conv_shift_fwd_kernel<BN, KH, DACT, U8>;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     if (e != cudaSuccess) {
@@ -930,22 +655,22 @@ static int launch_fwd(const CUtensorMap& tmX, const CUtensorMap& tmW, const Shif
     attr = true;
   }
   const int grid = p.num_tiles < device_num_sms() ? p.num_tiles : device_num_sms();
-  kern<<<grid, sh_fwd_threads(U8), SMEM, st>>>(tmX, tmW, p);
+  kern<<<grid, sh_threads(U8), SMEM, st>>>(tmX, tmW, p);
   return check_launch("conv_shift_fwd_kernel");
 }
 
-template <int BN, int KH, bool U8 = false, int KX = 1>
-static int launch_wgrad(const CUtensorMap& tmX, const CUtensorMap& tmD, const ShiftWgradParams& p, int grid,
+template <int BN, int KH, bool U8 = false>
+static int launch_wgrad(const CUtensorMap& tmX, const CUtensorMap& tmD, const ShiftWgradParams& p, dim3 grid,
                         cudaStream_t st) {
   constexpr int STAGES = (KH == 1) ? 8 : 6;
   constexpr int KR = sh_wgrad_krows(U8);
   constexpr int BROWB = (BN >= 64) ? 128 : BN * 2;
-  constexpr int B_REGION = ((KR + KX - 1) * BROWB + 1023) & ~1023;
+  constexpr int B_REGION = (KR * BROWB + 1023) & ~1023;
   constexpr int SMEM =
       (U8 ? U8Ring<KR, STAGES>::BYTES + STAGES * B_REGION : STAGES * (KH * SH_WABYTES + B_REGION)) + 1024 + 512;
   static_assert(SMEM <= 227 * 1024, "conv_shift_wgrad: shared memory budget");
   static bool attr = false;
-  auto kern = conv_shift_wgrad_kernel<BN, KH, U8, KX>;
+  auto kern = conv_shift_wgrad_kernel<BN, KH, U8>;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
     if (e != cudaSuccess) {
@@ -954,7 +679,7 @@ static int launch_wgrad(const CUtensorMap& tmX, const CUtensorMap& tmD, const Sh
     }
     attr = true;
   }
-  kern<<<grid, SH_THREADS + (U8 ? U8_THREADS : 0), SMEM, st>>>(tmX, tmD, p);
+  kern<<<grid, sh_threads(U8), SMEM, st>>>(tmX, tmD, p);
   return check_launch("conv_shift_wgrad_kernel");
 }
 
@@ -992,9 +717,10 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
   ShiftParams p = {};
   int lo = shifts[0], hi = shifts[0];
   for (int t = 1; t < taps; ++t) { lo = shifts[t] < lo ? shifts[t] : lo; hi = shifts[t] > hi ? shifts[t] : hi; }
-  B200RL_REQUIRE(hi - lo <= sh_arows(C / 64) - SH_BM, "conv_shift_fwd: shift span %d too large for C = %d", hi - lo, C);
+  B200RL_REQUIRE(hi - lo + kx - 1 <= sh_arows(C / 64) - SH_BM, "conv_shift_fwd: shift span %d too large for C = %d",
+                 hi - lo + kx - 1, C);
   B200RL_REQUIRE(B * Hg * Wg < (1LL << 31) - 4096, "conv_shift_fwd: too many rows");
-  p.M = B * Hg * Wg; p.Hg = Hg; p.Wg = Wg; p.N = N; p.taps = taps; p.min_shift = lo;
+  p.M = B * Hg * Wg; p.Hg = Hg; p.Wg = Wg; p.N = N; p.taps = taps; p.kx = kx; p.min_shift = lo;
   for (int t = 0; t < taps; ++t) p.shift[t] = shifts[t] - lo;
   p.vy = vy; p.vx = vx; p.out = reinterpret_cast<__half*>(out);
   B200RL_REQUIRE(fill_map(p.omap, omap), "conv_shift_fwd: output map needs power-of-two Cq >= 16 and s");
@@ -1004,17 +730,15 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
   if (smap) B200RL_REQUIRE(fill_map(p.smap, smap), "conv_shift_fwd: saved map needs power-of-two Cq >= 16 and s");
   B200RL_REQUIRE(!(saved && !smap), "conv_shift_fwd: saved needs smap");
   if (saved_bits && !saved) p.saved = reinterpret_cast<const __half*>(saved_bits);   // non-null marker: masking is on
-  // the epilogue moves 16 fp16 columns per lane with one 256-bit access
+  // the epilogue stores column pairs as 4-byte words and writes the activation bits per 16-column chunk
   B200RL_REQUIRE(((omap[1] | omap[2] | omap[3]) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 31) == 0,
                  "conv_shift_fwd: output strides must be multiples of 16 elements, base 32-byte aligned");
   if (saved)
     B200RL_REQUIRE(((smap[1] | smap[2] | smap[3]) & 15) == 0 && (reinterpret_cast<uintptr_t>(saved) & 31) == 0,
                    "conv_shift_fwd: saved strides must be multiples of 16 elements, base 32-byte aligned");
   p.bias = bias; p.act = act; p.dact = dact; p.alpha = alpha;
-  p.tstep = SH_BM - (kx - 1);
-  p.num_tiles = (int)((p.M + p.tstep - 1) / p.tstep);
+  p.num_tiles = (int)((p.M + SH_BM - 1) / SH_BM);
   p.u8 = make_u8src(u8_x, u8_idx, u8_H, u8_W, u8_C, u8_s);
-  p.debug = conv_debug_mask();
   B200RL_REQUIRE(Hg >= 2 && Wg >= 2, "conv_shift_fwd: grid must be at least 2x2");
   p.fwg = make_fastdiv((uint32_t)Wg);
   p.fhg = make_fastdiv((uint32_t)Hg);
@@ -1029,14 +753,6 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
   }
   if ((rc = make_tmap_2d_f16(&tmX, X, p.M, C, C, 64, sh_arows(C / 64))) != 0) return rc;
   const int KH = C / 64;
-  if (kx > 1) {
-    if (kx == 2 && N == 32 && KH == 1) return launch_fwd<64, 1, false, false, 2>(tmX, tmW, p, stream);
-    if (kx == 2 && N == 64 && KH == 2) return launch_fwd<128, 2, false, false, 2>(tmX, tmW, p, stream);
-    if (kx == 2 && N == 64 && KH == 1) return launch_fwd<128, 1, false, false, 2>(tmX, tmW, p, stream);
-    if (kx == 3 && N == 64 && KH == 1) return launch_fwd<192, 1, false, false, 3>(tmX, tmW, p, stream);
-    set_last_error("conv_shift_fwd: no x-folded kernel for kx=%d N=%d C=%d", kx, N, C);
-    return B200RL_ERR_UNSUPPORTED;
-  }
 #define SHIFT_FWD_CASE(bn)                                                                                    \
   if (N == bn) {                                                                                              \
     if (dact) return KH == 1 ? launch_fwd<bn, 1, true>(tmX, tmW, p, stream) : launch_fwd<bn, 2, true>(tmX, tmW, p, stream); \
@@ -1065,15 +781,13 @@ int conv_shift_wgrad_impl(const void* X, long long rows, int C, const void* dY, 
   B200RL_REQUIRE(N == 32 || N == 64, "conv_shift_wgrad: N must be 32 or 64 (got %d)", N);
   B200RL_REQUIRE(taps >= 1 && taps <= SH_MAX_TAPS, "conv_shift_wgrad: 1..%d taps", SH_MAX_TAPS);
   const int KH = C / 64;
-  const int n_mt = (taps * KH + 1) / 2;
-  B200RL_REQUIRE(n_mt * kx * N <= 512, "conv_shift_wgrad: accumulators exceed TMEM");
   ShiftWgradParams p = {};
   for (int t = 0; t < taps; ++t) {
-    B200RL_REQUIRE(shifts[t] >= 0 && shifts[t] <= SH_WROWS_K - 64, "conv_shift_wgrad: shift %d out of range", shifts[t]);
+    B200RL_REQUIRE(shifts[t] >= 0 && shifts[t] + kx - 1 <= SH_WROWS_K - 64, "conv_shift_wgrad: shift %d out of range",
+                   shifts[t]);
     p.shift[t] = shifts[t];
-    if (t > 0 && KH == 1) B200RL_REQUIRE(shifts[t] > shifts[t - 1], "conv_shift_wgrad: shifts must increase");
   }
-  p.M = rows; p.N = N; p.taps = taps; p.G = G; p.ldg = ldg; p.alpha = alpha;
+  p.M = rows; p.N = N; p.taps = taps; p.kx = kx; p.G = G; p.ldg = ldg; p.alpha = alpha;
   p.gbias = gbias; p.alpha_b = alpha_b;
   const int KR = sh_wgrad_krows(u8_x != nullptr);
   p.kb_total = (int)((rows + KR - 1) / KR);
@@ -1081,28 +795,28 @@ int conv_shift_wgrad_impl(const void* X, long long rows, int C, const void* dY, 
   if (max_ctas > 0 && max_ctas < ctas) ctas = max_ctas;
   if (ctas > p.kb_total) ctas = p.kb_total;
   p.kb_per_cta = (p.kb_total + ctas - 1) / ctas;
-  const int grid = (p.kb_total + p.kb_per_cta - 1) / p.kb_per_cta;
+  const int qw = sh_wgrad_qw(N, u8_x != nullptr);
+  const dim3 grid((p.kb_total + p.kb_per_cta - 1) / p.kb_per_cta, (taps * kx * KH + 2 * qw - 1) / (2 * qw));
   p.u8 = make_u8src(u8_x, u8_idx, u8_H, u8_W, u8_C, u8_s);
-  p.debug = conv_debug_mask();
+  p.grows = (long long)taps * kx * KH * 64;
+  const size_t g_floats = (size_t)grid.x * p.grows * N;
+  float* ws = det_workspace(g_floats + (size_t)grid.x * N, stream);
+  if (!ws) return B200RL_ERR_CUDA;
+  p.ws_g = ws;
+  p.ws_b = ws + g_floats;
   CUtensorMap tmX, tmD;
   int rc;
-  if ((rc = make_tmap_2d_f16(&tmD, dY, rows, N, N, N < 64 ? N : 64, KR + kx - 1)) != 0) return rc;
+  if ((rc = make_tmap_2d_f16(&tmD, dY, rows, N, N, N < 64 ? N : 64, KR)) != 0) return rc;
   if (u8_x) {
-    if (kx == 2) return launch_wgrad<32, 1, true, 2>(tmD, tmD, p, grid, stream);
-    B200RL_REQUIRE(kx == 1, "conv_shift_wgrad: the uint8-fed first layer supports kx = 1 or 2");
-    return launch_wgrad<32, 1, true>(tmD, tmD, p, grid, stream);
+    rc = launch_wgrad<32, 1, true>(tmD, tmD, p, grid, stream);
+  } else {
+    if ((rc = make_tmap_2d_f16(&tmX, X, rows, C, C, 64, SH_WROWS_K)) != 0) return rc;
+    if (N == 32) rc = KH == 1 ? launch_wgrad<32, 1>(tmX, tmD, p, grid, stream) : launch_wgrad<32, 2>(tmX, tmD, p, grid, stream);
+    else rc = KH == 1 ? launch_wgrad<64, 1>(tmX, tmD, p, grid, stream) : launch_wgrad<64, 2>(tmX, tmD, p, grid, stream);
   }
-  if ((rc = make_tmap_2d_f16(&tmX, X, rows, C, C, 64, SH_WROWS_K)) != 0) return rc;
-  if (kx > 1) {
-    if (kx == 2 && N == 32 && KH == 1) return launch_wgrad<32, 1, false, 2>(tmX, tmD, p, grid, stream);
-    if (kx == 2 && N == 64 && KH == 2) return launch_wgrad<64, 2, false, 2>(tmX, tmD, p, grid, stream);
-    if (kx == 2 && N == 64 && KH == 1) return launch_wgrad<64, 1, false, 2>(tmX, tmD, p, grid, stream);
-    if (kx == 3 && N == 64 && KH == 1) return launch_wgrad<64, 1, false, 3>(tmX, tmD, p, grid, stream);
-    set_last_error("conv_shift_wgrad: no x-folded kernel for kx=%d N=%d C=%d", kx, N, C);
-    return B200RL_ERR_UNSUPPORTED;
-  }
-  if (N == 32) return KH == 1 ? launch_wgrad<32, 1>(tmX, tmD, p, grid, stream) : launch_wgrad<32, 2>(tmX, tmD, p, grid, stream);
-  return KH == 1 ? launch_wgrad<64, 1>(tmX, tmD, p, grid, stream) : launch_wgrad<64, 2>(tmX, tmD, p, grid, stream);
+  if (rc == B200RL_OK) rc = sum_partials(p.ws_g, (int)grid.x, p.grows, N, G, ldg, stream);
+  if (rc == B200RL_OK && gbias) rc = sum_partials(p.ws_b, (int)grid.x, 1, N, gbias, N, stream);
+  return rc;
 }
 
 }  // namespace b200rl

@@ -76,7 +76,7 @@ int obs_encode_impl(const float* x, const long long* src_idx, long long B, int r
                     reinterpret_cast<__half*>(out)};
   const long long total = B * (in_pad / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 16LL * device_num_sms()) blocks = 16LL * device_num_sms();
   obs_encode_kernel<<<(int)blocks, 256, 0, stream>>>(p);
   return check_launch("obs_encode_kernel");
 }

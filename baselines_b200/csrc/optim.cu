@@ -1,4 +1,4 @@
-// Flat-buffer optimiser kernels (all HBM-bound; float4 accesses, grid = multiple of 148 SMs).
+// Flat-buffer optimiser kernels (all HBM-bound; float4 accesses, grid = multiple of the SM count).
 //   sumsq            : sum of squares of the flat gradient -> device double (tf.clip_by_global_norm,
 //                      ppo2/model.py:105-107), or per-tensor norms (tf.clip_by_norm, deepq/build_graph.py:416-421)
 //   clip_adam        : g *= clip/max(||g||, clip) fused with TF-Adam exactly as pinned by the reference's
@@ -11,9 +11,14 @@
 
 namespace b200rl {
 
+static constexpr int SUMSQ_MAX_BLOCKS = 1024;
+__device__ double g_sumsq_part[SUMSQ_MAX_BLOCKS];
+__device__ unsigned int g_sumsq_done = 0;
+
 __global__ void __launch_bounds__(256)
 sumsq_kernel(const float* __restrict__ g, long long n, double* __restrict__ out) {
   __shared__ double red[8];
+  __shared__ bool last;
   double acc = 0.0;
   const long long n4 = n >> 2;
   const float4* g4 = reinterpret_cast<const float4*>(g);
@@ -31,13 +36,24 @@ sumsq_kernel(const float* __restrict__ g, long long n, double* __restrict__ out)
   if (threadIdx.x == 0) {
     double s = 0.0;
     for (int w = 0; w < 8; ++w) s += red[w];
-    atomicAdd(out, s);
+    // the last block to finish adds the blocks' sums in block order: the norm is the same on every run
+    g_sumsq_part[blockIdx.x] = s;
+    __threadfence();
+    last = (atomicAdd(&g_sumsq_done, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (last && threadIdx.x == 0) {
+    __threadfence();
+    double t = 0.0;
+    for (int b = 0; b < (int)gridDim.x; ++b) t += *((volatile double*)&g_sumsq_part[b]);
+    *out = t;
+    g_sumsq_done = 0;
   }
 }
 
-// segment s covers [seg_off[s], seg_off[s+1]); one block per (segment, slice)
+// segment s covers [seg_off[s], seg_off[s+1]); block (s, y) stores its slice's sum at part[s * gridDim.y + y]
 __global__ void __launch_bounds__(256)
-seg_sumsq_kernel(const float* __restrict__ g, const long long* __restrict__ seg_off, double* __restrict__ out) {
+seg_sumsq_kernel(const float* __restrict__ g, const long long* __restrict__ seg_off, double* __restrict__ part) {
   __shared__ double red[8];
   const int s = blockIdx.x;
   const long long a = seg_off[s], b = seg_off[s + 1];
@@ -52,7 +68,17 @@ seg_sumsq_kernel(const float* __restrict__ g, const long long* __restrict__ seg_
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int w = 0; w < 8; ++w) t += red[w];
-    atomicAdd(out + s, t);
+    part[s * gridDim.y + blockIdx.y] = t;
+  }
+}
+
+// out[s] = sum of the segment's gridDim.y slice sums, in slice order
+__global__ void seg_sumsq_finish_kernel(const double* __restrict__ part, int nseg, int slices, double* __restrict__ out) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < nseg) {
+    double t = 0.0;
+    for (int k = 0; k < slices; ++k) t += part[(long long)s * slices + k];
+    out[s] = t;
   }
 }
 
@@ -204,7 +230,7 @@ dgrad_weights_kernel(const float* __restrict__ w, __half* __restrict__ out, int 
 
 static int grid_for(long long n, int threads, int per_sm) {
   long long blocks = (n + threads - 1) / threads;
-  const long long cap = 148LL * per_sm;
+  const long long cap = (long long)device_num_sms() * per_sm;
   return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
 }
 
@@ -212,14 +238,19 @@ int sumsq_impl(const float* g, long long n, double* out, cudaStream_t stream) {
   B200RL_REQUIRE(g && out && n > 0, "sumsq: bad args");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "sumsq: gradient buffer must be 16 B aligned");
   cudaMemsetAsync(out, 0, sizeof(double), stream);
-  sumsq_kernel<<<grid_for(n / 4 + 1, 256, 4), 256, 0, stream>>>(g, n, out);
+  const int grid = grid_for(n / 4 + 1, 256, 4);
+  B200RL_REQUIRE(grid <= SUMSQ_MAX_BLOCKS, "sumsq: %d blocks exceed the partial-sum slots", grid);
+  sumsq_kernel<<<grid, 256, 0, stream>>>(g, n, out);
   return check_launch("sumsq_kernel");
 }
 
 int seg_sumsq_impl(const float* g, const long long* seg_off, int nseg, double* out, cudaStream_t stream) {
   B200RL_REQUIRE(g && seg_off && out && nseg > 0, "seg_sumsq: bad args");
-  cudaMemsetAsync(out, 0, sizeof(double) * nseg, stream);
-  seg_sumsq_kernel<<<dim3(nseg, 16), 256, 0, stream>>>(g, seg_off, out);
+  constexpr int SLICES = 16;
+  double* part = reinterpret_cast<double*>(det_workspace((size_t)nseg * SLICES * 2, stream));
+  if (!part) return B200RL_ERR_CUDA;
+  seg_sumsq_kernel<<<dim3(nseg, SLICES), 256, 0, stream>>>(g, seg_off, part);
+  seg_sumsq_finish_kernel<<<ceil_div(nseg, 128), 128, 0, stream>>>(part, nseg, SLICES, out);
   return check_launch("seg_sumsq_kernel");
 }
 

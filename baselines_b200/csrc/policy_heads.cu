@@ -293,12 +293,13 @@ __global__ void __launch_bounds__(256)
 gauss_loss_kernel(const float* __restrict__ mean, long long ld, const float* __restrict__ logstd, int d,
                   const float* __restrict__ vpred, long long ldv, const float* __restrict__ actions, PpoCommon pc,
                   __half* __restrict__ dmean, long long ld_dm, __half* __restrict__ dv, long long ld_dv,
-                  float* __restrict__ dlogstd, float inv_M, long long B) {
-  extern __shared__ float s_dls[];                   // [d] block partial of dL/dlogstd, then [d] std, [d] logstd
-  float* s_std = s_dls + d;
-  float* s_ls = s_dls + 2 * d;
+                  float* __restrict__ dls_part, float inv_M, long long B) {
+  // [8 warps][d] per-warp partials of dL/dlogstd, then [d] std, [d] logstd; dls_part[block, j] gets the block's sum
+  extern __shared__ float s_dls[];
+  float* s_std = s_dls + 8 * d;
+  float* s_ls = s_dls + 9 * d;
+  for (int j = threadIdx.x; j < 8 * d; j += blockDim.x) s_dls[j] = 0.0f;
   for (int j = threadIdx.x; j < d; j += blockDim.x) {
-    s_dls[j] = 0.0f;
     const float ls = logstd[j];
     s_ls[j] = ls;
     s_std[j] = expf(ls);
@@ -348,8 +349,8 @@ gauss_loss_kernel(const float* __restrict__ mean, long long ld, const float* __r
 #pragma unroll
     for (int j = 0; j < TN; ++j) t[j] = 0.0f;
   }
-  // every lane takes part in the warp reductions of dL/dlogstd (inactive rows contribute 0): one shared-memory
-  // atomic per warp and action dimension instead of one per sample
+  // every lane takes part in the warp reductions of dL/dlogstd (inactive rows contribute 0); each warp adds into its own
+  // shared-memory slot, so the block's sum has a fixed order
   const bool vec = ((ld_dm & 7) == 0) && ((reinterpret_cast<uintptr_t>(dmean) & 15) == 0) && (((d + 7) & ~7) <= ld_dm);
   auto chunk8 = [&](int j0, const float* t8) {       // t8: this sample's 8 standardised residuals (null: recompute)
     __align__(16) __half g8[8];
@@ -366,7 +367,7 @@ gauss_loss_kernel(const float* __restrict__ mean, long long ld, const float* __r
       g8[jj] = __float2half_rn(gm);
       if (j < d) {                                   // uniform across the warp
         gl = warp_sum(gl);
-        if ((threadIdx.x & 31) == 0) atomicAdd(&s_dls[j], gl);
+        if ((threadIdx.x & 31) == 0) s_dls[(threadIdx.x >> 5) * d + j] += gl;
       }
     }
     if (b < B) {
@@ -386,7 +387,11 @@ gauss_loss_kernel(const float* __restrict__ mean, long long ld, const float* __r
   }
   if (b < B) dv[b * ld_dv] = __float2half_rn(g_v);   // after dmean: with a fused [pi | vf] head dv is column d of the same row
   __syncthreads();
-  for (int j = threadIdx.x; j < d; j += blockDim.x) atomicAdd(dlogstd + j, s_dls[j] * inv_M);
+  for (int j = threadIdx.x; j < d; j += blockDim.x) {
+    float t = 0.0f;
+    for (int w = 0; w < 8; ++w) t += s_dls[w * d + j];
+    dls_part[(long long)blockIdx.x * d + j] = t * inv_M;
+  }
   block_accumulate5(st, pc.stats);
 }
 
@@ -443,20 +448,23 @@ int gauss_loss_impl(const float* mean, long long ld, const float* logstd, int d,
                  "gauss_loss: bad args");
   PpoCommon pc{src_idx, returns, old_values, old_neglogp, adv_stats, cliprange, ent_coef, vf_coef, stats, cliprange_dev};
   const int grid = (int)ceil_div_ll(B, 256);
-  const size_t sm = 3 * (size_t)d * sizeof(float);
+  const size_t sm = 10 * (size_t)d * sizeof(float);
+  float* part = det_workspace((size_t)grid * d, stream);
+  if (!part) return B200RL_ERR_CUDA;
   if (d <= 8)
     gauss_loss_kernel<8><<<grid, 256, sm, stream>>>(mean, ld, logstd, d, vpred, ldv, actions, pc,
                                                     reinterpret_cast<__half*>(dmean), ld_dm,
-                                                    reinterpret_cast<__half*>(dv), ld_dv, dlogstd, inv_M, B);
+                                                    reinterpret_cast<__half*>(dv), ld_dv, part, inv_M, B);
   else if (d <= 24)
     gauss_loss_kernel<24><<<grid, 256, sm, stream>>>(mean, ld, logstd, d, vpred, ldv, actions, pc,
                                                      reinterpret_cast<__half*>(dmean), ld_dm,
-                                                     reinterpret_cast<__half*>(dv), ld_dv, dlogstd, inv_M, B);
+                                                     reinterpret_cast<__half*>(dv), ld_dv, part, inv_M, B);
   else
     gauss_loss_kernel<0><<<grid, 256, sm, stream>>>(mean, ld, logstd, d, vpred, ldv, actions, pc,
                                                     reinterpret_cast<__half*>(dmean), ld_dm,
-                                                    reinterpret_cast<__half*>(dv), ld_dv, dlogstd, inv_M, B);
-  return check_launch("gauss_loss_kernel");
+                                                    reinterpret_cast<__half*>(dv), ld_dv, part, inv_M, B);
+  const int rc = check_launch("gauss_loss_kernel");
+  return rc == B200RL_OK ? sum_partials(part, grid, 1, d, dlogstd, d, stream) : rc;
 }
 
 }  // namespace b200rl

@@ -1,22 +1,31 @@
-// Device helpers shared by the tcgen05 GEMM / convolution kernels.
+// Device helpers shared by the wgmma GEMM / convolution kernels.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace b200rl {
 
 enum : int { MODE_F16_ACT = 0, MODE_F32_STORE = 1, MODE_F32_ATOMIC = 2, MODE_F16_DACT = 3, MODE_F16_SHUFFLE = 4 };
 enum : int { ACT_NONE = 0, ACT_RELU = 1, ACT_TANH = 2 };
 
-// smem matrix descriptor; layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
+// wgmma shared-memory matrix descriptor; layout: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B.
+// The swizzle is a function of the shared-memory address, so a descriptor may start at any 16-byte column of any row.
+__host__ __device__ constexpr uint32_t sdesc_layout(int row_bytes) {
+  return row_bytes == 128 ? 1u : row_bytes == 64 ? 2u : 3u;
+}
 __device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)layout << 61;
+  d |= (uint64_t)layout << 62;
   return d;
 }
+
+// Register position of accumulator element e (0 .. N/2-1) of a m64nN wgmma tile for thread t of the warpgroup:
+// row = 16*(t/32) + (t%32)/4 + 8*((e/2)%2), column = 8*(e/4) + 2*(t%4) + e%2.
+__device__ __forceinline__ int acc_row(int t, int e) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((e >> 1) & 1); }
+__device__ __forceinline__ int acc_col(int t, int e) { return 8 * (e >> 2) + 2 * (t & 3) + (e & 1); }
 
 __device__ __forceinline__ void tma_load_im2col_4d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c, int w,
                                                    int h, int n, uint16_t off_w, uint16_t off_h) {
@@ -38,56 +47,8 @@ __device__ __forceinline__ float act_grad_from_saved(float h, int act) {
   return 1.0f;
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.256): one full 32-byte sector per lane and half the LSU instructions
-// of two 128-bit accesses.  The address must be 32-byte aligned.
-__device__ __forceinline__ void ldg256(const void* p, uint32_t (&w)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
-               : "l"(p));
-}
-__device__ __forceinline__ void stg256(void* p, const uint32_t (&w)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-               : "memory");
-}
-
-// v[16] *= act'(saved[0..16)); vec: one 32-byte load (sv 32-byte aligned)
-__device__ __forceinline__ void mask16(float (&v)[16], const __half* sv, bool vec, int nvalid, int act) {
-  if (vec) {
-    uint32_t w[8];
-    ldg256(sv, w);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-      v[2 * i] *= act_grad_from_saved(f.x, act);
-      v[2 * i + 1] *= act_grad_from_saved(f.y, act);
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (i < nvalid) v[i] *= act_grad_from_saved(__half2float(sv[i]), act);
-  }
-}
-__device__ __forceinline__ void store16_f16(const float (&v)[16], __half* out, bool vec, int nvalid) {
-  if (vec) {
-    uint32_t w[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const __half2 h = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-      w[i] = *reinterpret_cast<const uint32_t*>(&h);
-    }
-    stg256(out, w);
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (i < nvalid) out[i] = __float2half_rn(v[i]);
-  }
-}
-
-
-// host helpers implemented in gemm_tcgen05.cu
+// host helpers implemented in gemm_wgmma.cu
 int make_tmap_2d_f16(CUtensorMap* tm, const void* ptr, long long rows, long long cols, long long ld, int box_cols,
                      int box_rows);
-int device_num_sms();
 
 }  // namespace b200rl

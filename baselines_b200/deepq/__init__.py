@@ -1,4 +1,4 @@
-"""B200-native DQN learner: same public surface as baselines/deepq/__init__.py:1-4."""
+"""H100-native DQN learner: same public surface as baselines/deepq/__init__.py:1-4."""
 from .replay_buffer import ReplayBuffer, PrioritizedReplayBuffer  # noqa: F401
 from .build_graph import build_train, build_act  # noqa: F401
 from .deepq import learn, load_act, ActWrapper  # noqa: F401

@@ -1,4 +1,4 @@
-"""DQN act / train / update_target on B200 kernels.
+"""DQN act / train / update_target on the H100 kernels.
 
 Behavioural mirror of baselines/deepq/build_graph.py (build_act :146-199, build_train :317-449) and
 baselines/deepq/models.py (build_q_func :5-45): the same (act, train, update_target, debug) callables, built on a

@@ -1,4 +1,4 @@
-"""deepq.learn on B200 kernels -- same signature, schedules, bookkeeping and return type as the reference's
+"""deepq.learn on the H100 kernels -- same signature, schedules, bookkeeping and return type as the reference's
 baselines/deepq/deepq.py:95-332 (learn) and :23-92 (ActWrapper / load_act).
 
 The act -> env.step -> replay.add -> sample -> train -> update_priorities -> update_target loop (deepq.py:259-307) is

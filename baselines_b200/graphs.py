@@ -9,6 +9,7 @@ between replays (Adam step size, clip range, sampler stream position, minibatch 
 
 B200RL_NO_GRAPHS=1 disables replay (every call runs eagerly) -- used by tests to check both paths agree.
 """
+import gc
 import os
 
 import torch
@@ -42,6 +43,10 @@ class GraphCache:
                 return
             g = torch.cuda.CUDAGraph()
             before = _lib.LAUNCHES
+            # torch.cuda.graph collects garbage before the capture begins; a collection DURING the capture could free a
+            # pinned host buffer of a dead object, whose release makes a CUDA call that invalidates the capture
+            gc_on = gc.isenabled()
+            gc.disable()
             try:
                 with torch.cuda.graph(g):
                     fn()
@@ -56,6 +61,9 @@ class GraphCache:
                 _lib.LAUNCHES = before
                 fn()
                 return
+            finally:
+                if gc_on:
+                    gc.enable()
             ent = self.graphs[key] = (g, _lib.LAUNCHES - before)
             _lib.LAUNCHES = before                               # nothing ran during capture
         ent[0].replay()

@@ -186,7 +186,7 @@ class Linear:
         bn = 256 if (self.N > 128 and self.N % 256 == 0) else (128 if self.N > 64 else 64)   # gemm_f16_impl's N tile
         tiles = -(-self.K // 128) * -(-self.N // bn)
         kb = -(-M // 64)
-        split = max(1, min(kb // 2 if kb >= 2 else 1, -(-296 // tiles)))
+        split = max(1, min(kb // 2 if kb >= 2 else 1, -(-2 * ops.num_sms() // tiles)))
         ops.gemm(x, dz, self.gw, M=self.K, N=self.N, K=M, lda=ldx, ldb=lddz, ldc=self.N, mn_major=True,
                  mode=ops.MODE_F32_ATOMIC, alpha=alpha * self.in_scale, split_k=split, tag="wgrad." + self.name)
         if self.split_in:                                  # + lo^T dz
@@ -209,7 +209,7 @@ class Linear:
 
 
 class Conv(Linear):
-    """NHWC convolution lowered to im2col + tcgen05 GEMM (a2c/utils.py:37-56)."""
+    """NHWC convolution lowered to im2col + wgmma GEMM (a2c/utils.py:37-56)."""
 
     def __init__(self, store, name, H, W, C, nf, rf, stride, act, w_init, same_pad=False, in_scale=1.0,
                  tf_w=None, tf_b=None, b_shape=None, allow_s2d=False):
@@ -300,7 +300,7 @@ class Conv(Linear):
         H, W, C, R, S, sh, sw, pt, pl = self.geom
         tiles = -(-self.K // 128)
         rows = B * self.P
-        split = max(1, min((rows // 64) // 2 if rows >= 128 else 1, -(-296 // tiles)))
+        split = max(1, min((rows // 64) // 2 if rows >= 128 else 1, -(-2 * ops.num_sms() // tiles)))
         ops.conv_gemm(x, B, H, W, C, R, S, sh, sw, pt, pl, self.OH, self.OW, dz, self.nf, self.gw, self.nf, self.nf, 1,
                       ops.MODE_F32_ATOMIC, alpha=alpha * self.in_scale, split_k=split, tag="wgrad." + self.name)
         ops.colsum(dz, self.gb, rows, self.nf, self.nf, alpha=alpha)
@@ -450,9 +450,8 @@ class Tower:
         cap, cv = self.cap, self.convs
         self.sg = []                                   # per layer: dict(Hg, Wg, Cg, k, shifts, s)
         import os
-        # the x-fold pays off in the weight-gradient kernels (-14 ms per cfg-2 update) but not in the forward ones, which
-        # are bound by warp-instruction issue and get 3 extra instructions per output element from the cross-lane sum
-        # (measured +17 ms): forward fold only on request
+        # x-fold: the kx horizontally adjacent taps of a filter row share one weight row block (conv_shift.cu walks them
+        # as taps shifted by one more grid row each); forward fold only on request
         xfold = os.environ.get("B200RL_NO_XFOLD", "0") != "1"
         xfold_fwd = os.environ.get("B200RL_XFOLD_FWD", "0") == "1"
         for c in cv:

@@ -1,6 +1,6 @@
 """Torch-tensor front end of the C-ABI: tensors only supply device pointers and the current stream.
 
-Every function launches hand-written sm_100a kernels from libb200rl.so; nothing here computes with
+Every function launches hand-written sm_90a kernels from libb200rl.so; nothing here computes with
 torch ops (torch is plumbing: allocation, streams, torch.distributed).
 """
 import torch
@@ -18,6 +18,17 @@ def _ptr(t):
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
+
+
+_SMS = {}
+
+
+def num_sms():
+    """Streaming multiprocessors of the current device (132 on an H100 SXM); split-K factors aim at two CTAs per SM."""
+    d = torch.cuda.current_device()
+    if d not in _SMS:
+        _SMS[d] = torch.cuda.get_device_properties(d).multi_processor_count
+    return _SMS[d]
 
 
 def _chk(t, dtype, name):

@@ -1,4 +1,4 @@
-"""PPO2 learner object on B200 kernels -- drop-in for the reference's baselines/ppo2/model.py Model.
+"""PPO2 learner object on the H100 kernels -- drop-in for the reference's baselines/ppo2/model.py Model.
 
 Same constructor keywords (model.py:27-28) and the same duck-typed protocol the reference's Runner / learn /
 run.py consume (SURVEY.md 8b): step, value, train, initial_state, loss_names, save, load.  Added device
@@ -22,7 +22,7 @@ class Model(object):
                  train_chunk=None):
         if not torch.cuda.is_available():
             raise RuntimeError("baselines_b200.ppo2.Model needs a CUDA device: the learner hot path is "
-                               "hand-written sm_100a CUDA and has no CPU fallback")
+                               "hand-written sm_90a CUDA and has no CPU fallback")
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.ent_coef, self.vf_coef, self.max_grad_norm = float(ent_coef), float(vf_coef), max_grad_norm
         self.nbatch_act, self.nbatch_train, self.nsteps = nbatch_act, nbatch_train, nsteps

@@ -97,7 +97,8 @@ class ClockSampler:
 
 
 def load_peaks():
-    peaks = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback"}
+    # H100 SXM data sheet (700 W card): dense fp16 / bf16 tensor rate and HBM3 bandwidth; never reached in practice
+    peaks = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "src": "H100 SXM data sheet"}
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peaks.update(json.load(open(pk)))
@@ -255,6 +256,22 @@ def run_reference(args, cfg):
     print(json.dumps(out), flush=True)
 
 
+# ---------------------------------------------------------------------------------------------- output dump
+DUMP_MAX_ELEMS = 1 << 20          # larger arrays: a fixed, seeded sample of this many elements (flat order)
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy: floating point as float32, integers as float64 (exact)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+        a = a.astype(np.float64 if a.dtype.kind in "iub" else np.float32)
+        if a.size > DUMP_MAX_ELEMS:
+            pick = np.sort(np.random.RandomState(0).randint(0, a.size, DUMP_MAX_ELEMS))   # O(sample), not O(size)
+            a = a.reshape(-1)[pick]
+        np.save(os.path.join(out_dir, name.replace("/", "_") + ".npy"), a)
+
+
 # ---------------------------------------------------------------------------------------------- rooflines
 def summarize_profile(prof, steps):
     """prof: {label: [ms, calls, flops, bytes]} accumulated over the timed region."""
@@ -269,26 +286,7 @@ def summarize_profile(prof, steps):
     return out
 
 
-# bench label -> kernel template instance (conv_shift.cu dispatch for the NatureCNN layers): <BN,KH,DACT,U8,KX> for the
-# forward / dgrad kernel, <BN,KH,U8,KX> for the wgrad kernel
-TRAFFIC_KERNEL = {
-    "convs.fwd.pi/c1": "conv_shift_fwd_kernel<32, 1, 0, 1, 1>", "convs.fwd.pi/c2": "conv_shift_fwd_kernel<64, 2, 0, 0, 1>",
-    "convs.fwd.pi/c3": "conv_shift_fwd_kernel<64, 1, 0, 0, 1>", "convs.dgrad.pi/c3": "conv_shift_fwd_kernel<64, 1, 1, 0, 1>",
-    "convs.dgrad.pi/c2": "conv_shift_fwd_kernel<128, 1, 1, 0, 1>", "convs.wgrad.pi/c1": "conv_shift_wgrad_kernel<32, 1, 1, 2>",
-    "convs.wgrad.pi/c2": "conv_shift_wgrad_kernel<64, 2, 0, 2>", "convs.wgrad.pi/c3": "conv_shift_wgrad_kernel<64, 1, 0, 3>",
-}
-
-
-def load_traffic():
-    """DRAM bytes per SAMPLE of each conv kernel instance from the committed `ncu --set full` capture
-    (profiles/r2_traffic.json, written by `tools/summarize_ncu.py traffic <rep> ... <samples>` from the .ncu-rep raw
-    page: dram__bytes_read.sum + dram__bytes_write.sum of one launch / the samples that launch processed).  bench
-    multiplies by the samples one of ITS launches processes; every launch here and in the capture is >> L2."""
-    tj = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    return json.load(open(tj)) if os.path.exists(tj) else {}
-
-
-def kernel_roofline(name, k, peaks, traffic=None):
+def kernel_roofline(name, k, peaks):
     n_launch = max(1.0, k["launches_per_step"])
     f_tensor = f_hbm = 0.0
     if k.get("flops_per_step"):
@@ -297,16 +295,11 @@ def kernel_roofline(name, k, peaks, traffic=None):
         f_hbm = k["bytes_per_step"] / (k["ms_per_step"] / 1e3) / 1e9 / peaks["hbm_gbs"]
     if f_tensor >= f_hbm:
         r = {"kernel": name, "bound": "tensor", "achieved": f_tensor * peaks["bf16_tflops_sustained"],
-             "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s", "frac": f_tensor,
-             "peak_src": peaks["src"] + " (sustained cuBLAS bf16: kernel timed inside a long step)"}
+             "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s", "frac": f_tensor, "peak_src": peaks["src"]}
     else:
         r = {"kernel": name, "bound": "hbm", "achieved": f_hbm * peaks["hbm_gbs"], "peak": peaks["hbm_gbs"],
-             "unit": "GB/s", "frac": f_hbm, "peak_src": peaks["src"] + " (copy bandwidth)"}
-    t = (traffic or {}).get(TRAFFIC_KERNEL.get(name.split("@")[0], ""))
-    samples = k.get("samples_per_launch")
-    r.update({"traffic": t["dram_bytes_per_sample"] * samples if t and samples else None,
-              "traffic_src": (t.get("src") + f", {t['capture_samples']} samples/launch, scaled per sample") if t else None,
-              "algorithmic_bytes_per_launch": k.get("bytes_per_step", 0.0) / n_launch,
+             "unit": "GB/s", "frac": f_hbm, "peak_src": peaks["src"]}
+    r.update({"algorithmic_bytes_per_launch": k.get("bytes_per_step", 0.0) / n_launch,
               "algorithmic_flops_per_launch": k.get("flops_per_step", 0.0) / n_launch,
               "flops_are": "useful (valid conv outputs only)", "frac_tensor": f_tensor, "frac_hbm": f_hbm,
               "ms_per_launch": k["ms_per_step"] / n_launch, "launches_per_step": n_launch, "share_of_step": k.get("share")})
@@ -340,10 +333,13 @@ def run_ppo2(cfg, args, steps, warmup, with_profile, with_e2e, dist_ctx):
                       train_chunk=cfg["train_chunk"])
         return model, Runner(env=env, model=model, nsteps=T, gamma=cfg["gamma"], lam=cfg["lam"])
 
+    last = {}
+
     def update(model, runner):
         ro, _ = runner.run_device()
         st = run_epochs(model, ro, cfg["lr"], cfg["cliprange"], nbatch, nbatch_train, cfg["noptepochs"], dev,
                         shuffle=args.shuffle)
+        last.update(ro=ro, st=st)
         return torch.stack(st).mean(dim=0)
 
     def timed(model, runner, steps, warmup, read_back, profile=False):
@@ -379,6 +375,12 @@ def run_ppo2(cfg, args, steps, warmup, with_profile, with_e2e, dist_ctx):
         sampler.start()
     ms_step, launches = timed(model, runner, steps, warmup, read_back=False)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        ro = last["ro"]
+        out = {"loss_stats": torch.stack(last["st"])}
+        out.update({k: getattr(ro, k) for k in ("actions", "values", "neglogpacs", "advs", "returns")})
+        out.update({"param." + k: v for k, v in model.get_params().items()})
+        dump_outputs(args.dump_outputs, out)
     prof = None
     ms_prof = None
     if with_profile:
@@ -464,10 +466,13 @@ def run_deepq(cfg, args, steps, warmup, with_profile, with_e2e, dist_ctx):
     rb._set_priorities(torch.arange(n_fill, device=dev), pr)
     torch.cuda.synchronize()
 
+    last = {}
+
     def step():
         idx, w32, _ = rb.sample_device(B, beta=cfg["beta"])
         td = model.train_device(rb._obs_t, rb._obs_tp1, rb._actions, rb._rewards, rb._dones, w32, idx, B)
         rb.update_priorities_device(idx, td, 1e-6)
+        last.update(idx=idx, weights=w32, td_error=td)
 
     def timed(fn, steps, warmup, profile=False):
         for _ in range(warmup):
@@ -489,6 +494,10 @@ def run_deepq(cfg, args, steps, warmup, with_profile, with_e2e, dist_ctx):
         sampler.start()
     ms_step, launches = timed(step, steps, warmup)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        out = {k: v[:B] for k, v in last.items()}
+        out.update({"param." + k: v for k, v in model.q.store.export_tf("params").items()})
+        dump_outputs(args.dump_outputs, out)
     prof = None
     if with_profile:
         timed(step, 20, 0, profile=True)
@@ -546,6 +555,8 @@ def main():
     ap.add_argument("--no-profile", action="store_true", help="skip the per-kernel CUDA-event profile pass")
     ap.add_argument("--no-targets", action="store_true", help="skip the stand-alone GAE / fc1 / PER microbenchmarks")
     ap.add_argument("--no-others", action="store_true", help="default config only: skip the short cfg3 / cfg4 measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     cfg = dict(CFGS[args.config])
     if args.nenvs and cfg["kind"] == "ppo2":
@@ -582,7 +593,8 @@ def main():
             oc = dict(CFGS[key])
             try:
                 fn = run_deepq if oc["kind"] == "deepq" else run_ppo2
-                r = fn(oc, args, oc["steps"], oc["warmup"], True, True, ctx)
+                r = fn(oc, argparse.Namespace(**{**vars(args), "dump_outputs": None}), oc["steps"], oc["warmup"], True,
+                       True, ctx)
                 m, u = metric_of(oc)
                 others[key] = {"metric": m, "unit": u, "workload": oc["name"], "value": r["value"],
                                "ms_per_step": r["ms_step"], "steps": oc["steps"], "warmup": oc["warmup"],
@@ -598,7 +610,6 @@ def main():
         return
 
     peaks = load_peaks()
-    traffic = load_traffic()
     kernels = _kernels_of(res)
     roofline, roofline_all = None, []
     if kernels and cfg["kind"] == "ppo2":
@@ -609,7 +620,7 @@ def main():
     if kernels:
         for name, k in sorted(kernels.items(), key=lambda kv: -kv[1]["ms_per_step"]):
             if k.get("flops_per_step") or k.get("bytes_per_step"):
-                roofline_all.append(kernel_roofline(name, k, peaks, traffic))
+                roofline_all.append(kernel_roofline(name, k, peaks))
         if roofline_all:
             roofline = roofline_all[0]
 
@@ -645,7 +656,6 @@ def main():
                                                f"variant {gcase['variant']})", "bound": "hbm", "achieved": gcase["gbs"],
                                      "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gcase["gbs"] / peaks["hbm_gbs"],
                                      "ms_per_launch": gcase["ms"], "algorithmic_bytes_per_launch": gcase["bytes"],
-                                     "traffic": (traffic.get(f"gae_scan_{gcase['T']}x{gcase['N']}") or {}).get("dram_bytes_per_launch"),
                                      "stand_alone": True, "target": 0.6})
         for c in mb.get("fc1") or []:
             if isinstance(c, dict) and "tflops" in c:

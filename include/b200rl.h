@@ -1,4 +1,4 @@
-/* libb200rl -- C-ABI of the B200-native PPO2 / DQN learner hot path.
+/* libb200rl -- C-ABI of the H100-native (sm_90a) PPO2 / DQN learner hot path.
  *
  * The reference (openai/baselines) has NO FFI: its hot path is TF1 graph ops + numpy loops called from
  * Python.  Each entry point below therefore names the reference interface (file:line) whose arithmetic it
@@ -27,7 +27,7 @@ extern "C" {
 /* GEMM epilogues */
 #define B200RL_MODE_F16_ACT 0    /* C16 = act(alpha*acc + bias)                      (forward)            */
 #define B200RL_MODE_F32_STORE 1  /* C32 = alpha*acc + bias                           (heads)              */
-#define B200RL_MODE_F32_ATOMIC 2 /* C32 += alpha*acc (red.add.f32; split-K capable)  (weight gradients)   */
+#define B200RL_MODE_F32_ATOMIC 2 /* C32 += alpha*acc (split-K parts added in order) (weight gradients)   */
 #define B200RL_MODE_F16_DACT 3   /* C16 = alpha*acc * act'(saved)                    (data gradients)     */
 #define B200RL_MODE_F16_SHUFFLE 4 /* conv data gradient, pixel-shuffle scatter: row (n,i,j), col (py,px,c)
                                      -> dx[n, s*i+py, s*j+px, c] * act'(saved there)  (b200rl_conv_gemm only) */
@@ -45,7 +45,7 @@ int b200rl_gae_scan(const float* rewards, const float* values, const uint8_t* do
                     const uint8_t* last_dones, float* advs, float* returns, int T, int N, double gamma, double lam,
                     int variant, void* stream);
 
-/* fp16 x fp16 -> fp32 tcgen05 GEMM: tf.matmul a2c/utils.py:63; after im2col also tf.nn.conv2d a2c/utils.py:56
+/* fp16 x fp16 -> fp32 wgmma GEMM: tf.matmul a2c/utils.py:63; after im2col also tf.nn.conv2d a2c/utils.py:56
  * and their gradients (ppo2/model.py:102).
  *   mn_major = 0 : A[M,K] (lda), B[N,K] (ldb), C = A * B^T
  *   mn_major = 1 : A[K,M] (lda), B[K,N] (ldb), C = A^T * B   (reduction over rows; use split_k > 1)

@@ -721,8 +721,8 @@ def test_gemm_column_remap(ops):
 @pytest.mark.parametrize("B,gather", [(3, False), (37, True), (700, True), (4000, True)])
 def test_conv_shift_fused_uint8_source(ops, B, gather):
     """First conv layer straight from uint8 frames: the producer warps' gather + cast + space-to-depth tile must
-    give the same forward (bit-exact: same fp16 operands, same MMA order) and the same wgrad (split-K float
-    atomics -> tolerance) as s2d_gather followed by the fp16 TMA path."""
+    give the same forward (bit-exact: same fp16 operands, same MMA order) and the same wgrad (different
+    reduction blocking -> tolerance) as s2d_gather followed by the fp16 TMA path."""
     torch.manual_seed(B)
     H = W = 84
     C, s, Hg, Wg, N = 4, 4, 21, 21, 32
@@ -941,3 +941,38 @@ def test_shuffle_indices_is_a_keyed_permutation(ops, n, T, N):
     out3 = torch.empty(n, dtype=torch.int64, device="cuda")
     ops.shuffle_indices(out3, n, 0x1234567890ABCDEF, T, N)
     assert torch.equal(out1, out3)                                         # reproducible given the key
+
+
+def test_weight_gradient_reductions_repeat_bit_for_bit(ops):
+    """Cross-CTA reductions (split-K GEMM weight gradient, shift-conv weight and bias gradients, bias column sums,
+    gradient sum of squares) add their per-CTA parts in a fixed order: the same inputs give the same bits on every
+    call, so a training run repeats exactly."""
+    torch.manual_seed(7)
+    Kred, M, N = 20000, 576, 64
+    A = (torch.randn(Kred, M, device="cuda") * 0.5).half()
+    B = (torch.randn(Kred, N, device="cuda") * 0.5).half()
+    B_, Hg, Wg, Nc = 64, 21, 21, 32
+    x16 = (torch.randn(B_ * Hg * Wg, 64, device="cuda")).half()
+    dz = torch.zeros(B_, Hg, Wg, Nc, dtype=torch.float16, device="cuda")
+    dz[:, :20, :20] = (torch.randn(B_, 20, 20, Nc, device="cuda") * 0.5).half()
+    g = torch.randn(1 << 20, device="cuda")
+
+    def run():
+        C = torch.zeros(M, N, device="cuda")
+        ops.gemm(A, B, C, M=M, N=N, K=Kred, lda=M, ldb=N, ldc=N, mn_major=True, mode=ops.MODE_F32_ATOMIC,
+                 alpha=0.25, split_k=16)
+        G = torch.zeros(256, Nc, device="cuda")
+        gb = torch.zeros(Nc, device="cuda")
+        ops.conv_shift_wgrad(x16, B_ * Hg * Wg, 64, dz, Nc, [0, 1, Wg, Wg + 1], G, Nc, alpha=1.0 / 255, gbias=gb)
+        db = torch.zeros(N, device="cuda")
+        ops.colsum(B, db, Kred, N, N)
+        ss = torch.zeros(1, dtype=torch.float64, device="cuda")
+        ops.sumsq(g, ss)
+        torch.cuda.synchronize()
+        return C, G, gb, db, ss
+
+    first = run()
+    assert float(first[0].abs().max()) > 0 and float(first[1].abs().max()) > 0
+    for _ in range(3):
+        for a, b in zip(first, run()):
+            assert torch.equal(a, b)

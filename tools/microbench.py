@@ -3,7 +3,7 @@
 launching stream, >=3 warm-ups, and an L2 flush (write of a 512 MB buffer) between timed iterations.
 
     python tools/microbench.py            # prints one JSON object
-Used by bench.py (extra `targets` key) and under ncu for profiles/ (tools/microbench.py --only gae|fc1)."""
+Used by bench.py (extra `targets` key); `tools/microbench.py --only gae|fc1` runs one case."""
 import argparse
 import json
 import os
@@ -179,11 +179,11 @@ def dqn_case(flush, batch=512):
 
 
 def run(only=None, quick=False):
-    flush = torch.empty(128 * 1024 * 1024, dtype=torch.float32, device="cuda")      # 512 MB > 126 MB L2
+    flush = torch.empty(128 * 1024 * 1024, dtype=torch.float32, device="cuda")      # 512 MB > 50 MB L2
     out = {"l2_flush": "512 MB write between iterations"}
     Ms = [8192, 131072] if not quick else [131072]
     cases = [
-        # cfg-2 size (L2-resident), cfg-3 size (142 MB ~ L2), and 4x L2 (570 MB: a DRAM steady-state measurement)
+        # cfg-2 size (L2-resident), cfg-3 size (142 MB, ~3x L2), and 570 MB (~11x L2: a DRAM steady-state measurement)
         ("gae", "gae", lambda: [gae_case(128, 4096, -1, flush), gae_case(512, 16384, 1, flush),
                                 gae_case(512, 16384, 0, flush), gae_case(2048, 16384, 1, flush)]),
         ("fc1", "fc1", lambda: [fc1_case(M, k, flush) for M in Ms for k in ("fwd", "dgrad", "wgrad")]),
