@@ -8,6 +8,8 @@ import numpy as np
 import pytest
 import torch
 
+import _refs
+
 pytestmark = pytest.mark.gpu
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
@@ -17,6 +19,15 @@ GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
 def ops():
     from baselines_b200 import ops as _ops
     return _ops
+
+
+@pytest.fixture(autouse=True)
+def _fp32_references_without_tf32():
+    """fp32 references are true fp32: TF32 is off for torch matmuls and cudnn convolutions."""
+    old = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    yield
+    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
 
 
 def dev(x, dtype=None):
@@ -509,19 +520,8 @@ def test_dqn_td_vs_oracle(ops):
 
 # ------------------------------------------------------------------------------------------ implicit-GEMM conv
 def _patches(x, R, S, sh, sw, ph, pw, OH, OW):
-    """x [B,H,W,C] float -> [B*OH*OW, R*S*C] with K ordered (r, s, c); zero padding (ph, pw) on the low side and
-    whatever is needed on the high side."""
-    import torch.nn.functional as F
-    B, H, W, C = x.shape
-    hi_h = max((OH - 1) * sh + R - ph - H, 0)
-    hi_w = max((OW - 1) * sw + S - pw - W, 0)
-    xp = F.pad(x.permute(0, 3, 1, 2), (pw, hi_w, ph, hi_h))
-    un = F.unfold(xp, (R, S), stride=(sh, sw))                        # [B, C*R*S, L]
-    L = un.shape[-1]
-    oh_full = (xp.shape[2] - R) // sh + 1
-    ow_full = (xp.shape[3] - S) // sw + 1
-    un = un.view(B, C, R, S, oh_full, ow_full)[:, :, :, :, :OH, :OW]
-    return un.permute(0, 4, 5, 2, 3, 1).reshape(B * OH * OW, R * S * C)
+    """float64 patch matrix [B*OH*OW, R*S*C] of x [B,H,W,C], K ordered (r, s, c) (tests/_refs.py)."""
+    return _refs.patches(x.double(), R, S, sh, sw, ph, pw, OH, OW)
 
 
 CONV_CASES = [
@@ -546,7 +546,7 @@ def test_conv_gemm_forward_and_wgrad(ops, name, B, H, W, C, R, S, sh, sw, N):
     ops.conv_gemm(x, B, H, W, C, R, S, sh, sw, 0, 0, OH, OW, wt, K, out, N, N, 0, ops.MODE_F16_ACT, act=ops.ACT_RELU,
                   bias=bias)
     torch.cuda.synchronize()
-    want = torch.relu(P @ wt.float().t() + bias)
+    want = torch.relu(P @ wt.double().t() + bias.double()).float()
     err = float((out.float() - want).abs().max())
     assert torch.allclose(out.float(), want, atol=2e-2, rtol=5e-3), (name, err)
     # wgrad: gw[K, N] += alpha * patches^T dz
@@ -555,7 +555,7 @@ def test_conv_gemm_forward_and_wgrad(ops, name, B, H, W, C, R, S, sh, sw, N):
     ops.conv_gemm(x, B, H, W, C, R, S, sh, sw, 0, 0, OH, OW, dz, N, gw, N, N, 1, ops.MODE_F32_ATOMIC, alpha=0.5,
                   split_k=3)
     torch.cuda.synchronize()
-    want = 1.0 + 0.5 * (P.t() @ dz.float())
+    want = (1.0 + 0.5 * (P.t() @ dz.double())).float()
     err = float((gw - want).abs().max())
     assert torch.allclose(gw, want, atol=2e-3 * rows ** 0.5, rtol=2e-3), (name, err)
 
@@ -563,8 +563,7 @@ def test_conv_gemm_forward_and_wgrad(ops, name, B, H, W, C, R, S, sh, sw, N):
 @pytest.mark.parametrize("B,Hin,Cin,Cout,rf,s", [(7, 20, 32, 64, 4, 2), (11, 9, 64, 64, 3, 1), (3, 84, 16, 32, 8, 4)])
 def test_conv_gemm_dgrad_pixel_shuffle(ops, B, Hin, Cin, Cout, rf, s):
     """dx = conv_transpose(dz, W) * relu'(h_in), computed as ONE implicit GEMM over dz with the rearranged
-    weights and the pixel-shuffle epilogue; reference = autograd of F.conv2d."""
-    import torch.nn.functional as F
+    weights and the pixel-shuffle epilogue; reference = the float64 transposed convolution of tests/_refs.py."""
     torch.manual_seed(Hin + Cin)
     OHc = (Hin - rf) // s + 1                                 # conv output size
     w = (torch.randn(rf, rf, Cin, Cout, device="cuda") * 0.2)
@@ -579,10 +578,7 @@ def test_conv_gemm_dgrad_pixel_shuffle(ops, B, Hin, Cin, Cout, rf, s):
     ops.conv_gemm(dz, B, OHc, OHc, Cout, An, An, 1, 1, An - 1, An - 1, G, G, wdg, ldw, dx, 0, s * s * Cin, 0,
                   ops.MODE_F16_SHUFFLE, act=ops.ACT_RELU, saved=h_in, shuffle=(Hin, Hin, Cin, s))
     torch.cuda.synchronize()
-    xin = torch.zeros(B, Cin, Hin, Hin, device="cuda", requires_grad=True)
-    y = F.conv2d(xin, w.half().float().permute(3, 2, 0, 1), stride=s)
-    y.backward(dz.float().permute(0, 3, 1, 2))
-    want = xin.grad.permute(0, 2, 3, 1) * (h_in.float() > 0)
+    want = (_refs.conv2d_dgrad(dz, w.half(), Hin, Hin, (s, s), (0, 0)) * (h_in.double() > 0)).float()
     err = float((dx.float() - want).abs().max())
     assert torch.allclose(dx.float(), want, atol=3e-2, rtol=5e-3), err
 
@@ -609,7 +605,7 @@ def test_conv_shift_forward_wgrad_dgrad(ops, name, B, Hg, Wg, C, R, N):
     omap = (0, OH * OW * N, OW * N, N, 0, 0)
     ops.conv_shift_fwd(x, B, Hg, Wg, C, wt, K, N, shifts, OH, OW, out, omap, bias=bias, act=ops.ACT_RELU)
     torch.cuda.synchronize()
-    want = torch.relu(P @ wt.float().t() + bias).view(B, OH, OW, N)
+    want = torch.relu(P @ wt.double().t() + bias.double()).float().view(B, OH, OW, N)
     err = float((out.float() - want).abs().max())
     assert torch.allclose(out.float(), want, atol=3e-2, rtol=5e-3), (name, "fwd", err)
     # ---- wgrad: dY lives on the INPUT grid, zero outside the valid OHxOW window
@@ -622,7 +618,7 @@ def test_conv_shift_forward_wgrad_dgrad(ops, name, B, Hg, Wg, C, R, N):
     torch.cuda.synchronize()
     want_gb = 1.0 + 0.25 * dzv.float().reshape(-1, N).sum(0)           # fused bias gradient
     assert torch.allclose(gb, want_gb, atol=1e-2, rtol=1e-3), (name, "gbias", float((gb - want_gb).abs().max()))
-    wantG = 1.0 + 0.5 * (P.t() @ dzv.float().reshape(-1, N))
+    wantG = (1.0 + 0.5 * (P.t() @ dzv.double().reshape(-1, N))).float()
     err = float((G - wantG).abs().max())
     assert torch.allclose(G, wantG, atol=3e-3 * (B * OH * OW) ** 0.5, rtol=3e-3), (name, "wgrad", err)
     # ---- dgrad: dX[m] = sum_t dY[m - sh_t] W_t, W_t = [C rows (c_in), N cols (c_out)] = rows t*C.. of W_hwio[K, N]
@@ -676,7 +672,7 @@ def test_conv_shift_address_maps(ops):
     x = (torch.randn(B, Hg, Wg, C, device="cuda") * 0.5).half()
     wt = (torch.randn(N, 4 * C, device="cuda") * 0.1).half()
     P = _patches(x.float(), 2, 2, 1, 1, 0, 0, 20, 20)
-    want = (P @ wt.float().t()).view(B, 20, 20, N)
+    want = (P @ wt.double().t()).float().view(B, 20, 20, N)
     h1 = torch.zeros(B, 10, 10, 4 * N, dtype=torch.float16, device="cuda")
     ops.conv_shift_fwd(x, B, Hg, Wg, C, wt, 4 * C, N, shifts, 20, 20, h1, (2, 100 * 4 * N, 10 * 4 * N, 4 * N, N, 2))
     torch.cuda.synchronize()
@@ -822,7 +818,7 @@ def test_conv_shift_xfold_forward_and_wgrad(ops, name, B, Hg, Wg, C, R, N):
             t = a * R + b
             wf[b * N:(b + 1) * N, a * C:(a + 1) * C] = wt[:, t * C:(t + 1) * C]
     P = _patches(x.float(), R, R, 1, 1, 0, 0, OH, OW)
-    want = torch.relu(P @ wt.float().t() + bias).view(B, OH, OW, N)
+    want = torch.relu(P @ wt.double().t() + bias.double()).float().view(B, OH, OW, N)
     omap = (0, OH * OW * N, OW * N, N, 0, 0)
     out_f = torch.full((B, OH, OW, N), 7.0, dtype=torch.float16, device="cuda")
     bits_f = torch.zeros(B * OH * OW * N // 16, dtype=torch.int16, device="cuda")
@@ -848,7 +844,7 @@ def test_conv_shift_xfold_forward_and_wgrad(ops, name, B, Hg, Wg, C, R, N):
     torch.cuda.synchronize()
     want_gb = 1.0 + 0.25 * dzv.float().reshape(-1, N).sum(0)
     assert torch.allclose(gb, want_gb, atol=2e-2, rtol=1e-3), (name, "fold gbias", float((gb - want_gb).abs().max()))
-    wantG = 1.0 + 0.5 * (P.t() @ dzv.float().reshape(-1, N))
+    wantG = (1.0 + 0.5 * (P.t() @ dzv.double().reshape(-1, N))).float()
     err = float((G - wantG).abs().max())
     assert torch.allclose(G, wantG, atol=3e-3 * (B * OH * OW) ** 0.5, rtol=3e-3), (name, "fold wgrad", err)
 

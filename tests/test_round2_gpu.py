@@ -18,6 +18,15 @@ pytestmark = pytest.mark.gpu
 from test_ppo2_gpu import CASES, _mk, _obs      # noqa: E402  (shared builders)
 
 
+@pytest.fixture(autouse=True)
+def _fp32_references_without_tf32():
+    """fp32 references are true fp32: TF32 is off for torch matmuls and cudnn convolutions (cudnn's default is TF32)."""
+    old = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    yield
+    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = old
+
+
 # ----------------------------------------------------------------------------------------------- bench-shaped update
 def test_bench_shaped_multichunk_multiminibatch_update_matches_oracle():
     """The benchmarked path in miniature but with its structure intact: NatureCNN, 16 384 samples (32 steps x 512
@@ -79,7 +88,8 @@ def test_bench_shaped_multichunk_multiminibatch_update_matches_oracle():
 def test_conv_stack_large_batch_vs_fp32_torch(B):
     """conv_shift forward / wgrad / dgrad + the fc1 GEMMs at B = 8192 images (28 224 conv1 tiles: >= 190 tiles per
     persistent CTA, far beyond the handful the small-B kernel tests reach) against fp32 torch conv2d + autograd on the
-    GPU, using the weights exactly as the kernels see them (fp16-rounded)."""
+    GPU (TF32 off), using the weights exactly as the kernels see them (fp16-rounded)."""
+    assert not torch.backends.cudnn.allow_tf32 and not torch.backends.cuda.matmul.allow_tf32
     import torch.nn.functional as F
     from baselines_b200 import nn as bnn, ops
     dev = torch.device("cuda")
