@@ -26,13 +26,16 @@ SIGNATURES = {
     "b200rl_frame_stack": [_p, _p, _p, _p, _ll, _ll, _i, _i, _p],
     "b200rl_col2im": [_p, _p, _p, _ll, _i, _i, _i, _i, _i, _i, _i, _p],
     "b200rl_colsum": [_p, _p, _ll, _i, _ll, _f, _p],
-    "b200rl_cat_step": [_p, _ll, _i, _p, _ll, _p, _ull, _ull, _p, _p, _p, _p, _ll, _p],
+    "b200rl_cat_step": [_p, _ll, _i, _p, _i, _p, _ll, _p, _ull, _ull, _p, _p, _p, _p, _ll, _p],
+    "b200rl_bern_step": [_p, _ll, _i, _p, _ll, _p, _ull, _ull, _p, _p, _p, _p, _ll, _p],
     "b200rl_gauss_step": [_p, _ll, _p, _i, _p, _ll, _p, _ull, _ull, _p, _p, _p, _p, _ll, _p],
     "b200rl_set_scalars": [_p, _i, _f, _f, _f, _f, _p],
     "b200rl_shuffle_indices": [_p, _ll, _ull, _ll, _ll, _p],
     "b200rl_counter_add": [_p, _ull, _p],
     "b200rl_adv_stats": [_p, _p, _p, _ll, _p, _p],
-    "b200rl_cat_loss": [_p, _ll, _i, _p, _ll, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _ll, _p, _ll, _p, _ll, _p, _p],
+    "b200rl_cat_loss": [_p, _ll, _i, _p, _i, _p, _ll, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _ll, _p, _ll, _p, _ll, _p,
+                        _p],
+    "b200rl_bern_loss": [_p, _ll, _i, _p, _ll, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _ll, _p, _ll, _p, _ll, _p, _p],
     "b200rl_gauss_loss": [_p, _ll, _p, _i, _p, _ll, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _ll, _p, _ll, _p, _f,
                           _p, _ll, _p, _p],
     "b200rl_sumsq": [_p, _ll, _p, _p],
@@ -42,7 +45,7 @@ SIGNATURES = {
     "b200rl_cast_transpose": [_p, _i, _i, _p, _ll, _p, _ll, _f, _p],
     "b200rl_cast_transpose_batch": [_p, _i, _i, _i, _p],
     "b200rl_cast_f32_f16": [_p, _p, _ll, _i, _ll, _ll, _f, _p],
-    "b200rl_obs_encode": [_p, _p, _ll, _i, _i, _i, _p, _p, _f, _f, _i, _p, _p],
+    "b200rl_obs_encode": [_p, _p, _ll, _i, _i, _i, _p, _p, _f, _f, _i, _p, _i, _p, _p],
     "b200rl_tree_set": [_p, _p, _ll, _p, _p, _i, _p],
     "b200rl_tree_range_sum": [_p, _ll, _ll, _ll, _p, _p],
     "b200rl_per_sample": [_p, _p, _ll, _ll, _p, _i, _d, _p, _p, _p, _p],

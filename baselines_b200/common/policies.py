@@ -1,9 +1,9 @@
 """Policy / value network for the PPO2 learner on the H100 kernels.
 
 Behavioural mirror of the reference's common/policies.py (build_policy :121-179, PolicyWithValue
-:13-119), common/distributions.py (CategoricalPd :153-204, DiagGaussianPd :227-251) and
-common/input.py:43-63.  The object protocol (step / value) is kept; the TF graph is replaced by an
-explicit sequence of libb200rl kernel launches.
+:13-119), common/distributions.py (CategoricalPd :153-204, MultiCategoricalPd :206-225, DiagGaussianPd :227-251,
+BernoulliPd :254-276) and common/input.py:43-63.  The object protocol (step / value) is kept; the TF graph is
+replaced by an explicit sequence of libb200rl kernel launches.
 """
 import numpy as np
 import torch
@@ -50,20 +50,38 @@ class PolicyNet:
         self.device, self.cap = device, cap
         ob_space, ac_space = builder.ob_space, builder.ac_space
         self.ob_shape = tuple(ob_space.shape)
-        # common/input.py:54-55: Discrete(n) observations are fed one-hot; MultiDiscrete is not on the hot path
-        if hasattr(ob_space, "nvec"):
-            raise NotImplementedError("MultiDiscrete observations (common/input.py:58-61) are outside the hot-path scope")
+        # common/input.py:54-61: Discrete(n) / MultiDiscrete(nvec) observations are fed one-hot (MultiBinary ones are
+        # rejected there too)
+        self.ob_nvec = None
+        if spaces.is_multi_discrete(ob_space):
+            self.ob_nvec = [int(v) for v in np.asarray(ob_space.nvec).reshape(-1)]
+        if spaces.is_multi_binary(ob_space):
+            raise NotImplementedError("MultiBinary observations have no encoding in common/input.py:43-63")
         self.ob_onehot = int(ob_space.n) if spaces.is_discrete(ob_space) else 0
-        if self.ob_onehot and builder.network != "mlp":
-            raise NotImplementedError("Discrete observations need a vector network ('mlp')")
-        self.discrete = spaces.is_discrete(ac_space)
-        if self.discrete:
-            self.nout = int(ac_space.n)
+        if (self.ob_onehot or self.ob_nvec) and builder.network != "mlp":
+            raise NotImplementedError("Discrete / MultiDiscrete observations need a vector network ('mlp')")
+        # the action distribution (distributions.py:278-290 make_pdtype): 'cat' Categorical (Discrete), 'mcat'
+        # MultiCategorical (MultiDiscrete), 'bern' Bernoulli (MultiBinary), 'gauss' DiagGaussian (Box)
+        self.nvec = None
+        if spaces.is_multi_discrete(ac_space):
+            self.pd = "mcat"
+            self.nvec = [int(v) for v in np.asarray(ac_space.nvec).reshape(-1)]
+            if not self.nvec or min(self.nvec) < 1:                            # distributions.py:79
+                raise ValueError(f"MultiDiscrete action nvec entries must be >= 1, got {self.nvec}")
+            self.nout, self.act_dim = sum(self.nvec), len(self.nvec)
+        elif spaces.is_multi_binary(ac_space):
+            self.pd = "bern"
+            self.nout = self.act_dim = int(ac_space.n)
+        elif spaces.is_discrete(ac_space):
+            self.pd = "cat"
+            self.nout, self.act_dim = int(ac_space.n), 0
         elif spaces.is_box(ac_space):
+            self.pd = "gauss"
             assert len(ac_space.shape) == 1                                    # distributions.py:281
-            self.nout = int(ac_space.shape[0])
+            self.nout = self.act_dim = int(ac_space.shape[0])
         else:
-            raise NotImplementedError("only Discrete and Box action spaces are on the hot path (SURVEY 2, #6)")
+            raise NotImplementedError("action spaces: Discrete, MultiDiscrete, MultiBinary and Box "
+                                      "(distributions.py:278-290)")
         kind = builder.network
         self.kind = kind
         self.copy_vf = builder.value_network == "copy"
@@ -71,6 +89,8 @@ class PolicyNet:
         kw = dict(builder.network_kwargs)
         if self.ob_onehot:
             kw["onehot_n"] = self.ob_onehot
+        if self.ob_nvec:
+            kw["onehot_nvec"] = self.ob_nvec
         # creation order == the reference's variable creation order (it fixes the ortho_init RNG stream)
         self.tower_pi = nn.Tower(store, kind, self.ob_shape, "pi", f"{scope}/pi", rng, cap, **kw)
         self.tower_vf = nn.Tower(store, kind, self.ob_shape, "vf", f"{scope}/vf", rng, cap, **kw) if self.copy_vf else None
@@ -81,7 +101,7 @@ class PolicyNet:
         # no 'pi/w', 'pi/b' variables exist (and no ortho_init draw is consumed), like the reference.
         self.pi_identity = (L == self.nout)
         w_pi = np.eye(L, dtype=np.float32) if self.pi_identity else nn.ortho_init((L, self.nout), 0.01, rng)  # policies.py:49
-        if not self.discrete:
+        if self.pd == "gauss":
             store.add("pi/logstd", np.zeros((1, self.nout), np.float32))         # distributions.py:104
             store.map_tf(f"{scope}/pi/logstd:0", "pi/logstd", (1, self.nout))
         Lv = self.tower_vf.latent_dim if self.copy_vf else L
@@ -107,7 +127,7 @@ class PolicyNet:
         # in ppo2 ever updates those statistics, so they stay at their initial values (mean 0, std 1) unless a
         # checkpoint provides others; they are kept, saved and loaded under the reference's variable names.
         self.obs_rms = None
-        if builder.normalize_observations and not self.tower_pi.in_u8 and not self.ob_onehot:
+        if builder.normalize_observations and not self.tower_pi.in_u8 and not self.ob_onehot and not self.ob_nvec:
             d = self.tower_pi.raw_dim
             self.obs_rms = {"runningsum": np.zeros(self.ob_shape, np.float64),
                             "runningsumsq": np.full(self.ob_shape, 1e-2, np.float64),
@@ -170,13 +190,30 @@ class PolicyNet:
             self.dpi = torch.zeros(cap, self.ld_dpi, **f16)
             self.ld_dv = 64
             self.dv = torch.zeros(cap, 64, **f16)
-        if not self.discrete:
+        if self.pd == "gauss":
             self.logstd = self.store.views["pi/logstd"].view(-1)
             self.g_logstd = self.store.gviews["pi/logstd"].view(-1)
+        # MultiDiscrete: offsets of the components' logit blocks, allocated once (captured launch sequences read it)
+        self.seg_off = ops.segment_table(self.nvec, dev) if self.pd == "mcat" else None
         self.adv_st = torch.zeros(2, dtype=torch.float64, device=dev)
         self.stats = torch.zeros(5, dtype=torch.float64, device=dev)
         self.clip_dev = torch.zeros(1, dtype=torch.float32, device=dev)      # clip range of the current update
         self.rng_ctr = torch.zeros(1, dtype=torch.int64, device=dev)         # sampler stream position (Philox offset)
+
+    def action_shape(self, *lead):
+        """Device action rows: int64 [*] (Discrete), int64 [*, k] (MultiDiscrete), float32 [*, n] (MultiBinary),
+        float32 [*, d] (Box)."""
+        return tuple(lead) if self.pd == "cat" else tuple(lead) + (self.act_dim,)
+
+    @property
+    def action_dtype(self):
+        return torch.int64 if self.pd in ("cat", "mcat") else torch.float32
+
+    def actions_to_numpy(self, a):
+        """Device actions -> what the reference's pd.sample() hands out: int32 for MultiDiscrete
+        (distributions.py:222), float32 for MultiBinary (:273), int64 / float32 as before otherwise."""
+        out = a.cpu().numpy()
+        return out.astype(np.int32) if self.pd == "mcat" else out
 
     def set_obs_rms(self, values=None):
         """Install RunningMeanStd variables (mpi_running_mean_std.py:29-30: mean = sum/count,
@@ -282,9 +319,12 @@ class PolicyNet:
         is a device counter advanced after every pass, so the sequence can be replayed from a CUDA graph."""
         _lib.phase = "@act"
         self.forward(x, B, masks=False)
-        if self.discrete:
+        if self.pd in ("cat", "mcat"):
             ops.cat_step(self.pi_out, self.ld_pi, self.nout, self.v_out, self.ld_v, actions, values, neglogp, B,
-                         uniforms=noise, seed=seed, offset_dev=self.rng_ctr)
+                         uniforms=noise, seed=seed, offset_dev=self.rng_ctr, seg_off=self.seg_off)
+        elif self.pd == "bern":
+            ops.bern_step(self.pi_out, self.ld_pi, self.nout, self.v_out, self.ld_v, actions, values, neglogp, B,
+                          uniforms=noise, seed=seed, offset_dev=self.rng_ctr)
         else:
             ops.gauss_step(self.pi_out, self.ld_pi, self.logstd, self.nout, self.v_out, self.ld_v, actions, values,
                            neglogp, B, normals=noise, seed=seed, offset_dev=self.rng_ctr)
@@ -318,10 +358,14 @@ class PolicyNet:
         cliprange = 0.0 if cliprange is None else cliprange
         _lib.phase = "@train"
         self.forward(x, B, src_idx)
-        if self.discrete:
+        if self.pd in ("cat", "mcat"):
             ops.cat_loss(self.pi_out, self.ld_pi, self.nout, self.v_out, self.ld_v, actions, src_idx, returns,
                          old_values, old_neglogp, self.adv_st, cliprange, ent_coef, vf_coef, self.dpi, self.ld_dpi,
-                         self.dv, self.ld_dv, self.stats, B, cliprange_dev=clip_dev)
+                         self.dv, self.ld_dv, self.stats, B, cliprange_dev=clip_dev, seg_off=self.seg_off)
+        elif self.pd == "bern":
+            ops.bern_loss(self.pi_out, self.ld_pi, self.nout, self.v_out, self.ld_v, actions, src_idx, returns,
+                          old_values, old_neglogp, self.adv_st, cliprange, ent_coef, vf_coef, self.dpi, self.ld_dpi,
+                          self.dv, self.ld_dv, self.stats, B, cliprange_dev=clip_dev)
         else:
             ops.gauss_loss(self.pi_out, self.ld_pi, self.logstd, self.nout, self.v_out, self.ld_v, actions, src_idx,
                            returns, old_values, old_neglogp, self.adv_st, cliprange, ent_coef, vf_coef, self.dpi,

@@ -34,8 +34,11 @@ int s2d_gather_impl(const void*, const long long*, void*, long long, int, int, i
 int frame_stack_impl(const void*, const void*, const void*, void*, long long, long long, int, int, cudaStream_t);
 int col2im_impl(const void*, const void*, void*, long long, int, int, int, int, int, int, int, cudaStream_t);
 int colsum_impl(const void*, float*, long long, int, long long, float, cudaStream_t);
-int cat_step_impl(const float*, long long, int, const float*, long long, const float*, unsigned long long,
-                  unsigned long long, const unsigned long long*, long long*, float*, float*, long long, cudaStream_t);
+int cat_step_impl(const float*, long long, int, const int*, int, const float*, long long, const float*,
+                  unsigned long long, unsigned long long, const unsigned long long*, long long*, float*, float*,
+                  long long, cudaStream_t);
+int bern_step_impl(const float*, long long, int, const float*, long long, const float*, unsigned long long,
+                   unsigned long long, const unsigned long long*, float*, float*, float*, long long, cudaStream_t);
 int gauss_step_impl(const float*, long long, const float*, int, const float*, long long, const float*,
                     unsigned long long, unsigned long long, const unsigned long long*, float*, float*, float*,
                     long long, cudaStream_t);
@@ -43,9 +46,12 @@ int set_scalars_impl(float*, int, float, float, float, float, cudaStream_t);
 int shuffle_indices_impl(long long*, long long, unsigned long long, long long, long long, cudaStream_t);
 int counter_add_impl(unsigned long long*, unsigned long long, cudaStream_t);
 int adv_stats_impl(const float*, const float*, const long long*, long long, double*, cudaStream_t);
-int cat_loss_impl(const float*, long long, int, const float*, long long, const long long*, const long long*,
-                  const float*, const float*, const float*, const double*, float, float, float, void*, long long,
-                  void*, long long, double*, long long, const float*, cudaStream_t);
+int cat_loss_impl(const float*, long long, int, const int*, int, const float*, long long, const long long*,
+                  const long long*, const float*, const float*, const float*, const double*, float, float, float, void*,
+                  long long, void*, long long, double*, long long, const float*, cudaStream_t);
+int bern_loss_impl(const float*, long long, int, const float*, long long, const float*, const long long*, const float*,
+                   const float*, const float*, const double*, float, float, float, void*, long long, void*, long long,
+                   double*, long long, const float*, cudaStream_t);
 int gauss_loss_impl(const float*, long long, const float*, int, const float*, long long, const float*,
                     const long long*, const float*, const float*, const float*, const double*, float, float, float,
                     void*, long long, void*, long long, float*, float, double*, long long, const float*, cudaStream_t);
@@ -58,7 +64,7 @@ int cast_transpose_impl(const float*, int, int, void*, long long, void*, long lo
 int cast_f32_f16_impl(const float*, void*, long long, int, long long, long long, float, cudaStream_t);
 int cast_transpose_batch_impl(const void*, int, int, int, cudaStream_t);
 int obs_encode_impl(const float*, const long long*, long long, int, int, int, const float*, const float*, float, float,
-                    int, void*, cudaStream_t);
+                    int, const int*, int, void*, cudaStream_t);
 int tree_set_impl(double*, double*, long long, const long long*, const double*, int, cudaStream_t);
 int tree_range_sum_impl(const double*, long long, long long, long long, double*, cudaStream_t);
 int per_sample_impl(const double*, const double*, long long, long long, const double*, int, double, long long*,
@@ -146,12 +152,21 @@ int b200rl_colsum(const void* dz, float* db, long long rows, int C, long long ld
   return colsum_impl(dz, db, rows, C, ld, alpha, S(stream));
 }
 
-int b200rl_cat_step(const float* logits, long long ld, int nA, const float* vpred, long long ldv,
-                    const float* uniforms, unsigned long long seed, unsigned long long offset,
+// CategoricalPd / MultiCategoricalPd .sample + .neglogp (distributions.py:76-94,164-201,206-225)
+int b200rl_cat_step(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
+                    long long ldv, const float* uniforms, unsigned long long seed, unsigned long long offset,
                     const unsigned long long* offset_dev, long long* actions, float* values, float* neglogp,
                     long long B, void* stream) {
-  return cat_step_impl(logits, ld, nA, vpred, ldv, uniforms, seed, offset, offset_dev, actions, values, neglogp, B,
-                       S(stream));
+  return cat_step_impl(logits, ld, nA, seg_off, nseg, vpred, ldv, uniforms, seed, offset, offset_dev, actions, values,
+                       neglogp, B, S(stream));
+}
+// BernoulliPd.sample + .neglogp (distributions.py:115-128,254-276)
+int b200rl_bern_step(const float* logits, long long ld, int n, const float* vpred, long long ldv,
+                     const float* uniforms, unsigned long long seed, unsigned long long offset,
+                     const unsigned long long* offset_dev, float* actions, float* values, float* neglogp, long long B,
+                     void* stream) {
+  return bern_step_impl(logits, ld, n, vpred, ldv, uniforms, seed, offset, offset_dev, actions, values, neglogp, B,
+                        S(stream));
 }
 int b200rl_shuffle_indices(long long* out, long long n, unsigned long long key, long long T, long long N, void* stream) {
   return shuffle_indices_impl(out, n, key, T, N, S(stream));
@@ -173,13 +188,24 @@ int b200rl_adv_stats(const float* returns, const float* values, const long long*
                      void* stream) {
   return adv_stats_impl(returns, values, src_idx, M, out, S(stream));
 }
-int b200rl_cat_loss(const float* logits, long long ld, int nA, const float* vpred, long long ldv,
-                    const long long* actions, const long long* src_idx, const float* returns,
+// ppo2/model.py:57-91 with CategoricalPd / MultiCategoricalPd (distributions.py:76-94,164-198,206-225)
+int b200rl_cat_loss(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
+                    long long ldv, const long long* actions, const long long* src_idx, const float* returns,
                     const float* old_values, const float* old_neglogp, const double* adv_stats, float cliprange,
                     float ent_coef, float vf_coef, void* dlogits, long long ld_dl, void* dv, long long ld_dv,
                     double* stats, long long B, const float* cliprange_dev, void* stream) {
-  return cat_loss_impl(logits, ld, nA, vpred, ldv, actions, src_idx, returns, old_values, old_neglogp, adv_stats,
-                       cliprange, ent_coef, vf_coef, dlogits, ld_dl, dv, ld_dv, stats, B, cliprange_dev, S(stream));
+  return cat_loss_impl(logits, ld, nA, seg_off, nseg, vpred, ldv, actions, src_idx, returns, old_values, old_neglogp,
+                       adv_stats, cliprange, ent_coef, vf_coef, dlogits, ld_dl, dv, ld_dv, stats, B, cliprange_dev,
+                       S(stream));
+}
+// ppo2/model.py:57-91 with BernoulliPd (distributions.py:115-128,254-276)
+int b200rl_bern_loss(const float* logits, long long ld, int n, const float* vpred, long long ldv,
+                     const float* actions, const long long* src_idx, const float* returns, const float* old_values,
+                     const float* old_neglogp, const double* adv_stats, float cliprange, float ent_coef,
+                     float vf_coef, void* dlogits, long long ld_dl, void* dv, long long ld_dv, double* stats,
+                     long long B, const float* cliprange_dev, void* stream) {
+  return bern_loss_impl(logits, ld, n, vpred, ldv, actions, src_idx, returns, old_values, old_neglogp, adv_stats,
+                        cliprange, ent_coef, vf_coef, dlogits, ld_dl, dv, ld_dv, stats, B, cliprange_dev, S(stream));
 }
 int b200rl_gauss_loss(const float* mean, long long ld, const float* logstd, int d, const float* vpred,
                       long long ldv, const float* actions, const long long* src_idx, const float* returns,
@@ -217,11 +243,12 @@ int b200rl_cast_f32_f16(const float* src, void* dst, long long rows, int cols, l
   return cast_f32_f16_impl(src, dst, rows, cols, ld_src, ld_dst, scale, S(stream));
 }
 
+// common/input.py:43-63 encode_observation (Discrete :54-55, MultiDiscrete :58-61), policies.py:182-185
 int b200rl_obs_encode(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim, int in_pad,
-                      const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n, void* out,
-                      void* stream) {
-  return obs_encode_impl(x, src_idx, B, raw_dim, in_dim, in_pad, mean, inv_std, clip_lo, clip_hi, onehot_n, out,
-                         S(stream));
+                      const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n,
+                      const int* seg_off, int nseg, void* out, void* stream) {
+  return obs_encode_impl(x, src_idx, B, raw_dim, in_dim, in_pad, mean, inv_std, clip_lo, clip_hi, onehot_n, seg_off,
+                         nseg, out, S(stream));
 }
 
 int b200rl_tree_set(double* sum_tree, double* min_tree, long long capacity, const long long* idx, const double* vals,

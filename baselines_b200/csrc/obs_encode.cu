@@ -6,7 +6,9 @@
 //     hi = fp16(v),  lo = fp16(v - hi)          (v - hi is exact in fp32; |v - (hi + lo)| <= 2^-22 |v|)
 // laid out side by side as one operand row [hi(0..in_pad) | lo(0..in_pad)].  The first GEMM runs over K = 2*in_pad
 // against the weight matrix stacked twice ([W ; W]), i.e. x.W = hi.W + lo.W accumulated in fp32: the observation
-// itself is no longer quantised to 11 bits.  Discrete observations become exact one-hot rows (lo = 0).
+// itself is no longer quantised to 11 bits.  Discrete observations become exact one-hot rows (lo = 0); a MultiDiscrete
+// observation (k integers) becomes the concatenation of k one-hot blocks [seg_off[s], seg_off[s+1]) (input.py:58-61),
+// of which Discrete(n) is the single block [0, n).
 #include "common.cuh"
 
 namespace b200rl {
@@ -19,7 +21,9 @@ struct ObsEncodeParams {
   const float* mean;         // optional [raw_dim]
   const float* inv_std;      // optional [raw_dim]
   float clip_lo, clip_hi;    // applied when mean != nullptr
-  int onehot_n;              // > 0: Discrete(n) observation
+  int onehot_n;              // > 0: Discrete(n) / MultiDiscrete observation, one-hot row width (= in_dim)
+  const int* seg_off;        // optional [nseg + 1] one-hot block offsets (MultiDiscrete); null: one block [0, onehot_n)
+  int nseg;
   __half* out;               // [B, 2 * in_pad]
 };
 
@@ -33,10 +37,24 @@ __global__ void __launch_bounds__(256) obs_encode_kernel(const ObsEncodeParams p
     const long long r = p.src_idx ? p.src_idx[b] : b;
     const float* src = p.x + r * p.raw_dim;
     float v[8];
-    if (p.onehot_n > 0) {
+    if (p.onehot_n > 0 && p.seg_off == nullptr) {
       const int k = (int)src[0];
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[j] = (c0 + j == k) ? 1.0f : 0.0f;
+    } else if (p.onehot_n > 0) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = 0.0f;
+      for (int s = 0; s < p.nseg; ++s) {           // the hot column of every block that reaches into this group
+        const int lo = p.seg_off[s], hi = p.seg_off[s + 1];
+        if (hi <= c0 || lo >= c0 + 8) continue;
+        const int k = (int)src[s];
+        const int c = lo + k;
+        if (k >= 0 && c < hi && c >= c0 && c < c0 + 8) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            if (c0 + j == c) v[j] = 1.0f;
+        }
+      }
     } else {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -62,18 +80,21 @@ __global__ void __launch_bounds__(256) obs_encode_kernel(const ObsEncodeParams p
 }
 
 int obs_encode_impl(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim, int in_pad,
-                    const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n, void* out,
-                    cudaStream_t stream) {
+                    const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n,
+                    const int* seg_off, int nseg, void* out, cudaStream_t stream) {
   B200RL_REQUIRE(x && out && B > 0, "obs_encode: null operand");
   B200RL_REQUIRE(in_pad % 8 == 0 && in_pad >= in_dim && in_dim > 0, "obs_encode: in_pad must be a multiple of 8 >= in_dim");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "obs_encode: output must be 16-byte aligned");
   B200RL_REQUIRE((mean == nullptr) == (inv_std == nullptr), "obs_encode: mean and inv_std come together");
-  if (onehot_n > 0)
+  if (onehot_n > 0 && seg_off)
+    B200RL_REQUIRE(nseg >= 1 && raw_dim == nseg && in_dim == onehot_n && mean == nullptr,
+                   "obs_encode: MultiDiscrete one-hot needs raw_dim = nseg, in_dim = sum(nvec)");
+  else if (onehot_n > 0)
     B200RL_REQUIRE(raw_dim == 1 && in_dim == onehot_n && mean == nullptr, "obs_encode: one-hot needs raw_dim 1, in_dim n");
   else
     B200RL_REQUIRE(raw_dim == in_dim, "obs_encode: raw_dim != in_dim");
   ObsEncodeParams p{x, src_idx, B, raw_dim, in_dim, in_pad, mean, inv_std, clip_lo, clip_hi, onehot_n,
-                    reinterpret_cast<__half*>(out)};
+                    onehot_n > 0 ? seg_off : nullptr, nseg, reinterpret_cast<__half*>(out)};
   const long long total = B * (in_pad / 8);
   long long blocks = (total + 255) / 256;
   if (blocks > 16LL * device_num_sms()) blocks = 16LL * device_num_sms();

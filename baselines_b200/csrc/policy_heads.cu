@@ -1,6 +1,7 @@
 // Row-wise policy-head kernels (one thread per sample; all HBM/latency bound, no reuse):
-//   * act path  (PolicyWithValue.step, common/policies.py:77-96): Gumbel-max sample
-//     (distributions.py:199-201), neglogp (:164-183) / DiagGaussian sample+neglogp (:238-248)
+//   * act path  (PolicyWithValue.step, common/policies.py:77-96): Gumbel-max sample per categorical segment
+//     (distributions.py:199-201, MultiCategorical :76-94), neglogp (:164-183) / Bernoulli sample+neglogp (:115-128) /
+//     DiagGaussian sample+neglogp (:238-248)
 //   * train path (ppo2/model.py:57-91): clipped-surrogate + clipped-value + entropy loss, its five
 //     statistics, and the hand-derived gradient w.r.t. the head outputs (logits / mean, value), written
 //     as fp16 in "sum" scaling (the 1/M of tf.reduce_mean is applied as alpha in the wgrad epilogues so
@@ -33,36 +34,107 @@ __device__ __forceinline__ void philox4(uint64_t seed, uint64_t row, uint32_t ct
 }
 __device__ __forceinline__ float u01_open(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
 
-// ---------------------------------------------------------------- categorical: act
+// ---------------------------------------------------------------- categorical / multi-categorical: act
+// A row of nA logits is cut into segments [seg_off[s], seg_off[s+1]) (MultiCategoricalPd, distributions.py:76-94,
+// 206-225: one independent categorical per MultiDiscrete component); Discrete(n) is the single segment [0, n).
+// MULTI = false is that single segment with its bounds known at compile time.  Uniform j of a row is always column j
+// of the row's Philox stream (or of `uniforms`), whichever segment it falls in.
+template <bool MULTI>
+__device__ __forceinline__ void seg_bounds(const int* seg_off, int nA, int s, int& lo, int& hi) {
+  lo = MULTI ? seg_off[s] : 0;
+  hi = MULTI ? seg_off[s + 1] : nA;
+}
+
+// max, partition function and entropy (distributions.py:193-198) of the softmax over l[lo, hi)
+__device__ __forceinline__ void seg_softmax(const float* l, int lo, int hi, float& m, float& z, float& logz, float& H) {
+  m = -INFINITY;
+  for (int j = lo; j < hi; ++j) m = fmaxf(m, l[j]);
+  z = 0.0f;
+  for (int j = lo; j < hi; ++j) z += expf(l[j] - m);
+  logz = logf(z);
+  H = 0.0f;
+  for (int j = lo; j < hi; ++j) {
+    const float a0 = l[j] - m;
+    H += (expf(a0) / z) * (logz - a0);
+  }
+}
+
+template <bool MULTI>
 __global__ void __launch_bounds__(256)
-cat_step_kernel(const float* __restrict__ logits, long long ld, int nA, const float* __restrict__ vpred, long long ldv,
-                const float* __restrict__ uniforms, uint64_t seed, uint64_t offset,
-                const unsigned long long* __restrict__ offset_dev, long long* __restrict__ actions,
+cat_step_kernel(const float* __restrict__ logits, long long ld, int nA, const int* __restrict__ seg_off, int nseg,
+                const float* __restrict__ vpred, long long ldv, const float* __restrict__ uniforms, uint64_t seed,
+                uint64_t offset, const unsigned long long* __restrict__ offset_dev, long long* __restrict__ actions,
                 float* __restrict__ values, float* __restrict__ neglogp, long long B) {
   const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   if (offset_dev) offset = *offset_dev;            // stream position kept on the device (CUDA-graph replays)
+  if (!MULTI) nseg = 1;
   const float* l = logits + b * ld;
-  float m = -INFINITY;
-  for (int j = 0; j < nA; ++j) m = fmaxf(m, l[j]);
-  float z = 0.0f;
-  for (int j = 0; j < nA; ++j) z += expf(l[j] - m);
-  float best = -INFINITY;
-  int a = 0;
   uint32_t rnd[4];
-  for (int j = 0; j < nA; ++j) {
+  int held = -1;                                   // Philox counter whose 4 words are in rnd
+  float nlp = 0.0f;
+  for (int s = 0; s < nseg; ++s) {
+    int lo, hi;
+    seg_bounds<MULTI>(seg_off, nA, s, lo, hi);
+    float m = -INFINITY;
+    for (int j = lo; j < hi; ++j) m = fmaxf(m, l[j]);
+    float z = 0.0f;
+    for (int j = lo; j < hi; ++j) z += expf(l[j] - m);
+    float best = -INFINITY;
+    int a = lo;
+    for (int j = lo; j < hi; ++j) {
+      float u;
+      if (uniforms) {
+        u = uniforms[b * nA + j];
+      } else {
+        if ((j >> 2) != held) {
+          held = j >> 2;
+          philox4(seed, (uint64_t)b, (uint32_t)held, (uint32_t)offset, rnd);
+        }
+        u = u01_open(rnd[j & 3]);
+      }
+      const float sc = l[j] - logf(-logf(u));
+      if (sc > best) { best = sc; a = j; }   // first max wins (tf.argmax)
+    }
+    actions[b * nseg + s] = a - lo;
+    nlp += (m + logf(z)) - l[a];             // sum of the components' neglogp (distributions.py:86-87)
+  }
+  neglogp[b] = nlp;
+  values[b] = vpred[b * ldv];
+}
+
+// ---------------------------------------------------------------- Bernoulli (MultiBinary): act
+// BernoulliPd (distributions.py:115-128, 254-276): p = sigmoid(l); x = float(u < p); neglogp = sum sigmoid_xent(l, x)
+__device__ __forceinline__ float sigmoid_xent(float l, float y) {   // tf.nn.sigmoid_cross_entropy_with_logits
+  return fmaxf(l, 0.0f) - l * y + log1pf(expf(-fabsf(l)));
+}
+__device__ __forceinline__ float sigmoidf(float l) { return 1.0f / (1.0f + expf(-l)); }
+
+__global__ void __launch_bounds__(256)
+bern_step_kernel(const float* __restrict__ logits, long long ld, int n, const float* __restrict__ vpred, long long ldv,
+                 const float* __restrict__ uniforms, uint64_t seed, uint64_t offset,
+                 const unsigned long long* __restrict__ offset_dev, float* __restrict__ actions,
+                 float* __restrict__ values, float* __restrict__ neglogp, long long B) {
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  if (offset_dev) offset = *offset_dev;
+  const float* l = logits + b * ld;
+  uint32_t rnd[4];
+  float nlp = 0.0f;
+  for (int j = 0; j < n; ++j) {
     float u;
     if (uniforms) {
-      u = uniforms[b * nA + j];
+      u = uniforms[b * n + j];
     } else {
       if ((j & 3) == 0) philox4(seed, (uint64_t)b, (uint32_t)(j >> 2), (uint32_t)offset, rnd);
       u = u01_open(rnd[j & 3]);
     }
-    const float s = l[j] - logf(-logf(u));
-    if (s > best) { best = s; a = j; }      // first max wins (tf.argmax)
+    const float lj = l[j];
+    const float x = (u < sigmoidf(lj)) ? 1.0f : 0.0f;
+    actions[b * n + j] = x;
+    nlp += sigmoid_xent(lj, x);
   }
-  actions[b] = a;
-  neglogp[b] = (m + logf(z)) - l[a];
+  neglogp[b] = nlp;
   values[b] = vpred[b * ldv];
 }
 
@@ -224,28 +296,33 @@ __device__ __forceinline__ float pg_loss_grad(float nlp, float oldnlp, float adv
   return (ratio >= 1.0f - clip && ratio <= 1.0f + clip) ? adv * ratio : 0.0f;
 }
 
-// ---------------------------------------------------------------- categorical: loss + gradient
+// ---------------------------------------------------------------- categorical / multi-categorical: loss + gradient
+// actions: [*, nseg] rows (component index inside its segment), gathered through src_idx.  For logit j of segment s:
+//   d nlp/dl_j = p_j - 1{j = off_s + a_s};  d(-ent_coef * sum_s H_s)/dl_j = ent_coef * p_j * (log p_j + H_s)
+// with the segment's own entropy H_s.  The gradient pass recomputes each segment's softmax (MULTI = false: the single
+// segment's values of the first pass are reused).
+template <bool MULTI>
 __global__ void __launch_bounds__(256)
-cat_loss_kernel(const float* __restrict__ logits, long long ld, int nA, const float* __restrict__ vpred,
-                long long ldv, const long long* __restrict__ actions, PpoCommon pc, __half* __restrict__ dlogits,
-                long long ld_dl, __half* __restrict__ dv, long long ld_dv, long long B) {
+cat_loss_kernel(const float* __restrict__ logits, long long ld, int nA, const int* __restrict__ seg_off, int nseg,
+                const float* __restrict__ vpred, long long ldv, const long long* __restrict__ actions, PpoCommon pc,
+                __half* __restrict__ dlogits, long long ld_dl, __half* __restrict__ dv, long long ld_dv, long long B) {
   const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double st[5] = {0, 0, 0, 0, 0};
+  if (!MULTI) nseg = 1;
   if (b < B) {
     const long long s = pc.src_idx ? pc.src_idx[b] : b;
     const float* l = logits + b * ld;
-    float m = -INFINITY;
-    for (int j = 0; j < nA; ++j) m = fmaxf(m, l[j]);
-    float z = 0.0f;
-    for (int j = 0; j < nA; ++j) z += expf(l[j] - m);
-    const float logz = logf(z);
-    float H = 0.0f;                                    // distributions.py:193-198
-    for (int j = 0; j < nA; ++j) {
-      const float a0 = l[j] - m;
-      H += (expf(a0) / z) * (logz - a0);
+    const long long* arow = actions + s * nseg;
+    float m, z, logz, Hs;                              // softmax of the current segment
+    int lo, hi, a;
+    float nlp = 0.0f, H = 0.0f;
+    for (int g = 0; g < nseg; ++g) {
+      seg_bounds<MULTI>(seg_off, nA, g, lo, hi);
+      seg_softmax(l, lo, hi, m, z, logz, Hs);
+      a = lo + (int)arow[g];
+      nlp += (m + logz) - l[a];
+      H += Hs;
     }
-    const int a = (int)actions[s];
-    const float nlp = (m + logz) - l[a];
     const float R = pc.returns[s], oldv = pc.old_values[s];
     const float adv_raw = __fsub_rn(R, oldv);
     const float adv = (float)(((double)adv_raw - pc.adv_stats[0]) / (pc.adv_stats[1] + 1e-8));
@@ -257,28 +334,114 @@ cat_loss_kernel(const float* __restrict__ logits, long long ld, int nA, const fl
     // store-instruction bound: 32 rows x 2 B per instruction).  Columns past nA inside the last group are zero.
     __half* drow = dlogits + b * ld_dl;
     const bool vec = ((ld_dl & 7) == 0) && ((reinterpret_cast<uintptr_t>(dlogits) & 15) == 0) && (((nA + 7) & ~7) <= ld_dl);
-    for (int j0 = 0; j0 < nA; j0 += 8) {
+    if (MULTI) {
+      // segment by segment; the fp16 values pass through a 4-word shift register that leaves as one 16-byte store per
+      // 8-column group (registers only: the row's segment layout is not known at compile time)
+      uint32_t w0 = 0, w1 = 0, w2 = 0, w3 = 0;
+      auto push = [&](__half h) {
+        w0 = (w0 >> 16) | (w1 << 16);
+        w1 = (w1 >> 16) | (w2 << 16);
+        w2 = (w2 >> 16) | (w3 << 16);
+        w3 = (w3 >> 16) | ((uint32_t)__half_as_ushort(h) << 16);
+      };
+      for (int g = 0; g < nseg; ++g) {
+        seg_bounds<MULTI>(seg_off, nA, g, lo, hi);
+        seg_softmax(l, lo, hi, m, z, logz, Hs);
+        a = lo + (int)arow[g];
+        for (int j = lo; j < hi; ++j) {
+          const float a0 = l[j] - m;
+          const float pj = expf(a0) / z;
+          const float logpj = a0 - logz;
+          const __half h = __float2half_rn(g_nlp * (pj - (j == a ? 1.0f : 0.0f)) + pc.ent_coef * pj * (logpj + Hs));
+          if (vec) {
+            push(h);
+            if ((j & 7) == 7) *reinterpret_cast<uint4*>(drow + (j - 7)) = make_uint4(w0, w1, w2, w3);
+          } else {
+            drow[j] = h;
+          }
+        }
+      }
+      if (vec && (nA & 7)) {                           // last partial group: columns past nA are zero
+        for (int j = nA; j & 7; ++j) push(__float2half_rn(0.0f));
+        *reinterpret_cast<uint4*>(drow + (nA & ~7)) = make_uint4(w0, w1, w2, w3);
+      }
+    } else {
+      for (int j0 = 0; j0 < nA; j0 += 8) {
+        __align__(16) __half g8[8];
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = j0 + jj;
+          float gj = 0.0f;
+          if (j < nA) {
+            const float a0 = l[j] - m;
+            const float pj = expf(a0) / z;
+            const float logpj = a0 - logz;
+            gj = g_nlp * (pj - (j == a ? 1.0f : 0.0f)) + pc.ent_coef * pj * (logpj + Hs);
+          }
+          g8[jj] = __float2half_rn(gj);
+        }
+        if (vec) {
+          *reinterpret_cast<uint4*>(drow + j0) = *reinterpret_cast<const uint4*>(g8);
+        } else {
+          for (int jj = 0; jj < 8 && j0 + jj < nA; ++jj) drow[j0 + jj] = g8[jj];
+        }
+      }
+    }
+    dv[b * ld_dv] = __float2half_rn(g_v);
+    st[0] = pgl; st[1] = vl; st[2] = H; st[3] = kl; st[4] = cf;
+  }
+  block_accumulate5(st, pc.stats);
+}
+
+// ---------------------------------------------------------------- Bernoulli (MultiBinary): loss + gradient
+// actions: float32 [*, n] rows of 0 / 1.  neglogp = sum_j sigmoid_xent(l_j, x_j), entropy = sum_j sigmoid_xent(l_j, p_j)
+// (distributions.py:120-125).  TF differentiates the entropy through its labels p = sigmoid(l) too, so
+//   d nlp/dl_j = p_j - x_j;  d(-ent_coef * H)/dl_j = ent_coef * l_j * p_j * (1 - p_j)   (total derivative)
+__global__ void __launch_bounds__(256)
+bern_loss_kernel(const float* __restrict__ logits, long long ld, int n, const float* __restrict__ vpred, long long ldv,
+                 const float* __restrict__ actions, PpoCommon pc, __half* __restrict__ dlogits, long long ld_dl,
+                 __half* __restrict__ dv, long long ld_dv, long long B) {
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  double st[5] = {0, 0, 0, 0, 0};
+  if (b < B) {
+    const long long s = pc.src_idx ? pc.src_idx[b] : b;
+    const float* l = logits + b * ld;
+    const float* x = actions + s * n;
+    float nlp = 0.0f, H = 0.0f;
+    for (int j = 0; j < n; ++j) {
+      const float lj = l[j];
+      nlp += sigmoid_xent(lj, x[j]);
+      H += sigmoid_xent(lj, sigmoidf(lj));
+    }
+    const float R = pc.returns[s], oldv = pc.old_values[s];
+    const float adv_raw = __fsub_rn(R, oldv);
+    const float adv = (float)(((double)adv_raw - pc.adv_stats[0]) / (pc.adv_stats[1] + 1e-8));
+    float pgl, kl, cf, vl;
+    const float clip = pc.cliprange_dev ? *pc.cliprange_dev : pc.cliprange;
+    const float g_nlp = pg_loss_grad(nlp, pc.old_neglogp[s], adv, clip, pgl, kl, cf);
+    const float g_v = value_loss_grad(vpred[b * ldv], oldv, R, clip, pc.vf_coef, vl);
+    __half* drow = dlogits + b * ld_dl;
+    const bool vec = ((ld_dl & 7) == 0) && ((reinterpret_cast<uintptr_t>(dlogits) & 15) == 0) && (((n + 7) & ~7) <= ld_dl);
+    for (int j0 = 0; j0 < n; j0 += 8) {
       __align__(16) __half g8[8];
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
         const int j = j0 + jj;
-        float g = 0.0f;
-        if (j < nA) {
-          const float a0 = l[j] - m;
-          const float pj = expf(a0) / z;
-          const float logpj = a0 - logz;
-          // d nlp/dl_j = p_j - 1{j=a};  d(-ent_coef*H)/dl_j = ent_coef * p_j * (log p_j + H)
-          g = g_nlp * (pj - (j == a ? 1.0f : 0.0f)) + pc.ent_coef * pj * (logpj + H);
+        float gj = 0.0f;
+        if (j < n) {
+          const float lj = l[j];
+          const float pj = sigmoidf(lj);
+          gj = g_nlp * (pj - x[j]) + pc.ent_coef * lj * pj * (1.0f - pj);
         }
-        g8[jj] = __float2half_rn(g);
+        g8[jj] = __float2half_rn(gj);
       }
       if (vec) {
         *reinterpret_cast<uint4*>(drow + j0) = *reinterpret_cast<const uint4*>(g8);
       } else {
-        for (int jj = 0; jj < 8 && j0 + jj < nA; ++jj) drow[j0 + jj] = g8[jj];
+        for (int jj = 0; jj < 8 && j0 + jj < n; ++jj) drow[j0 + jj] = g8[jj];
       }
     }
-    dv[b * ld_dv] = __float2half_rn(g_v);
+    dv[b * ld_dv] = __float2half_rn(g_v);             // after the logit stores: column n of the same row when fused
     st[0] = pgl; st[1] = vl; st[2] = H; st[3] = kl; st[4] = cf;
   }
   block_accumulate5(st, pc.stats);
@@ -396,13 +559,29 @@ gauss_loss_kernel(const float* __restrict__ mean, long long ld, const float* __r
 }
 
 // ---------------------------------------------------------------- launchers
-int cat_step_impl(const float* logits, long long ld, int nA, const float* vpred, long long ldv, const float* uniforms,
-                  unsigned long long seed, unsigned long long offset, const unsigned long long* offset_dev,
-                  long long* actions, float* values, float* neglogp, long long B, cudaStream_t stream) {
+int cat_step_impl(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
+                  long long ldv, const float* uniforms, unsigned long long seed, unsigned long long offset,
+                  const unsigned long long* offset_dev, long long* actions, float* values, float* neglogp, long long B,
+                  cudaStream_t stream) {
   B200RL_REQUIRE(logits && vpred && actions && values && neglogp && B > 0 && nA > 0, "cat_step: bad args");
-  cat_step_kernel<<<(int)ceil_div_ll(B, 256), 256, 0, stream>>>(logits, ld, nA, vpred, ldv, uniforms, seed, offset,
-                                                                 offset_dev, actions, values, neglogp, B);
+  B200RL_REQUIRE(seg_off == nullptr || (nseg >= 1 && nseg <= nA), "cat_step: a segment table needs 1 <= nseg <= nA");
+  const int grid = (int)ceil_div_ll(B, 256);
+  if (seg_off)
+    cat_step_kernel<true><<<grid, 256, 0, stream>>>(logits, ld, nA, seg_off, nseg, vpred, ldv, uniforms, seed, offset,
+                                                    offset_dev, actions, values, neglogp, B);
+  else
+    cat_step_kernel<false><<<grid, 256, 0, stream>>>(logits, ld, nA, nullptr, 1, vpred, ldv, uniforms, seed, offset,
+                                                     offset_dev, actions, values, neglogp, B);
   return check_launch("cat_step_kernel");
+}
+
+int bern_step_impl(const float* logits, long long ld, int n, const float* vpred, long long ldv, const float* uniforms,
+                   unsigned long long seed, unsigned long long offset, const unsigned long long* offset_dev,
+                   float* actions, float* values, float* neglogp, long long B, cudaStream_t stream) {
+  B200RL_REQUIRE(logits && vpred && actions && values && neglogp && B > 0 && n > 0, "bern_step: bad args");
+  bern_step_kernel<<<(int)ceil_div_ll(B, 256), 256, 0, stream>>>(logits, ld, n, vpred, ldv, uniforms, seed, offset,
+                                                                  offset_dev, actions, values, neglogp, B);
+  return check_launch("bern_step_kernel");
 }
 
 int gauss_step_impl(const float* mean, long long ld, const float* logstd, int d, const float* vpred, long long ldv,
@@ -423,19 +602,41 @@ int adv_stats_impl(const float* returns, const float* values, const long long* s
   return check_launch("adv_stats_kernel");
 }
 
-int cat_loss_impl(const float* logits, long long ld, int nA, const float* vpred, long long ldv,
-                  const long long* actions, const long long* src_idx, const float* returns, const float* old_values,
-                  const float* old_neglogp, const double* adv_stats, float cliprange, float ent_coef, float vf_coef,
-                  void* dlogits, long long ld_dl, void* dv, long long ld_dv, double* stats, long long B,
-                  const float* cliprange_dev, cudaStream_t stream) {
+int cat_loss_impl(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
+                  long long ldv, const long long* actions, const long long* src_idx, const float* returns,
+                  const float* old_values, const float* old_neglogp, const double* adv_stats, float cliprange,
+                  float ent_coef, float vf_coef, void* dlogits, long long ld_dl, void* dv, long long ld_dv,
+                  double* stats, long long B, const float* cliprange_dev, cudaStream_t stream) {
   B200RL_REQUIRE(logits && vpred && actions && returns && old_values && old_neglogp && adv_stats && dlogits && dv &&
-                     stats && B > 0,
+                     stats && B > 0 && nA > 0,
                  "cat_loss: bad args");
+  B200RL_REQUIRE(seg_off == nullptr || (nseg >= 1 && nseg <= nA), "cat_loss: a segment table needs 1 <= nseg <= nA");
   PpoCommon pc{src_idx, returns, old_values, old_neglogp, adv_stats, cliprange, ent_coef, vf_coef, stats, cliprange_dev};
-  cat_loss_kernel<<<(int)ceil_div_ll(B, 256), 256, 0, stream>>>(logits, ld, nA, vpred, ldv, actions, pc,
-                                                                 reinterpret_cast<__half*>(dlogits), ld_dl,
-                                                                 reinterpret_cast<__half*>(dv), ld_dv, B);
+  const int grid = (int)ceil_div_ll(B, 256);
+  if (seg_off)
+    cat_loss_kernel<true><<<grid, 256, 0, stream>>>(logits, ld, nA, seg_off, nseg, vpred, ldv, actions, pc,
+                                                    reinterpret_cast<__half*>(dlogits), ld_dl,
+                                                    reinterpret_cast<__half*>(dv), ld_dv, B);
+  else
+    cat_loss_kernel<false><<<grid, 256, 0, stream>>>(logits, ld, nA, nullptr, 1, vpred, ldv, actions, pc,
+                                                     reinterpret_cast<__half*>(dlogits), ld_dl,
+                                                     reinterpret_cast<__half*>(dv), ld_dv, B);
   return check_launch("cat_loss_kernel");
+}
+
+int bern_loss_impl(const float* logits, long long ld, int n, const float* vpred, long long ldv, const float* actions,
+                   const long long* src_idx, const float* returns, const float* old_values, const float* old_neglogp,
+                   const double* adv_stats, float cliprange, float ent_coef, float vf_coef, void* dlogits,
+                   long long ld_dl, void* dv, long long ld_dv, double* stats, long long B, const float* cliprange_dev,
+                   cudaStream_t stream) {
+  B200RL_REQUIRE(logits && vpred && actions && returns && old_values && old_neglogp && adv_stats && dlogits && dv &&
+                     stats && B > 0 && n > 0,
+                 "bern_loss: bad args");
+  PpoCommon pc{src_idx, returns, old_values, old_neglogp, adv_stats, cliprange, ent_coef, vf_coef, stats, cliprange_dev};
+  bern_loss_kernel<<<(int)ceil_div_ll(B, 256), 256, 0, stream>>>(logits, ld, n, vpred, ldv, actions, pc,
+                                                                  reinterpret_cast<__half*>(dlogits), ld_dl,
+                                                                  reinterpret_cast<__half*>(dv), ld_dv, B);
+  return check_launch("bern_loss_kernel");
 }
 
 int gauss_loss_impl(const float* mean, long long ld, const float* logstd, int d, const float* vpred, long long ldv,

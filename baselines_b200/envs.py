@@ -5,6 +5,7 @@ importable, cmd_util.make_env uses `gym.make` for ids that are not registered be
 reference's plumbing tests and the benchmark workload:
 
   DiscreteIdentity-v0 / BoxIdentity-v0   common/tests/envs/identity_env.py:7-90 (test_identity.py)
+  MultiDiscreteIdentity-v0               identity_env.py:62-74 with dims (3, 3) (test_identity.py:43-56)
   CartPole-v0 / CartPole-v1              classic cart-pole of common/tests/test_cartpole.py:14 (gym's dynamics: Barto,
                                          Sutton & Anderson 1983, Euler step, tau = 0.02)
   SyntheticAtari-v0                      84x84x1 uint8 frames, 6 actions: the bench.py workload as a steppable env
@@ -135,6 +136,17 @@ class DiscreteIdentityEnv(IdentityEnv):
         return 1 if state == actions else 0
 
 
+class MultiDiscreteIdentityEnv(IdentityEnv):
+    """identity_env.py:62-74: observation and action are MultiDiscrete(dims); reward 1 iff every component matches."""
+
+    def __init__(self, dims, episode_len=None, delay=0):
+        self.action_space = spaces.MultiDiscrete(dims)
+        super().__init__(episode_len=episode_len, delay=delay)
+
+    def _get_reward(self, state, actions):
+        return 1 if np.all(np.asarray(state) == np.asarray(actions)) else 0
+
+
 class BoxIdentityEnv(IdentityEnv):
     def __init__(self, shape, episode_len=None):
         self.action_space = spaces.Box(low=-1.0, high=1.0, shape=shape, dtype=np.float32)
@@ -210,6 +222,7 @@ class SyntheticAtariEnv(Env):
 
 
 register("DiscreteIdentity-v0", DiscreteIdentityEnv, "identity", dim=10, episode_len=100)
+register("MultiDiscreteIdentity-v0", MultiDiscreteIdentityEnv, "identity", dims=(3, 3), episode_len=100)
 register("BoxIdentity-v0", BoxIdentityEnv, "identity", shape=(1,), episode_len=100)
 register("CartPole-v0", CartPoleEnv, "classic_control", max_episode_steps=200)
 register("CartPole-v1", CartPoleEnv, "classic_control", max_episode_steps=500)

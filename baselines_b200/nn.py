@@ -346,7 +346,8 @@ class Tower:
     """A latent network (conv stack + fc, or mlp) with its activation workspace for `cap` samples."""
 
     def __init__(self, store, kind, ob_shape, prefix, tf_prefix, rng, cap, init="ortho", num_layers=2,
-                 num_hidden=64, convs=NATURE_CONVS, same_pad=False, fc_hidden=512, tf_style="a2c", onehot_n=0):
+                 num_hidden=64, convs=NATURE_CONVS, same_pad=False, fc_hidden=512, tf_style="a2c", onehot_n=0,
+                 onehot_nvec=None):
         self.kind, self.cap, self.store = kind, cap, store
         self.convs, self.fcs = [], []
         winit = (lambda shape, scale: ortho_init(shape, scale, rng)) if init == "ortho" else \
@@ -386,9 +387,15 @@ class Tower:
         elif kind == "mlp":
             self.in_u8 = False
             self.shift_mode = False
-            # Discrete(n) observations are one-hot encoded (common/input.py:54-55): raw rows hold the integer
-            self.onehot_n = int(onehot_n)
-            self.raw_dim = 1 if self.onehot_n else int(np.prod(ob_shape))
+            # Discrete(n) observations are one-hot encoded (common/input.py:54-55): raw rows hold the integer;
+            # MultiDiscrete(nvec) ones are the concatenated one-hots of their components (:58-61): raw rows hold the
+            # len(nvec) integers
+            self.onehot_nvec = None if onehot_nvec is None else [int(v) for v in onehot_nvec]
+            if self.onehot_nvec:
+                self.onehot_n, self.raw_dim = sum(self.onehot_nvec), len(self.onehot_nvec)
+            else:
+                self.onehot_n = int(onehot_n)
+                self.raw_dim = 1 if self.onehot_n else int(np.prod(ob_shape))
             nin = self.onehot_n if self.onehot_n else self.raw_dim
             self.in_dim, self.in_pad = nin, _pad8(nin)
             self.obs_norm = None                   # (mean, inv_std, lo, hi) float32 device tensors, policies.py:182-185
@@ -439,6 +446,7 @@ class Tower:
         self.ld_hfc = [l.Np for l in self.fcs]         # row pitch of hfc[i] / dzfc[i] (a fused first layer widens [0])
         if self.kind == "mlp":
             self.x0 = torch.zeros(cap, 2 * self.in_pad, **f16)      # [hi | lo] operand rows of the float32 observations
+            self.ob_seg = ops.segment_table(self.onehot_nvec, dev) if self.onehot_nvec else None
         # where the heads write d(loss)/d(latent pre-activation)
         if self.fcs:
             self.dlatent, self.ld_dlatent = self.dzfc[-1], self.fcs[-1].Np
@@ -569,7 +577,7 @@ class Tower:
         nm = self.obs_norm
         ops.obs_encode(x, self.x0, B, self.raw_dim, self.in_dim, self.in_pad, src_idx=src_idx,
                        mean=nm[0] if nm else None, inv_std=nm[1] if nm else None,
-                       clip=(nm[2], nm[3]) if nm else (0.0, 0.0), onehot_n=self.onehot_n)
+                       clip=(nm[2], nm[3]) if nm else (0.0, 0.0), onehot_n=self.onehot_n, seg_off=self.ob_seg)
         return self.x0
 
     def forward(self, x, B, src_idx=None, encoded=None, masks=True, skip_first=False):

@@ -205,14 +205,49 @@ def colsum(dz, db, rows, C, ld, alpha=1.0):
               label="colsum", nbytes=2.0 * rows * C)
 
 
+def segment_table(nvec, device):
+    """int32 device tensor [len(nvec) + 1] of the offsets of MultiDiscrete components in a row: 0, n0, n0 + n1, ...
+    (the seg_off argument of cat_step / cat_loss / obs_encode).  Every component needs at least one value
+    (distributions.py:79 asserts the same)."""
+    import numpy as np
+    nv = np.asarray(nvec, dtype=np.int64).reshape(-1)
+    if nv.size == 0 or np.any(nv < 1):
+        raise ValueError(f"MultiDiscrete nvec entries must be >= 1, got {list(nv)}")
+    off = np.concatenate([[0], np.cumsum(nv)]).astype(np.int32)
+    return torch.from_numpy(off).to(device)
+
+
+def _seg_args(seg_off):
+    if seg_off is None:
+        return None, 0
+    _chk(seg_off, torch.int32, "seg_off")
+    return _ptr(seg_off), seg_off.numel() - 1
+
+
 def cat_step(logits, ld, nA, vpred, ldv, actions, values, neglogp, B, uniforms=None, seed=0, offset=0,
-             offset_dev=None):
+             offset_dev=None, seg_off=None):
+    """Categorical sample + neglogp; with seg_off (segment_table(nvec), nA = sum(nvec)) one categorical per
+    MultiDiscrete component: actions int64 [B, len(nvec)], neglogp their sum."""
     _chk(logits, torch.float32, "logits")
     _chk(actions, torch.int64, "actions")
     _chk(uniforms, torch.float32, "uniforms")
     _chk(offset_dev, torch.int64, "offset_dev")
-    _lib.call("b200rl_cat_step", _ptr(logits), int(ld), int(nA), _ptr(vpred), int(ldv), _ptr(uniforms), int(seed),
-              int(offset), _ptr(offset_dev), _ptr(actions), _ptr(values), _ptr(neglogp), int(B), _stream())
+    so, nseg = _seg_args(seg_off)
+    _lib.call("b200rl_cat_step", _ptr(logits), int(ld), int(nA), so, nseg, _ptr(vpred), int(ldv), _ptr(uniforms),
+              int(seed), int(offset), _ptr(offset_dev), _ptr(actions), _ptr(values), _ptr(neglogp), int(B), _stream(),
+              **({} if so is None else dict(label="mcat_step", nbytes=float(B) * (4.0 * nA + 8.0 * nseg + 12.0))))
+
+
+def bern_step(logits, ld, n, vpred, ldv, actions, values, neglogp, B, uniforms=None, seed=0, offset=0,
+              offset_dev=None):
+    """Bernoulli (MultiBinary) sample + neglogp: actions float32 [B, n] of 0 / 1."""
+    _chk(logits, torch.float32, "logits")
+    _chk(actions, torch.float32, "actions")
+    _chk(uniforms, torch.float32, "uniforms")
+    _chk(offset_dev, torch.int64, "offset_dev")
+    _lib.call("b200rl_bern_step", _ptr(logits), int(ld), int(n), _ptr(vpred), int(ldv), _ptr(uniforms), int(seed),
+              int(offset), _ptr(offset_dev), _ptr(actions), _ptr(values), _ptr(neglogp), int(B), _stream(),
+              label="bern_step", nbytes=float(B) * (8.0 * n + 12.0))
 
 
 def gauss_step(mean, ld, logstd, d, vpred, ldv, actions, values, neglogp, B, normals=None, seed=0, offset=0,
@@ -251,13 +286,28 @@ def adv_stats(returns, values, src_idx, M, out):
 
 
 def cat_loss(logits, ld, nA, vpred, ldv, actions, src_idx, returns, old_values, old_neglogp, adv_st, cliprange,
-             ent_coef, vf_coef, dlogits, ld_dl, dv, ld_dv, stats, B, cliprange_dev=None):
+             ent_coef, vf_coef, dlogits, ld_dl, dv, ld_dv, stats, B, cliprange_dev=None, seg_off=None):
+    """Categorical PPO loss + logit gradient; with seg_off (segment_table(nvec)) the MultiCategorical one, actions
+    int64 [*, len(nvec)]."""
     _chk(actions, torch.int64, "actions")
     _chk(stats, torch.float64, "stats")
-    _lib.call("b200rl_cat_loss", _ptr(logits), int(ld), int(nA), _ptr(vpred), int(ldv), _ptr(actions), _ptr(src_idx),
+    so, nseg = _seg_args(seg_off)
+    _lib.call("b200rl_cat_loss", _ptr(logits), int(ld), int(nA), so, nseg, _ptr(vpred), int(ldv), _ptr(actions),
+              _ptr(src_idx), _ptr(returns), _ptr(old_values), _ptr(old_neglogp), _ptr(adv_st), float(cliprange),
+              float(ent_coef), float(vf_coef), _ptr(dlogits), int(ld_dl), _ptr(dv), int(ld_dv), _ptr(stats), int(B),
+              _ptr(cliprange_dev), _stream(),
+              **({} if so is None else dict(label="mcat_loss", nbytes=float(B) * (6.0 * nA + 8.0 * nseg + 28.0))))
+
+
+def bern_loss(logits, ld, n, vpred, ldv, actions, src_idx, returns, old_values, old_neglogp, adv_st, cliprange,
+              ent_coef, vf_coef, dlogits, ld_dl, dv, ld_dv, stats, B, cliprange_dev=None):
+    """Bernoulli (MultiBinary) PPO loss + logit gradient; actions float32 [*, n]."""
+    _chk(actions, torch.float32, "actions")
+    _chk(stats, torch.float64, "stats")
+    _lib.call("b200rl_bern_loss", _ptr(logits), int(ld), int(n), _ptr(vpred), int(ldv), _ptr(actions), _ptr(src_idx),
               _ptr(returns), _ptr(old_values), _ptr(old_neglogp), _ptr(adv_st), float(cliprange), float(ent_coef),
               float(vf_coef), _ptr(dlogits), int(ld_dl), _ptr(dv), int(ld_dv), _ptr(stats), int(B), _ptr(cliprange_dev),
-              _stream())
+              _stream(), label="bern_loss", nbytes=float(B) * (10.0 * n + 28.0))
 
 
 def gauss_loss(mean, ld, logstd, d, vpred, ldv, actions, src_idx, returns, old_values, old_neglogp, adv_st,
@@ -346,15 +396,18 @@ def cast_f32_f16(src, dst, rows, cols, ld_src, ld_dst, scale=1.0):
               float(scale), _stream())
 
 
-def obs_encode(x, out, B, raw_dim, in_dim, in_pad, src_idx=None, mean=None, inv_std=None, clip=(-5.0, 5.0), onehot_n=0):
-    """float32 observation rows -> fp16 [hi | lo] operand rows (input.py:43-63, policies.py:182-185, ppo2.py:165)."""
+def obs_encode(x, out, B, raw_dim, in_dim, in_pad, src_idx=None, mean=None, inv_std=None, clip=(-5.0, 5.0), onehot_n=0,
+               seg_off=None):
+    """float32 observation rows -> fp16 [hi | lo] operand rows (input.py:43-63, policies.py:182-185, ppo2.py:165).
+    onehot_n with seg_off (segment_table(nvec)): MultiDiscrete rows of len(nvec) integers -> concatenated one-hot."""
     _chk(x, torch.float32, "x")
     _chk(out, torch.float16, "out")
     _chk(src_idx, torch.int64, "src_idx")
     _chk(mean, torch.float32, "mean")
     _chk(inv_std, torch.float32, "inv_std")
+    so, nseg = _seg_args(seg_off)
     _lib.call("b200rl_obs_encode", _ptr(x), _ptr(src_idx), int(B), int(raw_dim), int(in_dim), int(in_pad), _ptr(mean),
-              _ptr(inv_std), float(clip[0]), float(clip[1]), int(onehot_n), _ptr(out), _stream(),
+              _ptr(inv_std), float(clip[0]), float(clip[1]), int(onehot_n), so, nseg, _ptr(out), _stream(),
               label="obs_encode", nbytes=float(B) * (4.0 * raw_dim + 4.0 * in_pad))
 
 

@@ -35,8 +35,7 @@ class Model(object):
             # ortho_init consumes the GLOBAL numpy stream seeded by set_global_seeds (ppo2.py:80), like the reference
             self.net = PolicyNet(policy, cap, self.device, rng=np.random)
             self.opt = _make_optimizer(self.net.store, max_grad_norm)
-            self._act_a = torch.zeros((nbatch_act,) if self.net.discrete else (nbatch_act, self.net.nout),
-                                      dtype=torch.int64 if self.net.discrete else torch.float32, device=self.device)
+            self._act_a = torch.zeros(self.net.action_shape(nbatch_act), dtype=self.net.action_dtype, device=self.device)
             self._act_v = torch.zeros(nbatch_act, dtype=torch.float32, device=self.device)
             self._act_nlp = torch.zeros(nbatch_act, dtype=torch.float32, device=self.device)
         self.loss_names = ['policy_loss', 'value_loss', 'policy_entropy', 'approxkl', 'clipfrac']   # model.py:115
@@ -83,7 +82,7 @@ class Model(object):
             a, v, n = self._bufs(B)
             nz = None if noise is None else torch.as_tensor(np.ascontiguousarray(noise), dtype=torch.float32).to(self.device)
             self.step_device(x, a, v, n, noise=nz)
-            return a.cpu().numpy(), v.cpu().numpy(), None, n.cpu().numpy()
+            return self.net.actions_to_numpy(a), v.cpu().numpy(), None, n.cpu().numpy()
 
     def value(self, ob, *args, **kwargs):
         with torch.cuda.device(self.device):
@@ -99,8 +98,7 @@ class Model(object):
         if B > self.net.cap:
             raise ValueError(f"batch {B} exceeds the workspace capacity {self.net.cap}")
         dev = self.device
-        a = torch.zeros((B,) if self.net.discrete else (B, self.net.nout),
-                        dtype=torch.int64 if self.net.discrete else torch.float32, device=dev)
+        a = torch.zeros(self.net.action_shape(B), dtype=self.net.action_dtype, device=dev)
         return a, torch.zeros(B, device=dev), torch.zeros(B, device=dev)
 
     # ------------------------------------------------------------------------------------ train path
@@ -181,10 +179,7 @@ class Model(object):
         with torch.cuda.device(self.device):
             dev = self.device
             x = self.net.encode_obs(np.asarray(obs))
-            if self.net.discrete:
-                a = torch.as_tensor(np.ascontiguousarray(actions), dtype=torch.int64).to(dev)
-            else:
-                a = torch.as_tensor(np.ascontiguousarray(actions), dtype=torch.float32).to(dev).contiguous()
+            a = torch.as_tensor(np.ascontiguousarray(actions), dtype=self.net.action_dtype).to(dev).contiguous()
             f = lambda z: torch.as_tensor(np.ascontiguousarray(z), dtype=torch.float32).to(dev)
             st = self.train_rollout(float(lr), float(cliprange), x, a, f(returns), f(values), f(neglogpacs), None)
             return [float(s) for s in st.cpu().numpy()]

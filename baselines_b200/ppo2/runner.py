@@ -18,7 +18,9 @@ class Rollout:
     """Time-major [T, N] rollout arrays in HBM.  Flat env-major index i = e*T + t (runner.py:69-74) maps to
     buffer offset t*N + e."""
 
-    def __init__(self, T, N, obs_store_shape, obs_dtype, discrete, act_dim, device):
+    def __init__(self, T, N, obs_store_shape, obs_dtype, discrete, act_dim, device, act_dtype=None):
+        """discrete: int64 [T, N] actions (Discrete); otherwise [T, N, act_dim] rows of act_dtype (float32 for Box and
+        MultiBinary, int64 for MultiDiscrete)."""
         self.T, self.N, self.device = T, N, device
         f32 = dict(dtype=torch.float32, device=device)
         self.obs = torch.zeros((T, N) + tuple(obs_store_shape), dtype=obs_dtype, device=device)
@@ -27,7 +29,7 @@ class Rollout:
         self.neglogpacs = torch.zeros(T, N, **f32)
         self.dones = torch.zeros(T, N, dtype=torch.uint8, device=device)        # done BEFORE step t (runner.py:34)
         self.actions = torch.zeros((T, N) if discrete else (T, N, act_dim),
-                                   dtype=torch.int64 if discrete else torch.float32, device=device)
+                                   dtype=torch.int64 if discrete else (act_dtype or torch.float32), device=device)
         self.advs = torch.zeros(T, N, **f32)
         self.returns = torch.zeros(T, N, **f32)
         self.last_values = torch.zeros(N, **f32)
@@ -76,8 +78,8 @@ class Runner:
         # vector observations are kept as the float32 the env produced (the reference never narrows them,
         # common/input.py:56-57); the encode kernel reads them through the minibatch indices
         store_shape = tuple(ob_space.shape) if self.u8 else (net.tower_pi.raw_dim,)
-        self.rollout = Rollout(nsteps, nenv, store_shape, torch.uint8 if self.u8 else torch.float32, net.discrete,
-                               net.nout, self.device)
+        self.rollout = Rollout(nsteps, nenv, store_shape, torch.uint8 if self.u8 else torch.float32, net.pd == "cat",
+                               net.act_dim, self.device, act_dtype=net.action_dtype)
         # pinned staging for the per-step host<->device traffic
         pin = torch.cuda.is_available()
         np_dtype = np.dtype(ob_space.dtype.name) if hasattr(ob_space.dtype, "name") else np.dtype(ob_space.dtype)
@@ -85,8 +87,7 @@ class Runner:
         if pin:
             self._obs_pin = self._obs_pin.pin_memory()
         self.obs = self._obs_pin.numpy()                                       # runners.py:10 self.obs
-        act_shape = (nenv,) if net.discrete else (nenv, net.nout)
-        self._act_pin = torch.zeros(act_shape, dtype=torch.int64 if net.discrete else torch.float32)
+        self._act_pin = torch.zeros(net.action_shape(nenv), dtype=net.action_dtype)
         self._rew_host = torch.zeros(nsteps, nenv, dtype=torch.float32)
         self._done_host = torch.zeros(nsteps, nenv, dtype=torch.uint8)
         if pin:
@@ -202,8 +203,8 @@ class Runner:
             self._f32_sync.record()
 
     def run_device(self, noise=None):
-        """Collect nsteps transitions; returns (Rollout, epinfos).  noise: optional [T, N, nA|d] float32 host
-        array of injected sampling noise (parity tests)."""
+        """Collect nsteps transitions; returns (Rollout, epinfos).  noise: optional [T, N, nout] float32 host
+        array of injected sampling noise (parity tests; nout = nA, sum(nvec), n or d)."""
         ro, model, T, N = self.rollout, self.model, self.nsteps, self.nenv
         epinfos = []
         with torch.cuda.device(self.device):
@@ -231,6 +232,8 @@ class Runner:
                 self._act_pin.copy_(ro.actions[t], non_blocking=True)
                 torch.cuda.current_stream().synchronize()
                 actions = self._act_pin.numpy()
+                if self.model.net.pd == "mcat":
+                    actions = actions.astype(np.int32)                      # distributions.py:222 tf.int32
                 if self.fs:
                     frames, rewards, self.dones, infos = self.env.step_frames(actions)
                     self.dones = np.asarray(self.dones, dtype=np.bool_)
@@ -275,5 +278,8 @@ class Runner:
             o = ro.obs.cpu().numpy().reshape((self.nsteps, self.nenv) + tuple(sp.shape))
             obs = o.swapaxes(0, 1).reshape(self.batch_ob_shape).astype(np.dtype(sp.dtype), copy=False)
         masks = ro.to_reference_numpy("dones").astype(np.bool_)
-        return (obs, ro.to_reference_numpy("returns"), masks, ro.to_reference_numpy("actions"),
+        actions = ro.to_reference_numpy("actions")
+        if self.model.net.pd == "mcat":
+            actions = actions.astype(np.int32)                              # distributions.py:222 tf.int32
+        return (obs, ro.to_reference_numpy("returns"), masks, actions,
                 ro.to_reference_numpy("values"), ro.to_reference_numpy("neglogpacs"), self.states, epinfos)

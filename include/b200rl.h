@@ -120,11 +120,21 @@ int b200rl_col2im(const void* dcols, const void* saved, void* dx, long long B, i
 int b200rl_colsum(const void* dz, float* db, long long rows, int C, long long ld, float alpha, void* stream);
 
 /* act path: PolicyWithValue.step common/policies.py:77-96; CategoricalPd.sample/neglogp
- * common/distributions.py:164-201; DiagGaussianPd :238-248.  noise == NULL -> counter-based Philox. */
-int b200rl_cat_step(const float* logits, long long ld, int nA, const float* vpred, long long ldv,
-                    const float* uniforms, unsigned long long seed, unsigned long long offset,
+ * common/distributions.py:164-201; DiagGaussianPd :238-248.  noise == NULL -> counter-based Philox, uniform j of
+ * row b = word j&3 of philox4(seed, b, j>>2, offset).
+ * cat_step also replaces MultiCategoricalPd.sample/neglogp (distributions.py:76-94,206-225): seg_off = device int32
+ * [nseg + 1] offsets of the components' logit blocks in the row (seg_off[nseg] == nA), actions = [B, nseg] indices
+ * inside each block, neglogp = the components' sum.  seg_off == NULL: one block [0, nA) (Discrete), actions [B]. */
+int b200rl_cat_step(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
+                    long long ldv, const float* uniforms, unsigned long long seed, unsigned long long offset,
                     const unsigned long long* offset_dev, long long* actions, float* values, float* neglogp,
                     long long B, void* stream);
+/* BernoulliPd.sample/neglogp (distributions.py:115-128,254-276): actions float32 [B, n] = (u < sigmoid(l)),
+ * neglogp = sum sigmoid_cross_entropy_with_logits(l, x). */
+int b200rl_bern_step(const float* logits, long long ld, int n, const float* vpred, long long ldv,
+                     const float* uniforms, unsigned long long seed, unsigned long long offset,
+                     const unsigned long long* offset_dev, float* actions, float* values, float* neglogp, long long B,
+                     void* stream);
 int b200rl_gauss_step(const float* mean, long long ld, const float* logstd, int d, const float* vpred,
                       long long ldv, const float* normals, unsigned long long seed, unsigned long long offset,
                       const unsigned long long* offset_dev, float* actions, float* values, float* neglogp,
@@ -145,12 +155,19 @@ int b200rl_adv_stats(const float* returns, const float* values, const long long*
                      void* stream);
 
 /* PPO2 loss + gradient w.r.t. head outputs: ppo2/model.py:57-91.  stats[5] += per-sample sums of
- * {pg_loss, vf_loss, entropy, approxkl, clipfrac} (model.py:115); gradients in "sum" scaling. */
-int b200rl_cat_loss(const float* logits, long long ld, int nA, const float* vpred, long long ldv,
-                    const long long* actions, const long long* src_idx, const float* returns,
+ * {pg_loss, vf_loss, entropy, approxkl, clipfrac} (model.py:115); gradients in "sum" scaling.
+ * cat_loss: Categorical (seg_off == NULL, actions [*]) or MultiCategorical (distributions.py:76-94; seg_off / nseg as
+ * for cat_step, actions [*, nseg]); bern_loss: Bernoulli (distributions.py:115-128, actions float32 [*, n]). */
+int b200rl_cat_loss(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
+                    long long ldv, const long long* actions, const long long* src_idx, const float* returns,
                     const float* old_values, const float* old_neglogp, const double* adv_stats, float cliprange,
                     float ent_coef, float vf_coef, void* dlogits, long long ld_dl, void* dv, long long ld_dv,
                     double* stats, long long B, const float* cliprange_dev, void* stream);
+int b200rl_bern_loss(const float* logits, long long ld, int n, const float* vpred, long long ldv,
+                     const float* actions, const long long* src_idx, const float* returns, const float* old_values,
+                     const float* old_neglogp, const double* adv_stats, float cliprange, float ent_coef,
+                     float vf_coef, void* dlogits, long long ld_dl, void* dv, long long ld_dv, double* stats,
+                     long long B, const float* cliprange_dev, void* stream);
 int b200rl_gauss_loss(const float* mean, long long ld, const float* logstd, int d, const float* vpred,
                       long long ldv, const float* actions, const long long* src_idx, const float* returns,
                       const float* old_values, const float* old_neglogp, const double* adv_stats, float cliprange,
@@ -182,10 +199,12 @@ int b200rl_cast_f32_f16(const float* src, void* dst, long long rows, int cols, l
  * clip((x - mean) / std, lo, hi) of common/policies.py:182-185, and the minibatch row gather of ppo2/ppo2.py:165.
  * x: float32 [*, raw_dim]; out: fp16 [B, 2*in_pad] = [hi | lo] with hi = fp16(v), lo = fp16(v - hi), so the first
  * GEMM (K = 2*in_pad against [W ; W]) sees the float32 observation to 2^-22 instead of an fp16-rounded copy.
- * onehot_n > 0: x holds the Discrete value (raw_dim = 1), out row = one_hot(x, n). */
+ * onehot_n > 0: x holds the Discrete value (raw_dim = 1), out row = one_hot(x, n).
+ * onehot_n > 0 with seg_off (device int32 [nseg + 1]): x holds a MultiDiscrete value (raw_dim = nseg integers), out
+ * row = concat_s one_hot(x[s], seg_off[s+1] - seg_off[s]) of width onehot_n = seg_off[nseg] (input.py:58-61). */
 int b200rl_obs_encode(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim, int in_pad,
-                      const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n, void* out,
-                      void* stream);
+                      const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n,
+                      const int* seg_off, int nseg, void* out, void* stream);
 
 /* prioritized replay: common/segment_tree.py:76-86 (__setitem__), :51-74 (reduce), :105-131
  * (find_prefixsum_idx); deepq/replay_buffer.py:107-115 (_sample_proportional), :157-165 (weights),
