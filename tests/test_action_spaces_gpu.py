@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import _action_oracle as ao
+import _loss_refs as lr
 from oracle import nets
 
 pytestmark = pytest.mark.gpu
@@ -30,50 +31,12 @@ def _dev(a, dt=None):
 HEADS = [("mcat", (1, 2, 3)), ("mcat", (3, 3)), ("mcat", (20, 30, 17)), ("bern", 5), ("bern", 33)]
 
 
-def _head_bufs(nout, B, fused):
-    """Device buffers in the two layouts PolicyNet uses: the fused [pi | vf] head (value in column nout of the logit
-    row, dv in column nout of the gradient row) and value_network='copy' (separate buffers)."""
-    if fused:
-        ld, ld_g = _pad(nout + 1, 16), _pad(nout + 1, 64)
-        ho = torch.zeros(B, ld, device="cuda")
-        g = torch.full((B, ld_g), float("nan"), dtype=torch.float16, device="cuda")
-        return ho, ld, ho[:, nout:], ld, g, ld_g, g[:, nout:], ld_g
-    ld = _pad(nout, 16)
-    return (torch.zeros(B, ld, device="cuda"), ld, torch.zeros(B, 16, device="cuda"), 16,
-            torch.full((B, _pad(nout, 64)), float("nan"), dtype=torch.float16, device="cuda"), _pad(nout, 64),
-            torch.zeros(B, 64, dtype=torch.float16, device="cuda"), 64)
-
-
 def _seg_entropies(l64, nvec):
     out = []
     for blk in torch.split(l64, list(nvec), dim=1):
         lp = torch.log_softmax(blk, 1)
         out.append(-(lp.exp() * lp).sum(1))
     return torch.stack(out, 1)
-
-
-def _ref_loss_grad(pd, arg, l32, v32, acts, R, oldv, oldnlp, adv, clip, ent_coef, vf_coef, drop_last_entropy=False):
-    """float64 per-row PPO loss (sum scaling) of ppo2/model.py:57-91 and its gradients w.r.t. logits and value."""
-    nvec = arg if pd == "mcat" else None
-    l = torch.tensor(l32, dtype=torch.float64, requires_grad=True)
-    v = torch.tensor(v32, dtype=torch.float64, requires_grad=True)
-    a = torch.as_tensor(acts)
-    nlp = ao.neglogp(pd, l, None, a.double() if pd == "bern" else a, nvec)
-    if drop_last_entropy:
-        H = _seg_entropies(l, nvec)[:, :-1].sum(1)
-    else:
-        H = ao.entropy(pd, l, None, nvec)
-    R, oldv, oldnlp, adv = (torch.tensor(x, dtype=torch.float64) for x in (R, oldv, oldnlp, adv))
-    ratio = torch.exp(oldnlp - nlp)
-    pg = torch.maximum(-adv * ratio, -adv * torch.clamp(ratio, 1 - clip, 1 + clip))
-    vcl = oldv + torch.clamp(v - oldv, -clip, clip)
-    vl = 0.5 * torch.maximum((v - R) ** 2, (vcl - R) ** 2)
-    loss = (pg - ent_coef * H + vf_coef * vl).sum()
-    gl, gv = torch.autograd.grad(loss, [l, v])
-    kl = 0.5 * (nlp - oldnlp) ** 2
-    cf = ((ratio - 1).abs() > clip).double()
-    stats = [float(x.sum()) for x in (pg, vl, H, kl, cf)]
-    return gl.detach().numpy(), gv.detach().numpy(), stats, nlp.detach().numpy()
 
 
 def _within_fp16(got, ref):
@@ -91,7 +54,8 @@ def test_head_kernels_vs_float64_autograd(pd, arg, gather, fused):
     nout = sum(nvec) if pd == "mcat" else arg
     k = len(nvec) if pd == "mcat" else arg
     seg = ops.segment_table(nvec, "cuda") if pd == "mcat" else None
-    lo, ld, vo, ldv, g, ld_g, dv, ld_dv = _head_bufs(nout, B, fused)
+    hb = lr.head_bufs(nout, B, "fused" if fused else "copy")
+    lo, ld, vo, ldv, g, ld_g, dv, ld_dv = hb.ho, hb.ld, hb.vo, hb.ldv, hb.g, hb.ld_g, hb.dv, hb.ld_dv
     l32 = (rng.randn(B, nout) * 1.5).astype(np.float32)
     v32 = rng.randn(B).astype(np.float32)
     lo[:, :nout] = _dev(l32)
@@ -137,8 +101,8 @@ def test_head_kernels_vs_float64_autograd(pd, arg, gather, fused):
     acts_buf = np.stack([rng.randint(0, n, Bbuf) for n in nvec], 1) if pd == "mcat" else \
         (rng.rand(Bbuf, k) < 0.5).astype(np.float32)
     acts = acts_buf[src]
-    nlp_cur = _ref_loss_grad(pd, arg, l32, v32, acts, np.zeros(B), np.zeros(B), np.zeros(B), np.zeros(B), 0.2,
-                             0.0, 0.0)[3]
+    nlp_cur = lr.ppo_ref(pd, l32, v32, acts, np.zeros(B), np.zeros(B), np.zeros(B), np.zeros(B), 0.2, 0.0, 0.0,
+                         nvec=nvec).nlp
     oldnlp_buf = rng.randn(Bbuf).astype(np.float32)
     oldnlp_buf[src] = (nlp_cur + rng.randn(B) * 0.1).astype(np.float32)
     oldv_buf = (rng.randn(Bbuf)).astype(np.float32)
@@ -158,7 +122,8 @@ def test_head_kernels_vs_float64_autograd(pd, arg, gather, fused):
     mean, std = adv_st.cpu().numpy()
     R, oldv, oldnlp = R_buf[src], oldv_buf[src], oldnlp_buf[src]
     adv = (((R - oldv).astype(np.float64) - mean) / (std + 1e-8)).astype(np.float32)
-    gl, gv, st, _ = _ref_loss_grad(pd, arg, l32, v32, acts, R, oldv, oldnlp, adv, clip, ent_coef, vf_coef)
+    ref = lr.ppo_ref(pd, l32, v32, acts, R, oldv, oldnlp, adv, clip, ent_coef, vf_coef, nvec=nvec)
+    gl, gv, st = ref.dhead, ref.dv, ref.stats
     got_g = g[:, :nout].float().cpu().numpy()
     ok = _within_fp16(got_g, gl)
     assert ok.all(), (np.argwhere(~ok)[:5], float(np.abs(got_g - gl).max()))
@@ -177,8 +142,8 @@ def test_head_kernels_vs_float64_autograd(pd, arg, gather, fused):
         H_col = np.repeat(Hs, nvec, axis=1)
         wrong_total = gl + ent_coef * p * (Hs.sum(1, keepdims=True) - H_col)    # total H in place of H_s
         assert not _within_fp16(got_g, wrong_total).all()
-        wrong_drop = _ref_loss_grad(pd, arg, l32, v32, acts, R, oldv, oldnlp, adv, clip, ent_coef, vf_coef,
-                                    drop_last_entropy=True)[0]
+        wrong_drop = lr.ppo_ref(pd, l32, v32, acts, R, oldv, oldnlp, adv, clip, ent_coef, vf_coef, nvec=nvec,
+                                mutant="drop_last_entropy").dhead
         assert not _within_fp16(got_g, wrong_drop).all()
 
 

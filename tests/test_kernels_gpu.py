@@ -63,7 +63,8 @@ def test_gae_bit_exact_vs_reference_golden(ops, name):
             assert np.array_equal(sf01(ret), g[f"returns{k}"]), (name, variant)
 
 
-@pytest.mark.parametrize("T,N", [(128, 4096), (37, 96), (512, 1024), (5, 7)])
+@pytest.mark.parametrize("T,N", [(128, 4096), (37, 96), (512, 1024), (5, 7),
+                                 (161, 64), (33, 32)])          # T % 32 != 0: the partial chunk comes first
 def test_gae_bit_exact_vs_oracle_random(ops, T, N):
     from oracle.gae import gae_reference_order
     rng = np.random.RandomState(T * 1000 + N)
