@@ -13,11 +13,17 @@
 //                                       (a CTA keeps the accumulators of up to 2*QW taps x 64 channels in registers;
 //                                        X and dY are read once per such group of taps)
 //
-// Warp roles: warps 0-7 are two consumer warpgroups (rows [64g, 64g+64) of every 128-row tile; they issue the
-// wgmma.mma_async chains, and run the epilogue -- or, in the wgrad, the fused bias-gradient sums -- from their own
-// registers) | warp 8 TMA loads | uint8-fed first layer only: warps 9-16 are uint8 producers that cast raw frames
-// into a rolling A ring instead of the TMA.  The forward epilogue can also write 1 bit per output element (act > 0);
-// the dgrad of the next layer reads that instead of the fp16 activation.
+// Warp roles: warps 0-7 are two consumer warpgroups (they issue the wgmma.mma_async chains, and run the epilogue --
+// or, in the wgrad, the fused bias-gradient sums -- from their own registers) | warp 8 TMA loads | uint8-fed first
+// layer only: warps 9-16 are uint8 producers that cast raw frames into a rolling A ring instead of the TMA.  The
+// forward epilogue can also write 1 bit per output element (act > 0); the dgrad of the next layer reads that instead
+// of the fp16 activation.
+//
+// "Ping-pong" schedule of the forward / dgrad: the two consumer warpgroups take whole 128-row tiles (even / odd) and
+// turns on the tensor cores.  Named barriers 2 and 3 order their MMA issue: a group issues its next tile only after
+// the other group has issued the previous one.  The tiles' MMAs therefore retire in order, and each group's epilogue
+// runs while the tensor cores work on the other group's tile.  (Cooperative schedule, where ping-pong does not pay:
+// each group takes 64 rows of every tile.)
 //
 // Outputs at grid positions that are not valid conv outputs are computed from wrapped rows and discarded (fwd),
 // or multiply a zero of the zero-bordered dY (wgrad / dgrad) -- so dY tensors live on the conv's INPUT grid.
@@ -38,13 +44,33 @@ static constexpr int SH_MAX_TAPS = 16;
 // halves per stage): span <= 16, so that four stages fit beside the weights.
 __host__ __device__ constexpr int sh_arows(int KH) { return KH == 1 ? 160 : 144; }
 __host__ __device__ constexpr int sh_stages(int KH) { return KH == 1 ? 6 : 4; }
+// uint8-fed first layer: its weights (N = 32, <= 4 taps) need 16 KB, so the rolling ring takes 12 tiles.  Both consumer
+// groups hold a tile (+ the next tile's head unit) under ping-pong; the deeper ring keeps the producer warps' loads
+// running ahead of them.
+static constexpr int SH_U8_STAGES = 12;
+static constexpr int SH_U8_WRES_BYTES = 16 * 1024;
 __host__ __device__ constexpr int sh_wgrad_krows(bool u8) { return u8 ? 128 : 64; }   // wgrad: reduction rows per stage
-// resident-weight region of the forward kernel (all taps): 80 KB beside 64-channel stages, 64 KB beside 128-channel ones
-__host__ __device__ constexpr int sh_wres_bytes(int KH) { return KH == 1 ? 80 * 1024 : 64 * 1024; }
+// resident-weight region of the forward kernel (all taps): 80 KB beside 64-channel stages, 64 KB beside 128-channel
+// ones, 16 KB beside the uint8 ring
+__host__ __device__ constexpr int sh_wres_bytes(int KH, bool u8) {
+  return u8 ? SH_U8_WRES_BYTES : KH == 1 ? 80 * 1024 : 64 * 1024;
+}
+static constexpr int SH_BAR_BYTES = 512;             // forward kernel: mbarrier block after the weights
 static constexpr int SH_WROWS_K = 96;                // wgrad: 64 + max shift span (<= 32)
 static constexpr int SH_WABYTES = SH_WROWS_K * 128;
 // wgrad: 64-channel accumulator chunks per consumer warpgroup (2 * QW * N/2 registers per thread)
 __host__ __device__ constexpr int sh_wgrad_qw(int BN, bool u8) { return u8 ? 2 : (BN == 64 ? 2 : 4); }
+
+// Ordered MMA issue of the two consumer warpgroups (barrier 0 is __syncthreads, 1 joins the consumer warps in the
+// wgrad).  Group g waits on barrier SH_ORDER_BAR + g for its turn and hands the turn over with an arrive on the other
+// group's barrier: every wait is matched by exactly one arrive, so neither group may skip one while the other waits.
+static constexpr int SH_ORDER_BAR = 2;
+__device__ __forceinline__ void order_wait(int wg) {
+  asm volatile("bar.sync %0, %1;" ::"r"(SH_ORDER_BAR + wg), "n"(SH_CONSUMER_WARPS * 32) : "memory");
+}
+__device__ __forceinline__ void order_pass(int wg) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(SH_ORDER_BAR + 1 - wg), "n"(SH_CONSUMER_WARPS * 32) : "memory");
+}
 
 // address map of an output / saved tensor: grid position (n, y, x) + column -> element offset
 struct AddrMap {
@@ -137,7 +163,8 @@ __device__ __forceinline__ void u8x16_to_f16(const uint4& q, uint4& lo, uint4& h
 // belongs to tile u / UPT, and the units are dealt round-robin to the U8_WARPS producer warps.  Each warp keeps
 // D units of loads in flight in registers (the sample index of the gather is looked up one round earlier).
 // Barriers per stage: full (UPT unit arrivals [+ the TMA of the other operand]), head (the first unit alone: the
-// tile in the PREVIOUS stage waits for it), empty (every consumer warp, once the tile's MMAs retired).
+// tile in the PREVIOUS stage waits for it), empty (8 consumer warp arrivals: a stage may be refilled only once its own
+// tile AND the tile of the previous stage, which read its first unit, have retired -- see the kernels).
 
 __device__ __forceinline__ uint4 ldg_stream_v4(const void* p) {
   uint4 v;
@@ -268,19 +295,26 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
                       const __grid_constant__ ShiftParams p) {
   constexpr int SH_ABYTES = sh_arows(KH) * 128;      // one 64-channel half of an A stage
   constexpr int STAGE_BYTES = KH * SH_ABYTES;
-  constexpr int STAGES = sh_stages(KH);
+  constexpr int STAGES = U8 ? SH_U8_STAGES : sh_stages(KH);
   using Ring = U8Ring<SH_BM, STAGES>;                // uint8-fed first layer: rolling ring instead of per-tile stages
+  // Ping-pong (whole tiles per group) or cooperative schedule (both groups on every tile, 64 rows each).  Ping-pong
+  // needs 2 * BN/2 accumulator registers per thread.  The 9 warps get at most 168 registers each (3 warps share one
+  // SM sub-partition's register file), and BN = 128 with the bias / bit-mask epilogue would spill: that instance
+  // keeps the cooperative schedule.
+  constexpr bool PINGPONG = !(BN == 128 && !DACT);
+  constexpr int MH = PINGPONG ? 2 : 1;               // m64 accumulators per thread
+  static_assert(PINGPONG || !U8, "the uint8 ring's release rule assumes ping-pong");
   constexpr int A_PITCH = U8 ? SH_BM * 128 : STAGE_BYTES;
   constexpr int A_TOTAL = U8 ? Ring::BYTES : STAGES * STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* wres = smem + A_TOTAL;                    // resident weights: taps*KH sub-tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(wres + sh_wres_bytes(KH));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(wres + sh_wres_bytes(KH, U8));
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
   uint64_t* w_bar = bars + 2 * STAGES;
   uint64_t* head_bar = bars + 2 * STAGES + 1;        // U8: first unit of the stage's tile is in place
-  static_assert((3 * STAGES + 1) * 8 <= 256, "barrier block");
+  static_assert((3 * STAGES + 1) * 8 <= SH_BAR_BYTES, "barrier block");
 
   __shared__ float s_bias[BN];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -289,12 +323,17 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], U8 ? Ring::UPT : 1);
-      // ring: a tile also reads the first unit of the next stage; the consumers finish tiles in order, so the next
-      // stage's own tile releasing it implies this one is done too
-      mbar_init(&empty_bar[s], SH_CONSUMER_WARPS);
+      // TMA-fed: a stage holds its own halo rows and is released by the 4 warps of the group that owns its tile (both
+      // groups' 8 warps without ping-pong).  Ring: a tile also reads the first unit of the next stage, and the two
+      // tiles belong to different groups, so a stage is released by 8 arrivals: 4 from its own tile and 4 from the
+      // tile of the previous stage
+      mbar_init(&empty_bar[s], (U8 || !PINGPONG) ? SH_CONSUMER_WARPS : 4);
       if (U8) mbar_init(&head_bar[s], 1);
     }
     mbar_init(w_bar, 1);
+    // the CTA's first tile has no predecessor to release the first fill of stage 0 as a head reader: arrive for it
+    if (U8)
+      for (int w = 0; w < 4; ++w) mbar_arrive(&empty_bar[0]);
     fence_barrier_init();
   }
   __syncthreads();
@@ -343,25 +382,28 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
     u8_ring_producer<SH_BM, STAGES, 2>(p.u8, p.M, (long long)tile_first * SH_BM + p.min_shift, tile_count, smem,
                                        full_bar, head_bar, empty_bar, warp - (SH_TMA_WARP + 1), lane);
   } else {
-    // consumer warpgroup wg: tile rows [64*wg, 64*wg + 64); thread t holds rows r0 and r0 + 8 of its accumulator
-    const int wg = warp >> 2, t = threadIdx.x & 127;
-    const int r0 = wg * 64 + acc_row(t, 0);
+    // consumer warpgroup wg: ping-pong: the CTA's tiles i = wg, wg + 2, ... whole, as two m64 accumulators (tile rows
+    // [0, 64) and [64, 128)); cooperative: rows [64*wg, 64*wg + 64) of every tile.  Thread t holds rows r0 and r0 + 8
+    // of each accumulator.  (wg is broadcast: the compiler then knows the tile loop is warp-uniform and keeps the
+    // wgmma chain asynchronous.)
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), t = threadIdx.x & 127;
+    const int row0 = PINGPONG ? 0 : wg * 64, r0 = row0 + acc_row(t, 0);
     const uint32_t w_base = smem_u32(wres);
     const float lo = (p.act == ACT_RELU) ? 0.0f : -INFINITY;
     const __half2 lo2 = __floats2half2_rn(lo, lo);
     const __half2 zero2 = __floats2half2_rn(0.0f, 0.0f);
-    float acc[BN / 2];
-    int s = 0;
-    uint32_t ph = 0;
+    float acc[MH][BN / 2];
     mbar_wait(w_bar, 0);
-    for (int i = 0; i < tile_count; ++i) {
+    for (int i = PINGPONG ? wg : 0; i < tile_count; i += PINGPONG ? 2 : 1) {
       const int tile = tile_first + i * tile_stride;
-      const int s1 = (s + 1 == STAGES) ? 0 : s + 1;
+      const int s = i % STAGES, s1 = (s + 1 == STAGES) ? 0 : s + 1;
+      const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
       mbar_wait(&full_bar[s], ph);
       if (U8) mbar_wait(&head_bar[s1], s1 == 0 ? ph ^ 1 : ph);   // the shifted taps read into the next tile's first unit
-      const uint32_t a_base = smem_u32(smem + s * A_PITCH) + (uint32_t)(wg * 64 * 128);
+      if (PINGPONG && i > 0) order_wait(wg);                      // the other group has issued tile i - 1
+      const uint32_t a_base = smem_u32(smem + s * A_PITCH) + (uint32_t)(row0 * 128);
       wgmma_fence();
-      // tap 0 overwrites the accumulator with its first MMA; the others accumulate
+      // tap 0 overwrites the accumulators with its first MMA; the others accumulate
 #pragma unroll 1
       for (int a = 0; a < p.taps; ++a) {
 #pragma unroll 1
@@ -372,21 +414,29 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
           for (int h = 0; h < KH; ++h) {
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-              const uint64_t adesc = make_sdesc(at + h * SH_ABYTES + k * 32, 16, 1024, 1);
               const uint64_t bdesc = make_sdesc(wt + h * w_sub + k * 32, 16, 1024, 1);
-              wgmma_f16<BN, 0, 0>(acc, adesc, bdesc, (a | b | h | k) ? 1u : 0u);
+#pragma unroll
+              for (int mh = 0; mh < MH; ++mh) {
+                const uint64_t adesc = make_sdesc(at + mh * 64 * 128 + h * SH_ABYTES + k * 32, 16, 1024, 1);
+                wgmma_f16<BN, 0, 0>(acc[mh], adesc, bdesc, (a | b | h | k) ? 1u : 0u);
+              }
             }
           }
         }
       }
       wgmma_commit();
+      if (PINGPONG && i + 1 < tile_count) order_pass(wg);         // the other group may issue tile i + 1
       wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[s]);
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if (U8) mbar_arrive(&empty_bar[s1]);                      // the head unit this tile read
+      }
 
 #pragma unroll
-      for (int hr = 0; hr < 2; ++hr) {
-        const uint32_t m = (uint32_t)tile * SH_BM + r0 + 8 * hr;         // M < 2^31 (checked on the host)
+      for (int q = 0; q < 2 * MH; ++q) {                              // accumulator mh, its row r0 + 8 * hr
+        const int mh = q >> 1, hr = q & 1;
+        const uint32_t m = (uint32_t)tile * SH_BM + mh * 64 + r0 + 8 * hr;   // M < 2^31 (checked on the host)
         const uint32_t t2 = p.fwg.div(m);
         const int x = (int)(m - t2 * (uint32_t)p.Wg);
         const int n = (int)p.fhg.div(t2);
@@ -398,7 +448,10 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 #pragma unroll
         for (int j = 0; j < BN / 16; ++j) {                  // 16-column chunks: two 8-column accumulator blocks
           uint32_t mw = 0xffffu;                              // activation-derivative bits of the chunk (DACT)
-          if (masked && p.saved_bits != nullptr) mw = __ldg(p.saved_bits + ((sbase + map_coloff(p.smap, 16 * j)) >> 4));
+          // a 16-column chunk never straddles a class of the maps: column 16 * j + cc lies at coloff(16 * j) + cc
+          const long long ocol = map_coloff(p.omap, 16 * j);
+          const long long scol = DACT ? map_coloff(p.smap, 16 * j) : 0;
+          if (masked && p.saved_bits != nullptr) mw = __ldg(p.saved_bits + ((sbase + scol) >> 4));
           uint32_t bits = 0;
 #pragma unroll
           for (int jj = 0; jj < 2; ++jj) {
@@ -409,26 +462,27 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
             if (DACT) {
               uint32_t mb = mw >> cc;
               if (masked && p.saved_bits == nullptr) {
-                const float2 h = __half22float2(*reinterpret_cast<const __half2*>(p.saved + sbase + map_coloff(p.smap, c)));
+                const float2 h = __half22float2(*reinterpret_cast<const __half2*>(p.saved + sbase + scol + cc));
                 mb = (h.x > lo ? 1u : 0u) | (h.y > lo ? 2u : 0u);
               }
-              o = __floats2half2_rn((mb & 1u) ? acc[e] * p.alpha : 0.0f, (mb & 2u) ? acc[e + 1] * p.alpha : 0.0f);
+              o = __floats2half2_rn((mb & 1u) ? acc[mh][e] * p.alpha : 0.0f,
+                                    (mb & 2u) ? acc[mh][e + 1] * p.alpha : 0.0f);
             } else {                                          // relu after the rounding: same result, one packed max
-              o = __hmax2(__floats2half2_rn(fmaf(acc[e], p.alpha, s_bias[c]), fmaf(acc[e + 1], p.alpha, s_bias[c + 1])),
+              o = __hmax2(__floats2half2_rn(fmaf(acc[mh][e], p.alpha, s_bias[c]),
+                                            fmaf(acc[mh][e + 1], p.alpha, s_bias[c + 1])),
                           lo2);
               const uint32_t gt = __hgt2_mask(o, zero2);
               bits |= ((gt & 1u) | ((gt >> 15) & 2u)) << cc;
             }
-            if (ok) *reinterpret_cast<__half2*>(p.out + obase + map_coloff(p.omap, c)) = o;
+            if (ok) *reinterpret_cast<__half2*>(p.out + obase + ocol + cc) = o;
           }
           if (!DACT && p.bits_out != nullptr) {               // the four lanes of a row assemble the chunk's 16 bits
             bits |= __shfl_xor_sync(0xffffffffu, bits, 1);
             bits |= __shfl_xor_sync(0xffffffffu, bits, 2);
-            if (ok && (t & 3) == 0) p.bits_out[(obase + map_coloff(p.omap, 16 * j)) >> 4] = (uint16_t)bits;
+            if (ok && (t & 3) == 0) p.bits_out[(obase + ocol) >> 4] = (uint16_t)bits;
           }
         }
       }
-      if (++s == STAGES) { s = 0; ph ^= 1; }
     }
   }
 }
@@ -489,7 +543,9 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], U8 ? 1 + Ring::UPT : 1);
-      mbar_init(&empty_bar[s], SH_CONSUMER_WARPS);   // ring: see the forward kernel
+      // ring: a k-block also reads the first unit of the next stage; both groups finish k-blocks in order, so the
+      // next stage's own k-block releasing it implies this one is done too
+      mbar_init(&empty_bar[s], SH_CONSUMER_WARPS);
       if (U8) mbar_init(&head_bar[s], 1);
     }
     fence_barrier_init();
@@ -641,8 +697,9 @@ static U8Src make_u8src(const void* x, const long long* idx, int H, int W, int C
 
 template <int BN, int KH, bool DACT, bool U8 = false>
 static int launch_fwd(const CUtensorMap& tmX, const CUtensorMap& tmW, const ShiftParams& p, cudaStream_t st) {
-  constexpr int STAGES = sh_stages(KH);
-  constexpr int SMEM = (U8 ? U8Ring<SH_BM, STAGES>::BYTES : STAGES * KH * sh_arows(KH) * 128) + sh_wres_bytes(KH) + 1024 + 256;
+  constexpr int STAGES = U8 ? SH_U8_STAGES : sh_stages(KH);
+  constexpr int SMEM = (U8 ? U8Ring<SH_BM, STAGES>::BYTES : STAGES * KH * sh_arows(KH) * 128) + sh_wres_bytes(KH, U8) +
+                       1024 + SH_BAR_BYTES;
   static_assert(SMEM + 1024 <= 227 * 1024, "conv_shift_fwd: shared memory budget (+ static bias array)");
   static bool attr = false;
   auto kern = conv_shift_fwd_kernel<BN, KH, DACT, U8>;
@@ -712,7 +769,7 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
   B200RL_REQUIRE(C == 64 || C == 128, "conv_shift_fwd: C must be 64 or 128 (got %d)", C);
   B200RL_REQUIRE(N == 32 || N == 64 || N == 128, "conv_shift_fwd: N must be 32, 64 or 128 (got %d)", N);
   B200RL_REQUIRE(taps >= 1 && taps <= SH_MAX_TAPS, "conv_shift_fwd: 1..%d taps", SH_MAX_TAPS);
-  B200RL_REQUIRE((C == 64 || C == 128) && (long long)taps * (C / 64) * kx * N * 128 <= sh_wres_bytes(C / 64),
+  B200RL_REQUIRE((C == 64 || C == 128) && (long long)taps * (C / 64) * kx * N * 128 <= sh_wres_bytes(C / 64, u8_x != nullptr),
                  "conv_shift_fwd: weights do not fit in smem");
   ShiftParams p = {};
   int lo = shifts[0], hi = shifts[0];
