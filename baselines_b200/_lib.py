@@ -15,8 +15,8 @@ _p, _i, _ll, _f, _d, _ull = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_do
 SIGNATURES = {
     "b200rl_gae_scan": [_p, _p, _p, _p, _p, _p, _p, _i, _i, _d, _d, _i, _p],
     "b200rl_gemm_f16": [_p, _p, _p, _p, _p, _i, _i, _i, _ll, _ll, _ll, _ll, _i, _i, _i, _f, _i, _i, _i, _i, _i, _p, _p],
-    "b200rl_conv_shift_fwd": [_p, _ll, _i, _i, _i, _p, _ll, _i, _i, _p, _i, _i, _p, _p, _p, _p, _p, _i, _i, _f,
-                              _p, _p, _i, _i, _i, _i, _p, _p, _i, _p],
+    "b200rl_conv_shift_fwd": [_p, _ll, _i, _i, _i, _p, _ll, _i, _i, _p, _i, _i, _p, _p, _p, _p, _i, _i, _f,
+                              _p, _p, _i, _i, _i, _i, _p, _p, _p],
     "b200rl_conv_shift_wgrad": [_p, _ll, _i, _p, _i, _i, _p, _p, _ll, _f, _p, _f, _i, _p, _p, _i, _i, _i, _i, _i, _p],
     "b200rl_conv_gemm": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _p, _ll, _p, _p, _ll, _i, _i, _i,
                          _i, _f, _i, _i, _i, _i, _i, _p],

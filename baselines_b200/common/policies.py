@@ -152,10 +152,9 @@ class PolicyNet:
         # parameters (checkpoint names / layouts unchanged); their fp16 forward operands, outputs and output gradients
         # are the two halves of shared buffers.
         tp, tv = self.tower_pi, self.tower_vf
-        import os
-        self.fuse0 = bool(tv is not None and tp.kind == "mlp" and os.environ.get("B200RL_NO_FUSE_FC0", "0") != "1" and
-                          tp.fcs[0].N == tv.fcs[0].N and tp.fcs[0].K == tv.fcs[0].K and
-                          tp.fcs[0].act == tv.fcs[0].act and 2 * tp.fcs[0].N in (64, 128, 256))
+        self.fuse0 = bool(tv is not None and tp.kind == "mlp" and tp.fcs[0].N == tv.fcs[0].N and
+                          tp.fcs[0].K == tv.fcs[0].K and tp.fcs[0].act == tv.fcs[0].act and
+                          2 * tp.fcs[0].N in (64, 128, 256))
         if self.fuse0:
             a, b = tp.fcs[0], tv.fcs[0]
             N = a.N

@@ -19,8 +19,8 @@ void set_last_error(const char* fmt, ...) {
 int gemm_f16_impl(const void*, const void*, void*, const float*, const void*, int, int, int, long long, long long,
                   long long, long long, int, int, int, float, int, int, int, int, int, const void*, cudaStream_t);
 int conv_shift_fwd_impl(const void*, long long, int, int, int, const void*, long long, int, int, const int*, int, int,
-                        void*, const long long*, const void*, const long long*, const float*, int, int, float,
-                        const void*, const long long*, int, int, int, int, void*, const void*, int, cudaStream_t);
+                        void*, const long long*, const long long*, const float*, int, int, float,
+                        const void*, const long long*, int, int, int, int, void*, const void*, cudaStream_t);
 int conv_shift_wgrad_impl(const void*, long long, int, const void*, int, int, const int*, float*, long long, float,
                           float*, float, int, const void*, const long long*, int, int, int, int, int, cudaStream_t);
 int conv_gemm_impl(const void*, long long, int, int, int, int, int, int, int, int, int, int, int, const void*,
@@ -104,11 +104,11 @@ int b200rl_gemm_f16(const void* A, const void* B, void* C, const float* bias, co
 
 int b200rl_conv_shift_fwd(const void* X, long long B, int Hg, int Wg, int C, const void* W, long long ldw, int N,
                           int taps, const int* shifts, int vy, int vx, void* out, const long long* omap,
-                          const void* saved, const long long* smap, const float* bias, int act, int dact, float alpha,
+                          const long long* smap, const float* bias, int act, int dact, float alpha,
                           const void* u8_x, const long long* u8_idx, int u8_H, int u8_W, int u8_C, int u8_s,
-                          void* act_bits_out, const void* saved_bits, int kx, void* stream) {
-  return conv_shift_fwd_impl(X, B, Hg, Wg, C, W, ldw, N, taps, shifts, vy, vx, out, omap, saved, smap, bias, act, dact,
-                             alpha, u8_x, u8_idx, u8_H, u8_W, u8_C, u8_s, act_bits_out, saved_bits, kx, S(stream));
+                          void* act_bits_out, const void* saved_bits, void* stream) {
+  return conv_shift_fwd_impl(X, B, Hg, Wg, C, W, ldw, N, taps, shifts, vy, vx, out, omap, smap, bias, act, dact, alpha,
+                             u8_x, u8_idx, u8_H, u8_W, u8_C, u8_s, act_bits_out, saved_bits, S(stream));
 }
 int b200rl_conv_shift_wgrad(const void* X, long long rows, int C, const void* dY, int N, int taps, const int* shifts,
                             float* G, long long ldg, float alpha, float* gbias, float alpha_b, int max_ctas,

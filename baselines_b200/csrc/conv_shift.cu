@@ -8,7 +8,7 @@
 //
 //   conv_shift_fwd_kernel   (K-major):  OUT[m, :] = act( sum_t X[m + sh_t, :] * W_t^T + b )          forward
 //                                       and, with negative shifts over a zero-bordered dY, the data gradient
-//                                       dX[m, :] = ( sum_t dY[m - sh_t, :] * W_t ) * act'(saved)
+//                                       dX[m, :] = ( sum_t dY[m - sh_t, :] * W_t ) * (saved activation > 0)
 //   conv_shift_wgrad_kernel (MN-major): G[t, c, n] += alpha * sum_m X[m + sh_t, c] * dY[m, n]         wgrad
 //                                       (a CTA keeps the accumulators of up to 2*QW taps x 64 channels in registers;
 //                                        X and dY are read once per such group of taps)
@@ -16,8 +16,8 @@
 // Warp roles: warps 0-7 are two consumer warpgroups (they issue the wgmma.mma_async chains, and run the epilogue --
 // or, in the wgrad, the fused bias-gradient sums -- from their own registers) | warp 8 TMA loads | uint8-fed first
 // layer only: warps 9-16 are uint8 producers that cast raw frames into a rolling A ring instead of the TMA.  The
-// forward epilogue can also write 1 bit per output element (act > 0); the dgrad of the next layer reads that instead
-// of the fp16 activation.
+// forward epilogue can also write 1 bit per output element (act > 0); the dgrad of the next layer reads that as its
+// ReLU mask.
 //
 // "Ping-pong" schedule of the forward / dgrad: the two consumer warpgroups take whole 128-row tiles (even / odd) and
 // turns on the tensor cores.  Named barriers 2 and 3 order their MMA issue: a group issues its next tile only after
@@ -269,26 +269,23 @@ struct ShiftParams {
   long long M;             // grid rows = B*Hg*Wg
   int Hg, Wg;              // grid
   int N;                   // output channels of the conv
-  int taps;                // filter rows (kx > 1) or taps (kx == 1)
-  int kx;                  // taps per filter row: tap (a, b) reads rows shifted by shift[a] + b
+  int taps;
   int shift[SH_MAX_TAPS];  // row shift of tap t, relative to min_shift (>= 0)
   int min_shift;           // smallest absolute shift (negative for dgrad)
   int vy, vx;              // rows with y < vy && x < vx produce an output
   __half* out;
   AddrMap omap;
-  const __half* saved;
   uint16_t* bits_out;           // optional (forward): bit k of word e/16 = (out element e + k) > 0, e = element offset
-  const uint16_t* saved_bits;   // optional (DACT): the same bit array of the saved activation, read instead of `saved`
+  const uint16_t* saved_bits;   // optional (DACT): the same bit array of the saved activation (ReLU mask)
   AddrMap smap;
   const float* bias;
-  int act, dact;           // dact = 1: multiply by act'(saved) instead of applying act
+  int act, dact;           // dact = 1: multiply by the saved_bits mask (if any) instead of applying act
   float alpha;
   int num_tiles;
 };
 
 // ------------------------------------------------------------------------------------------------ forward / dgrad
-// Weights: [kx*BN rows (b, n), taps*KH*64 columns (a, h, c)], all resident in shared memory as (a, h) sub-tiles of
-// kx*BN rows x 128 B; tap (a, b) uses rows [b*BN, b*BN + BN) of them.
+// Weights: [BN rows, taps*KH*64 columns (t, h, c)], all resident in shared memory as (t, h) sub-tiles of BN rows x 128 B.
 template <int BN, int KH, bool DACT, bool U8>
 __global__ void __launch_bounds__(sh_threads(U8), 1)
 conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
@@ -318,7 +315,7 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
 
   __shared__ float s_bias[BN];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int w_sub = p.kx * BN * 128;                 // one (a, h) weight sub-tile
+  constexpr int w_sub = BN * 128;                    // one (t, h) weight sub-tile
   if (threadIdx.x < BN) s_bias[threadIdx.x] = (p.bias && (int)threadIdx.x < p.N) ? p.bias[threadIdx.x] : 0.0f;
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
@@ -406,20 +403,17 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
       // tap 0 overwrites the accumulators with its first MMA; the others accumulate
 #pragma unroll 1
       for (int a = 0; a < p.taps; ++a) {
-#pragma unroll 1
-        for (int b = 0; b < p.kx; ++b) {
-          const uint32_t at = a_base + (uint32_t)(p.shift[a] + b) * 128u;
-          const uint32_t wt = w_base + (uint32_t)(a * KH * w_sub + b * BN * 128);
+        const uint32_t at = a_base + (uint32_t)p.shift[a] * 128u;
+        const uint32_t wt = w_base + (uint32_t)(a * KH * w_sub);
 #pragma unroll
-          for (int h = 0; h < KH; ++h) {
+        for (int h = 0; h < KH; ++h) {
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t bdesc = make_sdesc(wt + h * w_sub + k * 32, 16, 1024, 1);
+          for (int k = 0; k < 4; ++k) {
+            const uint64_t bdesc = make_sdesc(wt + h * w_sub + k * 32, 16, 1024, 1);
 #pragma unroll
-              for (int mh = 0; mh < MH; ++mh) {
-                const uint64_t adesc = make_sdesc(at + mh * 64 * 128 + h * SH_ABYTES + k * 32, 16, 1024, 1);
-                wgmma_f16<BN, 0, 0>(acc[mh], adesc, bdesc, (a | b | h | k) ? 1u : 0u);
-              }
+            for (int mh = 0; mh < MH; ++mh) {
+              const uint64_t adesc = make_sdesc(at + mh * 64 * 128 + h * SH_ABYTES + k * 32, 16, 1024, 1);
+              wgmma_f16<BN, 0, 0>(acc[mh], adesc, bdesc, (a | h | k) ? 1u : 0u);
             }
           }
         }
@@ -443,15 +437,15 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
         const int y = (int)(t2 - (uint32_t)n * (uint32_t)p.Hg);
         const bool ok = ((long long)m < p.M) && (y < p.vy) && (x < p.vx);
         const long long obase = map_rowbase(p.omap, n, y, x);
-        const long long sbase = DACT && p.saved ? map_rowbase(p.smap, n, y, x) : 0;
-        const bool masked = DACT && p.saved != nullptr && ok;
+        const bool masked = DACT && p.saved_bits != nullptr && ok;
+        const long long sbase = masked ? map_rowbase(p.smap, n, y, x) : 0;
 #pragma unroll
         for (int j = 0; j < BN / 16; ++j) {                  // 16-column chunks: two 8-column accumulator blocks
           uint32_t mw = 0xffffu;                              // activation-derivative bits of the chunk (DACT)
           // a 16-column chunk never straddles a class of the maps: column 16 * j + cc lies at coloff(16 * j) + cc
           const long long ocol = map_coloff(p.omap, 16 * j);
           const long long scol = DACT ? map_coloff(p.smap, 16 * j) : 0;
-          if (masked && p.saved_bits != nullptr) mw = __ldg(p.saved_bits + ((sbase + scol) >> 4));
+          if (masked) mw = __ldg(p.saved_bits + ((sbase + scol) >> 4));
           uint32_t bits = 0;
 #pragma unroll
           for (int jj = 0; jj < 2; ++jj) {
@@ -460,11 +454,7 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
             const int c = 16 * j + cc;
             __half2 o;
             if (DACT) {
-              uint32_t mb = mw >> cc;
-              if (masked && p.saved_bits == nullptr) {
-                const float2 h = __half22float2(*reinterpret_cast<const __half2*>(p.saved + sbase + scol + cc));
-                mb = (h.x > lo ? 1u : 0u) | (h.y > lo ? 2u : 0u);
-              }
+              const uint32_t mb = mw >> cc;
               o = __floats2half2_rn((mb & 1u) ? acc[mh][e] * p.alpha : 0.0f,
                                     (mb & 2u) ? acc[mh][e + 1] * p.alpha : 0.0f);
             } else {                                          // relu after the rounding: same result, one packed max
@@ -754,12 +744,10 @@ static bool fill_map(AddrMap& a, const long long* m) {       // {mode, sN, sY, s
 // shifts[taps]: absolute row shifts (all >= 0 for forward, all <= 0 for the data gradient).
 int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const void* W, long long ldw, int N,
                         int taps, const int* shifts, int vy, int vx, void* out, const long long* omap,
-                        const void* saved, const long long* smap, const float* bias, int act, int dact, float alpha,
+                        const long long* smap, const float* bias, int act, int dact, float alpha,
                         const void* u8_x, const long long* u8_idx, int u8_H, int u8_W, int u8_C, int u8_s,
-                        void* bits_out, const void* saved_bits, int kx, cudaStream_t stream) {
+                        void* bits_out, const void* saved_bits, cudaStream_t stream) {
   B200RL_REQUIRE((X || u8_x) && W && out && omap && B > 0, "conv_shift_fwd: null operand");
-  if (kx < 1) kx = 1;
-  B200RL_REQUIRE(kx <= 3 && (kx == 1 || !dact), "conv_shift_fwd: kx must be 1..3 (forward only)");
   B200RL_REQUIRE(!(bits_out && dact) && !(saved_bits && !(dact && smap)), "conv_shift_fwd: bits_out is a forward output, saved_bits a dact input (with smap)");
   if (u8_x) {
     B200RL_REQUIRE(C == 64 && u8_s * u8_C == 16 && u8_s == 4 && u8_H == Hg * u8_s && u8_W == Wg * u8_s && !dact &&
@@ -769,30 +757,26 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
   B200RL_REQUIRE(C == 64 || C == 128, "conv_shift_fwd: C must be 64 or 128 (got %d)", C);
   B200RL_REQUIRE(N == 32 || N == 64 || N == 128, "conv_shift_fwd: N must be 32, 64 or 128 (got %d)", N);
   B200RL_REQUIRE(taps >= 1 && taps <= SH_MAX_TAPS, "conv_shift_fwd: 1..%d taps", SH_MAX_TAPS);
-  B200RL_REQUIRE((C == 64 || C == 128) && (long long)taps * (C / 64) * kx * N * 128 <= sh_wres_bytes(C / 64, u8_x != nullptr),
+  B200RL_REQUIRE((C == 64 || C == 128) && (long long)taps * (C / 64) * N * 128 <= sh_wres_bytes(C / 64, u8_x != nullptr),
                  "conv_shift_fwd: weights do not fit in smem");
   ShiftParams p = {};
   int lo = shifts[0], hi = shifts[0];
   for (int t = 1; t < taps; ++t) { lo = shifts[t] < lo ? shifts[t] : lo; hi = shifts[t] > hi ? shifts[t] : hi; }
-  B200RL_REQUIRE(hi - lo + kx - 1 <= sh_arows(C / 64) - SH_BM, "conv_shift_fwd: shift span %d too large for C = %d",
-                 hi - lo + kx - 1, C);
+  B200RL_REQUIRE(hi - lo <= sh_arows(C / 64) - SH_BM, "conv_shift_fwd: shift span %d too large for C = %d", hi - lo,
+                 C);
   B200RL_REQUIRE(B * Hg * Wg < (1LL << 31) - 4096, "conv_shift_fwd: too many rows");
-  p.M = B * Hg * Wg; p.Hg = Hg; p.Wg = Wg; p.N = N; p.taps = taps; p.kx = kx; p.min_shift = lo;
+  p.M = B * Hg * Wg; p.Hg = Hg; p.Wg = Wg; p.N = N; p.taps = taps; p.min_shift = lo;
   for (int t = 0; t < taps; ++t) p.shift[t] = shifts[t] - lo;
   p.vy = vy; p.vx = vx; p.out = reinterpret_cast<__half*>(out);
   B200RL_REQUIRE(fill_map(p.omap, omap), "conv_shift_fwd: output map needs power-of-two Cq >= 16 and s");
-  p.saved = reinterpret_cast<const __half*>(saved);
   p.bits_out = reinterpret_cast<uint16_t*>(bits_out);
   p.saved_bits = reinterpret_cast<const uint16_t*>(saved_bits);
   if (smap) B200RL_REQUIRE(fill_map(p.smap, smap), "conv_shift_fwd: saved map needs power-of-two Cq >= 16 and s");
-  B200RL_REQUIRE(!(saved && !smap), "conv_shift_fwd: saved needs smap");
-  if (saved_bits && !saved) p.saved = reinterpret_cast<const __half*>(saved_bits);   // non-null marker: masking is on
   // the epilogue stores column pairs as 4-byte words and writes the activation bits per 16-column chunk
   B200RL_REQUIRE(((omap[1] | omap[2] | omap[3]) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 31) == 0,
                  "conv_shift_fwd: output strides must be multiples of 16 elements, base 32-byte aligned");
-  if (saved)
-    B200RL_REQUIRE(((smap[1] | smap[2] | smap[3]) & 15) == 0 && (reinterpret_cast<uintptr_t>(saved) & 31) == 0,
-                   "conv_shift_fwd: saved strides must be multiples of 16 elements, base 32-byte aligned");
+  if (saved_bits)
+    B200RL_REQUIRE(((smap[1] | smap[2] | smap[3]) & 15) == 0, "conv_shift_fwd: saved strides must be multiples of 16");
   p.bias = bias; p.act = act; p.dact = dact; p.alpha = alpha;
   p.num_tiles = (int)((p.M + SH_BM - 1) / SH_BM);
   p.u8 = make_u8src(u8_x, u8_idx, u8_H, u8_W, u8_C, u8_s);
@@ -802,9 +786,8 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
   CUtensorMap tmX, tmW;
   int rc;
   B200RL_REQUIRE(act == ACT_NONE || act == ACT_RELU, "conv_shift_fwd: activation must be none or relu");
-  if ((rc = make_tmap_2d_f16(&tmW, W, (long long)kx * N, (long long)taps * C, ldw, 64, kx * N)) != 0) return rc;
+  if ((rc = make_tmap_2d_f16(&tmW, W, N, (long long)taps * C, ldw, 64, N)) != 0) return rc;
   if (u8_x) {                                                          // tmX unused: A tiles come from the producers
-    B200RL_REQUIRE(kx == 1, "conv_shift_fwd: the uint8-fed first layer has no x-folded forward (rolling A ring)");
     B200RL_REQUIRE(hi - lo <= 32, "conv_shift_fwd: uint8-fed shift span %d exceeds one 32-row unit", hi - lo);
     return launch_fwd<32, 1, false, true>(tmW, tmW, p, stream);
   }

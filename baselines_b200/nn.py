@@ -7,7 +7,7 @@ Mirrors (by behaviour, not by code) the layer primitives of the reference:
 All math runs in hand-written CUDA (ops.*); torch here only allocates memory and provides streams.
 """
 import math
-from collections import OrderedDict
+from collections import OrderedDict, namedtuple
 
 import numpy as np
 import torch
@@ -211,20 +211,17 @@ class Linear:
 class Conv(Linear):
     """NHWC convolution lowered to im2col + wgmma GEMM (a2c/utils.py:37-56)."""
 
-    def __init__(self, store, name, H, W, C, nf, rf, stride, act, w_init, same_pad=False, in_scale=1.0,
-                 tf_w=None, tf_b=None, b_shape=None, allow_s2d=False):
+    def __init__(self, store, name, H, W, C, nf, rf, stride, act, w_init, plan, same_pad=False, in_scale=1.0,
+                 tf_w=None, tf_b=None, b_shape=None):
+        """plan: this layer's ConvLayerPlan (plan_conv_stack)."""
         self.H, self.W, self.C, self.nf, self.rf, self.stride, self.same = H, W, C, nf, rf, stride, same_pad
-        if same_pad:
-            self.OH, self.OW = -(-H // stride), -(-W // stride)
-        else:
-            self.OH, self.OW = (H - rf) // stride + 1, (W - rf) // stride + 1
+        self.OH, self.OW = ops._conv_out(H, W, rf, stride, same_pad)
         self.P = self.OH * self.OW
-        # space-to-depth view of a uint8 first layer: stride-s conv, filter k*s  ->  stride-1 conv, filter k, over
-        # s*s*C channels.  The fp32 master weight is stored with its K rows in (a, b, dy, dx, c) order; row_perm
-        # maps them back to the reference's HWIO (ky, kx, c) order for checkpoints.
-        self.s2d = bool(allow_s2d and stride > 1 and not same_pad and rf % stride == 0 and H % stride == 0 and
-                        W % stride == 0 and C * stride * stride in (16, 32, 64, 128) and (stride * C) % 8 == 0 and
-                        (W * C) % 8 == 0)
+        self.s2d, self.geom, self.implicit_dgrad = plan.s2d, plan.geom, plan.implicit_dgrad
+        self.implicit = plan.path == "implicit"
+        # space-to-depth view: stride-s conv, filter k*s  ->  stride-1 conv, filter k, over s*s*C channels.  The fp32
+        # master weight is stored with its K rows in (a, b, dy, dx, c) order; row_perm maps them back to the
+        # reference's HWIO (ky, kx, c) order for checkpoints.
         row_perm = None
         if self.s2d:
             s_, k = stride, rf // stride
@@ -247,44 +244,15 @@ class Conv(Linear):
     def col2im(self, dcols, saved, dx, B, act):
         ops.col2im(dcols, saved, dx, B, self.H, self.W, self.C, self.rf, self.stride, self.same, act=act, tag=self.name)
 
-    # ---- implicit-GEMM path (TMA im2col): no cols / dcols buffers ----------------------------------------
-    def plan_implicit(self):
-        """Geometry as seen by TMA.  Channels per tap must be 16/32/64; a first layer with few channels is
-        viewed through "super-pixels" of 16 consecutive (x, c) elements when the stride allows it."""
-        C, W, rf, st = self.C, self.W, self.rf, self.stride
-        if self.s2d:
-            self.geom = (self.H // st, W // st, C * st * st, rf // st, rf // st, 1, 1, 0, 0)
-            return self.geom
-        pad_t = pad_l = 0
-        if self.same:
-            ph = max((self.OH - 1) * st + rf - self.H, 0)
-            pw = max((self.OW - 1) * st + rf - W, 0)
-            pad_t, pad_l = ph // 2, pw // 2
-        m = 64 // C if C in (16, 32) else 1
-        if m > 1 and W % m == 0 and rf % m == 0 and st % m == 0 and pad_l % m == 0:
-            # merge m horizontally adjacent pixels into one 64-channel "pixel": same memory, same K order,
-            # but full 128-byte TMA rows and m x fewer taps
-            g = (self.H, W // m, C * m, rf, rf // m, st, st // m, pad_t, pad_l // m)
-        elif C in (16, 32, 64):
-            g = (self.H, W, C, rf, rf, st, st, pad_t, pad_l)
-        elif 16 % C == 0 and (W * C) % 16 == 0 and (rf * C) % 16 == 0 and (st * C) % 16 == 0 and (pad_l * C) % 16 == 0:
-            k = 16 // C
-            g = (self.H, W // k, 16, rf, rf // k, st, st // k, pad_t, pad_l // k)
-        else:
-            return None
-        self.geom = g
-        return g
-
+    # ---- implicit-GEMM path (TMA im2col through self.geom): no cols / dcols buffers -----------------------------
     def materialize(self):
         super().materialize()
-        self.implicit = self.plan_implicit() is not None
         self.wdg = None
-
-    def enable_dgrad(self):
-        An = -(-self.rf // self.stride)
-        self.An, self.ld_wdg = An, An * An * self.nf
-        self.wdg = torch.zeros(self.stride * self.stride * self.C, self.ld_wdg, dtype=torch.float16,
-                               device=self.store.device)
+        if self.implicit_dgrad:
+            An = -(-self.rf // self.stride)
+            self.An, self.ld_wdg = An, An * An * self.nf
+            self.wdg = torch.zeros(self.stride * self.stride * self.C, self.ld_wdg, dtype=torch.float16,
+                                   device=self.store.device)
 
     def refresh(self):
         super().refresh()
@@ -315,31 +283,111 @@ class Conv(Linear):
                       shuffle=(self.H, self.W, self.C, s), tag="dgrad." + self.name)
 
 
-def _shift_plan_ok(ob_shape, convs, same_pad):
-    """Shift-GEMM path (csrc/conv_shift.cu): every conv must be VALID with rf = k*stride on an input whose
-    space-to-depth view has 64 or 128 channels, with 32 / 64 output channels (NatureCNN qualifies)."""
-    if same_pad:
-        return False
+ConvLayerPlan = namedtuple("ConvLayerPlan", "path s2d geom implicit_dgrad kx")
+ConvLayerPlan.__doc__ = """How one conv layer runs.  path: "shift" (csrc/conv_shift.cu), "implicit" (TMA im2col GEMM over the
+input viewed as geom = (H, W, C, R, S, stride_h, stride_w, pad_t, pad_l)) or "explicit" (im2col + GEMM).  s2d: the
+layer reads its input space-to-depth'ed (and its master weight rows are stored in that order).  implicit_dgrad: the
+data gradient is one implicit GEMM with the pixel-shuffle epilogue instead of GEMM + col2im.  kx: taps per filter row
+the shift-GEMM weight gradient folds into one pass."""
+ConvStackPlan = namedtuple("ConvStackPlan", "shift fused_u8 layers")
+ConvStackPlan.__doc__ = """shift: every layer runs as shift-GEMM, and every layer writes its 1-bit ReLU mask, which the next
+data gradient (or fc1's) reads.  fused_u8: the first shift layer reads the uint8 frames itself."""
+
+# (k, nf, Cg) instances of the x-folded shift-GEMM weight gradient (csrc/conv_shift.cu conv_shift_wgrad_kernel)
+_XFOLD_WGRAD = ((2, 32, 64), (2, 64, 64), (2, 64, 128), (3, 64, 64))
+
+
+def _shift_stack_ok(ob_shape, convs):
+    """Every layer of a VALID conv stack passes the host checks of csrc/conv_shift.cu on its space-to-depth view: its
+    forward and weight gradient, and the data gradient that writes its input gradient."""
     H, W, C = ob_shape
     for i, (_nm, nf, rf, st) in enumerate(convs):
-        if rf % st or H % st or W % st or C * st * st not in (64, 128) or nf not in (32, 64):
+        if rf % st or H % st or W % st:                 # space-to-depth view: a stride-1 k x k conv
             return False
-        if i > 0 and nf != 64:          # its data gradient reads dY with C = nf channels (64-wide TMA rows)
+        k, Hg, Wg, Cg = rf // st, H // st, W // st, C * st * st
+        span = (k - 1) * Wg + (k - 1)                    # rows between the first and the last tap
+        # conv_shift_fwd_impl: C = 64 or 128, 1..16 taps, grid >= 2 x 2; conv_shift_wgrad_impl: N = 32 or 64
+        if Cg not in (64, 128) or k * k > 16 or Hg < 2 or Wg < 2 or nf not in (32, 64):
             return False
-        k = rf // st
-        if (k - 1) * (W // st) + (k - 1) > 32 or k * k > 16 or k * k * (C * st * st // 64) * nf * 128 > 80 * 1024:
+        # conv_shift_fwd_impl: span <= 32 rows for C = 64, <= 16 for C = 128 (sh_arows); resident weights
+        # taps * C/64 * N * 128 B <= 80 KB for C = 64, <= 64 KB for C = 128 (sh_wres_bytes)
+        if span > (32 if Cg == 64 else 16) or k * k * (Cg // 64) * nf * 128 > (80 if Cg == 64 else 64) * 1024:
             return False
-        OH, OW = (H - rf) // st + 1, (W - rf) // st + 1
+        # the data gradient of layer i > 0 is conv_shift_fwd_impl with C = nf: 64
+        if i > 0 and nf != 64:
+            return False
+        OH, OW = ops._conv_out(H, W, rf, st, False)
         if i + 1 < len(convs):
-            nst = convs[i + 1][3]
-            if OH % nst or OW % nst:
+            nrf, nst = convs[i + 1][2], convs[i + 1][3]
+            if OH % nst or OW % nst:                     # layer i writes its output space-to-depth'ed for layer i+1
                 return False
-            # the data gradient of layer i+1 is a GEMM with N = s^2*C_in outputs and resident [N, taps*nf] weights
-            kn = convs[i + 1][2] // nst
+            # the data gradient of layer i+1 writes N = s^2 * nf outputs (conv_shift_fwd_impl: N = 64 or 128 here, C =
+            # 64, resident weights taps * N * 128 B <= 80 KB)
+            kn = nrf // nst
             if nf * nst * nst not in (64, 128) or kn * kn * nf * nst * nst * 128 > 80 * 1024:
                 return False
         H, W, C = OH, OW, nf
     return True
+
+
+def _implicit_geom(H, W, C, rf, st, same_pad, s2d):
+    """The input as TMA im2col sees it, or None.  conv_gemm_impl: 16, 32 or 64 channels per tap; a layer with few
+    channels is viewed through "super-pixels" of 16 consecutive (x, c) elements when the stride allows it."""
+    if s2d:
+        return (H // st, W // st, C * st * st, rf // st, rf // st, 1, 1, 0, 0)
+    pad_t = pad_l = 0
+    if same_pad:
+        OH, OW = ops._conv_out(H, W, rf, st, True)
+        pad_t, pad_l = max((OH - 1) * st + rf - H, 0) // 2, max((OW - 1) * st + rf - W, 0) // 2
+    m = 64 // C if C in (16, 32) else 1
+    if m > 1 and W % m == 0 and rf % m == 0 and st % m == 0 and pad_l % m == 0:
+        # merge m horizontally adjacent pixels into one 64-channel "pixel": same memory, same K order,
+        # but full 128-byte TMA rows and m x fewer taps
+        return (H, W // m, C * m, rf, rf // m, st, st // m, pad_t, pad_l // m)
+    if C in (16, 32, 64):
+        return (H, W, C, rf, rf, st, st, pad_t, pad_l)
+    if 16 % C == 0 and (W * C) % 16 == 0 and (rf * C) % 16 == 0 and (st * C) % 16 == 0 and (pad_l * C) % 16 == 0:
+        k = 16 // C
+        return (H, W // k, 16, rf, rf // k, st, st // k, pad_t, pad_l // k)
+    return None
+
+
+def plan_conv_stack(ob_shape, convs, same_pad, has_fc):
+    """The convolution path of every layer of a conv stack over uint8 (H, W, C) observations, from the shapes alone.
+    convs: (name, filters, filter size, stride) per layer; has_fc: an fc layer follows the stack.  Returns a
+    ConvStackPlan.  A stack that passes the shift-GEMM checks runs as shift-GEMM; any other one layer by layer on the
+    implicit GEMM where its geometry allows, else on im2col + GEMM."""
+    if not same_pad and _shift_stack_ok(ob_shape, convs):
+        if not has_fc:
+            raise NotImplementedError("shift-mode conv_only towers")
+        H, W, C = ob_shape
+        layers = []
+        for _nm, nf, rf, st in convs:
+            k, Cg = rf // st, C * st * st
+            OH, OW = ops._conv_out(H, W, rf, st, False)
+            assert (OH * OW * nf) % 16 == 0                  # the 1-bit mask is written in 16-element words
+            layers.append(ConvLayerPlan("shift", st > 1, None, False, k if (k, nf, Cg) in _XFOLD_WGRAD else 1))
+            H, W, C = OH, OW, nf
+        _nm, nf0, rf0, st0 = convs[0]
+        # conv_shift_fwd_impl / conv_shift_wgrad_impl, uint8 source: s = 4, s*C = 16, N = 32, resident weights
+        # taps * N * 128 B <= 16 KB (SH_U8_WRES_BYTES)
+        fused_u8 = st0 == 4 and ob_shape[2] == 4 and nf0 == 32 and (rf0 // st0) ** 2 * nf0 * 128 <= 16 * 1024
+        return ConvStackPlan(True, fused_u8, layers)
+    H, W, C = ob_shape
+    layers = []
+    for i, (_nm, nf, rf, st) in enumerate(convs):
+        # first layer: space-to-depth'ed by s2d_gather_impl (H, W multiples of s; s*C, W*C multiples of 8) into the
+        # 16 / 32 / 64 channels per tap of conv_gemm_impl
+        s2d = (i == 0 and st > 1 and not same_pad and rf % st == 0 and H % st == 0 and W % st == 0 and
+               C * st * st in (16, 32, 64) and (st * C) % 8 == 0 and (W * C) % 8 == 0)
+        geom = _implicit_geom(H, W, C, rf, st, same_pad, s2d)
+        # pixel-shuffle data gradient (conv_gemm_impl over dz: 16 / 32 / 64 channels per tap; shuffle epilogue:
+        # C % 16 == 0; VALID padding only)
+        implicit_dgrad = i > 0 and geom is not None and not same_pad and nf in (16, 32, 64) and C % 16 == 0
+        layers.append(ConvLayerPlan("explicit" if geom is None else "implicit", s2d, geom, implicit_dgrad, 1))
+        H, W = ops._conv_out(H, W, rf, st, same_pad)
+        C = nf
+    return ConvStackPlan(False, False, layers)
 
 
 class Tower:
@@ -356,23 +404,17 @@ class Tower:
             H, W, C = ob_shape
             self.in_u8 = True
             scale_in = 1.0 / 255.0                                           # models.py:19 folded into c1 weights
-            import os
-            self.shift_mode = (os.environ.get("B200RL_EXPLICIT_CONV", "0") != "1" and
-                               os.environ.get("B200RL_NO_SHIFT", "0") != "1" and
-                               _shift_plan_ok(ob_shape, convs, same_pad))
-            for i, (nm, nf, rf, stride) in enumerate(convs):
+            self.plan = plan_conv_stack(ob_shape, convs, same_pad, kind == "cnn")
+            self.shift_mode = self.plan.shift
+            for i, ((nm, nf, rf, stride), lp) in enumerate(zip(convs, self.plan.layers)):
                 if tf_style == "a2c":
                     tfw, tfb, bshape = f"{tf_prefix}/{nm}/w:0", f"{tf_prefix}/{nm}/b:0", (1, nf, 1, 1)
                 else:
                     cn = "Conv" if i == 0 else f"Conv_{i}"
                     tfw, tfb, bshape = f"{tf_prefix}/convnet/{cn}/weights:0", f"{tf_prefix}/convnet/{cn}/biases:0", (nf,)
-                import os
                 conv = Conv(store, f"{prefix}/{nm}", H, W, C, nf, rf, stride, "relu",
-                            winit((rf, rf, C, nf), math.sqrt(2)), same_pad=same_pad,
-                            in_scale=scale_in if i == 0 else 1.0, tf_w=tfw, tf_b=tfb, b_shape=bshape,
-                            allow_s2d=(self.shift_mode or
-                                       (i == 0 and os.environ.get("B200RL_EXPLICIT_CONV", "0") != "1"
-                                        and os.environ.get("B200RL_NO_S2D", "0") != "1")))
+                            winit((rf, rf, C, nf), math.sqrt(2)), lp, same_pad=same_pad,
+                            in_scale=scale_in if i == 0 else 1.0, tf_w=tfw, tf_b=tfb, b_shape=bshape)
                 self.convs.append(conv)
                 H, W, C = conv.OH, conv.OW, nf
             self.flat = H * W * C
@@ -420,19 +462,8 @@ class Tower:
             self.hfc = [torch.empty(cap, l.Np, **f16) for l in self.fcs]
             self.dzfc = [torch.empty(cap, l.Np, **f16) for l in self.fcs]
             self.ld_hfc = [l.Np for l in self.fcs]     # row pitch of hfc[i] / dzfc[i]
-            if self.fcs:
-                self.dlatent, self.ld_dlatent = self.dzfc[-1], self.fcs[-1].Np
-            else:
-                raise NotImplementedError("shift-mode conv_only towers")
+            self.dlatent, self.ld_dlatent = self.dzfc[-1], self.fcs[-1].Np
             return
-        import os
-        allow = os.environ.get("B200RL_EXPLICIT_CONV", "0") != "1"
-        # implicit dgrad needs VALID padding, the dz tensor's channels in {16,32,64} and a zero-initialised dx
-        for i, c in enumerate(self.convs):
-            c.implicit = c.implicit and allow
-            c.implicit_dgrad = (i > 0 and c.implicit and not c.same and c.nf in (16, 32, 64) and c.C % 16 == 0)
-            if c.implicit_dgrad:
-                c.enable_dgrad()
         self.cols = [None if c.implicit else torch.empty(cap * c.P, c.K, **f16) for c in self.convs]
         self.hconv = [torch.empty(cap * c.P, c.nf, **f16) for c in self.convs]
         self.dcols = [None] + [None if c.implicit_dgrad else torch.empty(cap * c.P, c.K, **f16)
@@ -456,62 +487,36 @@ class Tower:
     # ---- shift-GEMM conv stack ---------------------------------------------------------------------------------
     def _materialize_shift(self, f16):
         cap, cv = self.cap, self.convs
-        self.sg = []                                   # per layer: dict(Hg, Wg, Cg, k, shifts, s)
-        import os
-        # x-fold: the kx horizontally adjacent taps of a filter row share one weight row block (conv_shift.cu walks them
-        # as taps shifted by one more grid row each); forward fold only on request
-        xfold = os.environ.get("B200RL_NO_XFOLD", "0") != "1"
-        xfold_fwd = os.environ.get("B200RL_XFOLD_FWD", "0") == "1"
-        for c in cv:
+        self.sg = []                                   # per layer: dict(Hg, Wg, Cg, k, s, kx, shifts, yshifts)
+        for c, lp in zip(cv, self.plan.layers):
             s_, k = c.stride, c.rf // c.stride
             Hg, Wg, Cg = c.H // s_, c.W // s_, c.C * s_ * s_
-            # x-fold (csrc/conv_shift.cu): the k taps of a filter row ride in the MMA's N dimension; kernels exist for
-            # (k, nf, Cg) in {(2, 32, 64), (2, 64, 64), (2, 64, 128), (3, 64, 64)}
-            kx = k if (xfold and (k, c.nf, Cg) in ((2, 32, 64), (2, 64, 64), (2, 64, 128), (3, 64, 64))) else 1
-            self.sg.append(dict(Hg=Hg, Wg=Wg, Cg=Cg, k=k, s=s_, kx=kx, kx_fwd=kx if xfold_fwd else 1,
+            # x-fold (weight gradient): the kx horizontally adjacent taps of a filter row are walked as taps shifted by
+            # one more grid row each, from the filter row's shift in yshifts
+            self.sg.append(dict(Hg=Hg, Wg=Wg, Cg=Cg, k=k, s=s_, kx=lp.kx,
                                 shifts=[a * Wg + b for a in range(k) for b in range(k)],
                                 yshifts=[a * Wg for a in range(k)]))
-        c0, g0 = cv[0], self.sg[0]
-        import os
+        g0 = self.sg[0]
         # first layer straight from the uint8 images (producer warps gather + cast + space-to-depth in smem)
-        self.fused_u8 = (os.environ.get("B200RL_NO_FUSED_U8", "0") != "1" and c0.stride == 4 and c0.C == 4 and
-                         c0.nf == 32 and g0["Cg"] == 64)
+        self.fused_u8 = self.plan.fused_u8
         self.x16 = None if self.fused_u8 else torch.empty(cap, g0["Hg"] * g0["Wg"] * g0["Cg"], **f16)
-        if self.fused_u8:
-            g0["kx_fwd"] = 1                           # the uint8-fed forward kernel (rolling A ring) has no folded variant
         # activations: layer i's output is stored space-to-depth'ed for layer i+1 (compact after the last conv)
         self.hconv = [torch.empty(cap, c.OH * c.OW * c.nf, **f16) for c in cv]
-        # 1 bit per element "activation > 0" of every conv output a later dgrad masks with: the backward kernels read
-        # these instead of the fp16 activations (16x less mask traffic)
-        self.hbits = [None] * len(cv)
-        if os.environ.get("B200RL_NO_RELU_BITS", "0") != "1":
-            for i, c in enumerate(cv):               # the last conv's mask serves the fc1 data gradient
-                if c.act == ops.ACT_RELU and (c.OH * c.OW * c.nf) % 16 == 0:
-                    self.hbits[i] = torch.zeros(cap * (c.OH * c.OW * c.nf // 16), dtype=torch.int16,
-                                                device=self.hconv[i].device)
+        # 1 bit per element "activation > 0" of every conv output: the ReLU mask of the next layer's data gradient (the
+        # last conv's serves the fc1 data gradient)
+        self.hbits = [torch.zeros(cap * (c.OH * c.OW * c.nf // 16), dtype=torch.int16, device=self.hconv[i].device)
+                      for i, c in enumerate(cv)]
         # gradients w.r.t. conv outputs live zero-bordered on the conv's INPUT grid
         self.dY = [torch.zeros(cap, g["Hg"] * g["Wg"] * c.nf, **f16) for c, g in zip(cv, self.sg)]
         # data-gradient weight operands [N' = Cg, taps * nf] (tap blocks of the master weight side by side)
         self.wd = [None] + [torch.zeros(g["Cg"], g["k"] * g["k"] * c.nf, **f16) for c, g in zip(cv[1:], self.sg[1:])]
-        # x-folded forward operands [kx * nf, ky * Cg]: row b*nf + n, column a*Cg + c = tap (a, b)
-        self.wfold = [torch.zeros(g["kx"] * c.nf, g["k"] * g["Cg"], **f16) if g["kx_fwd"] > 1 else None
-                      for c, g in zip(cv, self.sg)]
         self.flat = cv[-1].OH * cv[-1].OW * cv[-1].nf
 
     def _refresh_shift(self):
-        for i, (c, g) in enumerate(zip(self.convs, self.sg)):
-            if g["kx_fwd"] > 1:
-                k, Cg, nf = g["k"], g["Cg"], c.nf
-                for a in range(k):
-                    for b in range(k):
-                        t = a * k + b
-                        ops.cast_transpose(c.w[t * Cg:(t + 1) * Cg], Cg, nf, None, 0,
-                                           self.wfold[i][b * nf:(b + 1) * nf, a * Cg:], k * Cg, scale=c.in_scale)
-            if i == 0:
-                continue
+        for c, g, wd in zip(self.convs[1:], self.sg[1:], self.wd[1:]):
             taps, Cg, nf = g["k"] * g["k"], g["Cg"], c.nf
             for t in range(taps):                      # wd[:, t*nf:(t+1)*nf] = fp16(W[t*Cg:(t+1)*Cg, :])
-                ops.cast_transpose(c.w[t * Cg:(t + 1) * Cg], Cg, nf, self.wd[i][:, t * nf:], taps * nf, None, 0)
+                ops.cast_transpose(c.w[t * Cg:(t + 1) * Cg], Cg, nf, wd[:, t * nf:], taps * nf, None, 0)
 
     def _forward_shift(self, x, B, src_idx, masks=True):
         cv, sg = self.convs, self.sg
@@ -530,16 +535,10 @@ class Tower:
                 omap = (2, Hn * Wn * Cn, Wn * Cn, Cn, c.nf, sn)
             else:
                 omap = (0, c.OH * c.OW * c.nf, c.OW * c.nf, c.nf, 0, 0)
-            if g["kx_fwd"] > 1:
-                ops.conv_shift_fwd(cur, B, g["Hg"], g["Wg"], g["Cg"], self.wfold[i], g["k"] * g["Cg"], c.nf,
-                                   g["yshifts"], c.OH, c.OW, self.hconv[i], omap, bias=c.b, act=c.act,
-                                   tag="fwd." + c.name, u8=self._u8 if i == 0 else None, bits_out=self.hbits[i] if masks else None,
-                                   useful_rows=B * c.OH * c.OW, kx=g["kx_fwd"])
-            else:
-                ops.conv_shift_fwd(cur, B, g["Hg"], g["Wg"], g["Cg"], c.w_fwd, c.Kp, c.nf, g["shifts"], c.OH, c.OW,
-                                   self.hconv[i], omap, bias=c.b, act=c.act, tag="fwd." + c.name,
-                                   u8=self._u8 if i == 0 else None, bits_out=self.hbits[i] if masks else None,
-                                   useful_rows=B * c.OH * c.OW)
+            ops.conv_shift_fwd(cur, B, g["Hg"], g["Wg"], g["Cg"], c.w_fwd, c.Kp, c.nf, g["shifts"], c.OH, c.OW,
+                               self.hconv[i], omap, bias=c.b, act=c.act, tag="fwd." + c.name,
+                               u8=self._u8 if i == 0 else None, bits_out=self.hbits[i] if masks else None,
+                               useful_rows=B * c.OH * c.OW)
             cur = self.hconv[i]
         return cur, self.flat
 
@@ -562,7 +561,7 @@ class Tower:
             smap = (0, g["Hg"] * g["Wg"] * g["Cg"], g["Wg"] * g["Cg"], g["Cg"], 0, 0)
             ops.conv_shift_fwd(self.dY[i], B, g["Hg"], g["Wg"], c.nf, self.wd[i], g["k"] * g["k"] * c.nf, g["Cg"],
                                [-sft for sft in g["shifts"]], g["Hg"], g["Wg"], self.dY[i - 1], omap,
-                               saved=self.hconv[i - 1], smap=smap, act=ops.ACT_RELU, dact=True, tag="dgrad." + c.name,
+                               smap=smap, act=ops.ACT_RELU, dact=True, tag="dgrad." + c.name,
                                saved_bits=self.hbits[i - 1], useful_rows=B * c.OH * c.OW)
 
     def refresh(self):

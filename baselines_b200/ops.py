@@ -101,11 +101,11 @@ def _u8_args(u8):
     return _ptr(x), _ptr(idx), int(H), int(W), int(C), int(s)
 
 
-def conv_shift_fwd(X, B, Hg, Wg, C, W, ldw, N, shifts, vy, vx, out, omap, *, saved=None, smap=None, bias=None,
+def conv_shift_fwd(X, B, Hg, Wg, C, W, ldw, N, shifts, vy, vx, out, omap, *, smap=None, bias=None,
                    act=ACT_NONE, dact=False, alpha=1.0, tag=None, u8=None, bits_out=None, saved_bits=None,
-                   useful_rows=None, kx=1):
-    """Shift-GEMM convolution (forward, or data gradient with dact=True).  omap / smap: 6-tuples
-    (mode, sN, sY, sX, Cq, s).  useful_rows (accounting only): positions that are real conv outputs -- the kernel
+                   useful_rows=None):
+    """Shift-GEMM convolution (forward, or data gradient with dact=True, masked by the ReLU bits saved_bits of the
+    saved activation when given).  omap / smap: 6-tuples (mode, sN, sY, sX, Cq, s).  useful_rows (accounting only): positions that are real conv outputs -- the kernel
     also computes (and discards) the grid positions that are not; reported flops / bytes count the useful ones."""
     _chk(X, torch.float16, "X")
     _chk(W, torch.float16, "W")
@@ -120,13 +120,13 @@ def conv_shift_fwd(X, B, Hg, Wg, C, W, ldw, N, shifts, vy, vx, out, omap, *, sav
     useful = float(useful_rows) if useful_rows is not None else float(B) * vy * vx
     if dact:      # data gradient: reads the valid dY rows, writes every dX position, reads the activation mask
         nbytes = 2.0 * useful * C + 2.0 * rows * N
-        nbytes += 0.0 if saved is None and saved_bits is None else (0.125 if saved_bits is not None else 2.0) * rows * N
+        nbytes += 0.0 if saved_bits is None else 0.125 * rows * N
     else:         # forward: reads every input position, writes the valid outputs (+ 1 bit per element of mask)
         nbytes = (1.0 if u8 is not None else 2.0) * rows * C + 2.0 * useful * N + (0.125 * useful * N if bits_out is not None else 0.0)
     _lib.call("b200rl_conv_shift_fwd", _ptr(X), int(B), Hg, Wg, C, _ptr(W), int(ldw), int(N), len(shifts), sh, vy, vx,
-              _ptr(out), om, _ptr(saved), sm, _ptr(bias), int(act), int(bool(dact)), float(alpha), *u8a,
-              _ptr(bits_out), _ptr(saved_bits), int(kx), _stream(),
-              label="convs." + (tag or "fwd"), flops=2.0 * useful * N * len(shifts) * kx * C, nbytes=nbytes)
+              _ptr(out), om, sm, _ptr(bias), int(act), int(bool(dact)), float(alpha), *u8a,
+              _ptr(bits_out), _ptr(saved_bits), _stream(),
+              label="convs." + (tag or "fwd"), flops=2.0 * useful * N * len(shifts) * C, nbytes=nbytes)
 
 
 def conv_shift_wgrad(X, rows, C, dY, N, shifts, G, ldg, alpha=1.0, max_ctas=0, tag=None, gbias=None, alpha_b=1.0,

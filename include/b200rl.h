@@ -63,28 +63,27 @@ int b200rl_gemm_f16(const void* A, const void* B, void* C, const float* bias, co
  * (C = 64 or 128; strided convs arrive space-to-depth transformed).  Each X row is loaded into smem once; filter
  * tap t is the same buffer read through a descriptor shifted by shifts[t] rows.
  *   fwd  : out[map(n,y,x), :N] = act(sum_t X[m+shift_t] * W[:, t*C:(t+1)*C]^T + bias)   for y < vy, x < vx
- *          dact = 1: out = (sum_t ...) * act'(saved[smap(n,y,x)])  (data gradient: X = zero-bordered dY, shifts <= 0)
+ *          dact = 1: out = (sum_t ...) * (saved activation at smap(n,y,x) > 0) with the mask read from saved_bits,
+ *          or out = sum_t ... without saved_bits  (data gradient: X = zero-bordered dY, shifts <= 0)
  *   omap / smap: {mode, sN, sY, sX, Cq, s}: 0 = n*sN+y*sY+x*sX+col; 1 = depth->space; 2 = space->depth
  *   wgrad: G[t*C + c, n] += alpha * sum_m X[m+shift_t, c] * dY[m, n]  (dY on X's grid, zero at invalid positions) */
 int b200rl_conv_shift_fwd(const void* X, long long B, int Hg, int Wg, int C, const void* W, long long ldw, int N,
                           int taps, const int* shifts, int vy, int vx, void* out, const long long* omap,
-                          const void* saved, const long long* smap, const float* bias, int act, int dact, float alpha,
+                          const long long* smap, const float* bias, int act, int dact, float alpha,
                           const void* u8_x, const long long* u8_idx, int u8_H, int u8_W, int u8_C, int u8_s,
-                          void* act_bits_out, const void* saved_bits, int kx, void* stream);
+                          void* act_bits_out, const void* saved_bits, void* stream);
 /* act_bits_out (forward, optional): uint16[numel(out)/16]; bit k of word e/16 is set iff out element e+k > 0 (e = the
  * element offset the output map produces, always a multiple of 16).  saved_bits (dact, optional): the same array for
- * the saved activation; it is read instead of `saved` (1 bit instead of 16 per element of backward HBM traffic).
+ * the saved activation, addressed through smap (1 bit instead of 16 per element of backward HBM traffic).
  * u8_x != NULL (first layer): X is ignored; producer warps gather uint8 images u8_x[u8_idx[n], H, W, C], cast them
  * to fp16 and build the space-to-depth (factor u8_s) tile directly in shared memory (models.py:19, ppo2.py:165). */
 int b200rl_conv_shift_wgrad(const void* X, long long rows, int C, const void* dY, int N, int taps, const int* shifts,
                             float* G, long long ldg, float alpha, float* gbias, float alpha_b, int max_ctas,
                             const void* u8_x, const long long* u8_idx, int u8_H, int u8_W, int u8_C, int u8_s,
                             int kx, void* stream);
-/* kx > 1 ("x-fold", forward and wgrad): the filter is ky rows of kx horizontally adjacent taps (row shift of tap
- * (a, b) = a*Wg + b).  `shifts` then lists only the ky row shifts a*Wg, and the kx taps of a filter row ride in the
- * MMA's N dimension, so every X slab is fetched from shared memory once per filter row instead of once per tap.
- *   fwd  : W is [kx*N, ky*C] with row b*N + n, column a*C + c = filter tap (a, b), input channel c, output channel n
- *   wgrad: G keeps its [(a*kx + b)*C + c, n] row order. */   /* gbias != NULL: gbias[n] += alpha_b * sum_m dY[m, n] (fused) */
+/* kx > 1 ("x-fold"): the filter is ky rows of kx horizontally adjacent taps (row shift of tap (a, b) = a*Wg + b).
+ * `shifts` then lists only the ky row shifts a*Wg; tap (a, b) reads X shifted by shifts[a] + b, and G keeps its
+ * [(a*kx + b)*C + c, n] row order. */   /* gbias != NULL: gbias[n] += alpha_b * sum_m dY[m, n] (fused) */
 
 /* Implicit-GEMM convolution (tf.nn.conv2d a2c/utils.py:56 and its gradients): the A operand is read
  * straight from the NHWC fp16 activation x[B,H,W,C] by TMA im2col mode (C = 16, 32 or 64 channels per tap).

@@ -52,6 +52,9 @@ CASES = {
                            value_network="copy"),
     "mlp_gauss_shared": dict(network="mlp", ob_shape=(11,), ob_dtype=np.float32, discrete=False, nA=3,
                              value_network=None),
+    # 2 * 256 hidden units: the two first layers run as separate GEMMs (the fused one takes 2 * hidden <= 256)
+    "mlp_gauss_copy_unfused": dict(network="mlp", ob_shape=(11,), ob_dtype=np.float32, discrete=False, nA=3,
+                                   value_network="copy", num_hidden=256),
 }
 
 

@@ -355,55 +355,44 @@ def _shift_taps(k, Wg, kx):
     return [a * Wg for a in range(k)] if kx > 1 else [a * Wg + b for a in range(k) for b in range(k)]
 
 
-def _fold(w64, k, N, C):
-    """[N, (a, b, c)] weights -> x-folded [(b, n), (a, c)]."""
-    wf = torch.zeros(k * N, k * C, dtype=torch.float64, device=DEV)
-    for a in range(k):
-        for b in range(k):
-            t = a * k + b
-            wf[b * N:(b + 1) * N, a * C:(a + 1) * C] = w64[:, t * C:(t + 1) * C]
-    return wf
-
-
 SHIFT_FWD = [
-    # name, B, Hg, Wg, C, N, k, kx, omap ("compact" / "grid" / "s2d"), bits
-    ("c64_n32_span32_limit", 3, 9, 31, 64, 32, 2, 1, "grid", False),
-    ("c64_n64_3x3_bits", 5, 11, 11, 64, 64, 3, 1, "compact", True),
-    ("c64_n128_2x2", 4, 9, 13, 64, 128, 2, 1, "compact", True),
-    ("c128_n32_span16_limit", 3, 11, 15, 128, 32, 2, 1, "grid", False),
-    ("c128_n64_2x2_bits", 4, 10, 10, 128, 64, 2, 1, "compact", True),
-    ("c64_n32_s2d_out", 3, 21, 21, 64, 32, 2, 1, "s2d", True),
-    ("xfold_kx2_c64_n64", 5, 9, 12, 64, 64, 2, 2, "grid", False),
-    ("xfold_kx3_c64_n64_bits", 6, 9, 9, 64, 64, 3, 3, "compact", True),
-    ("xfold_kx2_c128_n64", 3, 10, 10, 128, 64, 2, 2, "compact", True),
-    ("c64_n32_many_tiles_per_cta", 400, 17, 31, 64, 32, 2, 1, "compact", True),
+    # name, B, Hg, Wg, C, N, k, omap ("compact" / "grid" / "s2d"), bits
+    ("c64_n32_span32_limit", 3, 9, 31, 64, 32, 2, "grid", False),
+    ("c64_n64_3x3_bits", 5, 11, 11, 64, 64, 3, "compact", True),
+    ("c64_n128_2x2", 4, 9, 13, 64, 128, 2, "compact", True),
+    ("c128_n32_span16_limit", 3, 11, 15, 128, 32, 2, "grid", False),
+    ("c128_n64_2x2_bits", 4, 10, 10, 128, 64, 2, "compact", True),
+    ("c64_n32_s2d_out", 3, 21, 21, 64, 32, 2, "s2d", True),
+    ("c64_n32_many_tiles_per_cta", 400, 17, 31, 64, 32, 2, "compact", True),
+    ("c128_n128_1x1_bits", 3, 10, 10, 128, 128, 1, "compact", True),
+    ("c64_n32_16taps_limit", 4, 9, 9, 64, 32, 4, "compact", True),
+    ("c128_n32_s2d_out", 3, 15, 15, 128, 32, 2, "s2d", True),
 ]
 
 
-@pytest.mark.parametrize("name,B,Hg,Wg,C,N,k,kx,omode,bits", SHIFT_FWD, ids=[c[0] for c in SHIFT_FWD])
-def test_conv_shift_forward_exact(ops, name, B, Hg, Wg, C, N, k, kx, omode, bits):
+@pytest.mark.parametrize("name,B,Hg,Wg,C,N,k,omode,bits", SHIFT_FWD, ids=[c[0] for c in SHIFT_FWD])
+def test_conv_shift_fwd_exact(ops, name, B, Hg, Wg, C, N, k, omode, bits):
     """Shift-GEMM forward (relu + bias, alpha 0.5) == the float64 k x k VALID convolution: shift spans at the limit
-    (32 rows for C = 64, 16 for C = 128), M not a multiple of 128, x-fold kx = 2 / 3, compact / full-grid / space-to-
-    depth output maps and the 1-bit ReLU mask.  Grid positions that are not conv outputs keep their sentinel."""
+    (32 rows for C = 64, 16 for C = 128), 16 taps, every (C, N) instance, M not a multiple of 128, compact /
+    full-grid / space-to-depth output maps and the 1-bit ReLU mask.  Grid positions that are not conv outputs keep their sentinel."""
     gen = _gen(B * Hg * Wg + N)
     OH, OW = Hg - k + 1, Wg - k + 1
     M = B * Hg * Wg
     assert M % 128
-    shifts = _shift_taps(k, Wg, kx)
-    span = max(shifts) - min(shifts) + kx - 1
+    shifts = _shift_taps(k, Wg, 1)
+    span = max(shifts) - min(shifts)
     assert span <= (32 if C == 64 else 16)
     K = k * k * C
     x64 = _ints((M, C), 0.5, gen)
     X = torch.full((M + 200, C), NAN16, dtype=torch.float16, device=DEV)
     X[:M] = x64.half()
     w64 = _ints((N, K), 0.5, gen)
-    wop = _fold(w64, k, N, C) if kx > 1 else w64
-    ldw = wop.shape[1] + 8
-    W = torch.full((wop.shape[0], ldw), NAN16, dtype=torch.float16, device=DEV)
-    W[:, :wop.shape[1]] = wop.half()
+    ldw = K + 8
+    W = torch.full((N, ldw), NAN16, dtype=torch.float16, device=DEV)
+    W[:, :K] = w64.half()
     bias = _ints((N,), 0.7, gen, -3, 3).float()
-    full = R.shift_conv(x64, [a * Wg + b for a in range(k) for b in range(k)], w64).view(B, Hg, Wg, N)
-    R.assert_exact_ok(R.shift_conv(x64.abs(), [a * Wg + b for a in range(k) for b in range(k)], w64.abs()), what=name)
+    full = R.shift_conv(x64, shifts, w64).view(B, Hg, Wg, N)
+    R.assert_exact_ok(R.shift_conv(x64.abs(), shifts, w64.abs()), what=name)
     ref = torch.relu(0.5 * full[:, :OH, :OW] + bias.double())
     if name.endswith("many_tiles_per_cta"):
         tiles = _cdiv(M, 128)
@@ -422,18 +411,19 @@ def test_conv_shift_forward_exact(ops, name, B, Hg, Wg, C, N, k, kx, omode, bits
         omap, want = (2, (OH // 2) * (OW // 2) * 4 * N, (OW // 2) * 4 * N, 4 * N, N, 2), R.space_to_depth(ref, 2)
     bo = torch.full((out.numel() // 16,), 0x5A5A, dtype=torch.int16, device=DEV) if bits else None
     ops.conv_shift_fwd(X, B, Hg, Wg, C, W, ldw, N, shifts, OH, OW, out, omap, bias=bias, act=ops.ACT_RELU, alpha=0.5,
-                       bits_out=bo, kx=kx)
+                       bits_out=bo)
     torch.cuda.synchronize()
     assert torch.equal(out.double(), want), (name, float((out.double() - want).abs().max()))
     if bits:
         assert torch.equal(bo, R.relu_bits(out)), (name, "bits")
 
 
-@pytest.mark.parametrize("k,mode,bits", [(3, "grid", False), (3, "grid", True), (2, "d2s", False), (2, "d2s", True)])
-def test_conv_shift_dgrad_exact(ops, k, mode, bits):
-    """Data gradient: negative shifts (min_shift < 0, so the first tile's TMA zero-fills), the relu mask from the
-    saved activation or from its bit array (smap), mode 0 output on the input grid or mode 1 depth->space into a
+@pytest.mark.parametrize("k,mode,mask", [(3, "grid", "none"), (3, "grid", "bits"), (2, "d2s", "none"), (2, "d2s", "bits")])
+def test_conv_shift_dgrad_exact(ops, k, mode, mask):
+    """Data gradient: negative shifts (min_shift < 0, so the first tile's TMA zero-fills), masked by the bit array of
+    the saved activation's ReLU (smap) or unmasked, mode 0 output on the input grid or mode 1 depth->space into a
     larger grid whose border keeps its sentinel."""
+    bits = mask == "bits"
     gen = _gen(k * 10 + bits)
     if mode == "grid":
         B, Hg, Wg, Cdz, Cout = 7, 9, 9, 64, 64
@@ -451,7 +441,7 @@ def test_conv_shift_dgrad_exact(ops, k, mode, bits):
     smap = (0, Hg * Wg * Cout, Wg * Cout, Cout, 0, 0)
     full = R.shift_conv(dY64.reshape(M, Cdz), [-s for s in shifts], wd64).view(B, Hg, Wg, Cout)
     R.assert_exact_ok(R.shift_conv(dY64.reshape(M, Cdz).abs(), [-s for s in shifts], wd64.abs()), what="dgrad")
-    dx = 0.5 * full * (saved.double() > 0)
+    dx = 0.5 * full * (saved.double() > 0) if bits else 0.5 * full
     if mode == "grid":
         out = torch.full((B, Hg, Wg, Cout), SENT, dtype=torch.float16, device=DEV)
         omap, want = smap, dx
@@ -462,11 +452,11 @@ def test_conv_shift_dgrad_exact(ops, k, mode, bits):
         omap = (1, Ho * Ho * Cq, Ho * Cq, Cq, Cq, 2)
         want = torch.full((B, Ho, Ho, Cq), SENT, dtype=torch.float64, device=DEV)
         want[:, :2 * Hg, :2 * Wg] = R.depth_to_space(dx, 2)
-    kw = dict(saved_bits=R.relu_bits(saved)) if bits else dict(saved=saved)
+    kw = dict(saved_bits=R.relu_bits(saved)) if bits else {}
     ops.conv_shift_fwd(dY, B, Hg, Wg, Cdz, wd64.half().contiguous(), taps * Cdz, Cout, [-s for s in shifts], Hg, Wg,
                        out, omap, smap=smap, act=ops.ACT_RELU, dact=True, alpha=0.5, **kw)
     torch.cuda.synchronize()
-    assert torch.equal(out.double(), want), (k, mode, bits, float((out.double() - want).abs().max()))
+    assert torch.equal(out.double(), want), (k, mode, mask, float((out.double() - want).abs().max()))
 
 
 def _u8_frames(pool, H, W, C, gen):
