@@ -309,6 +309,8 @@ def test_train_step_matches_oracle(name):
         p, po = model.get_params(), oracle.params_np()
         err = max(float(np.abs(p[k] - po[k]).max()) for k in p)
         worst = max(worst, err)
+        # the reference's tolerance.  Adam moves each element by at most ~lr per step whatever the gradient, so this
+        # bounds the step and cannot detect a gradient error (see test_update_composition_gpu.py)
         assert err < 3e-3, (it, err)
     print(f"[{name}] max |param - oracle| after 3 steps = {worst:.3e}")
 

@@ -21,6 +21,7 @@ import pytest
 import torch
 
 import _refs as R
+from _net_refs import kernel_act as _kernel_act, reference as _reference
 
 pytestmark = pytest.mark.gpu
 
@@ -163,40 +164,6 @@ def _build(name, B):
         l.b.copy_(torch.from_numpy(rng.randn(l.N).astype(np.float32) * 0.05).to(DEV))
     tower.refresh()
     return tower, store, rng
-
-
-def _kernel_act(tower, i, B):
-    """NHWC [B, OH, OW, nf] view of the kernels' stored activation of conv i."""
-    c = tower.convs[i]
-    h = tower.hconv[i]
-    if tower.shift_mode and i + 1 < len(tower.convs) and tower.convs[i + 1].stride > 1:
-        s = tower.convs[i + 1].stride
-        return R.depth_to_space(h[:B].view(B, c.OH // s, c.OW // s, s * s * c.nf), s)
-    return h.reshape(-1)[:B * c.P * c.nf].view(B, c.OH, c.OW, c.nf)
-
-
-def _pads(c):
-    if not c.same:
-        return 0, 0
-    return max((c.OH - 1) * c.stride + c.rf - c.H, 0) // 2, max((c.OW - 1) * c.stride + c.rf - c.W, 0) // 2
-
-
-def _reference(tower, imgs, Ws, bs, masks, dlat, B, rnd=True):
-    """float64 forward through the conv stack (+ fc1) with the given weights and ReLU masks; returns the last layer's
-    pre-activation and the pre-activations of every conv.  Backward: d(sum(pre_last * dlat) / B)."""
-    a = imgs
-    pres = []
-    nconv = len(tower.convs)
-    for i, c in enumerate(tower.convs):
-        pre = R.conv2d(a, Ws[i], (c.stride, c.stride), _pads(c), c.OH, c.OW) + bs[i]
-        pres.append(pre)
-        if i + 1 == nconv and not tower.fcs:
-            return pre.reshape(B, -1), pres
-        a = pre * masks[i]
-        if rnd:                                   # the kernels store activations in fp16
-            a = a + (a.half().double() - a).detach()
-    flat = a.reshape(B, -1)
-    return flat @ Ws[nconv] + bs[nconv], pres
 
 
 @pytest.mark.parametrize("B", [37, 300])

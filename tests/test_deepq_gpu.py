@@ -74,6 +74,8 @@ def test_dqn_train_step_matches_oracle(network, ob_shape, dtype, dueling):
         assert (num / den) ** 0.5 < 5e-2, (it, (num / den) ** 0.5, per)
         p, po = model.q.store.export_tf("params"), {k: v.numpy() for k, v in oracle.tp.items()}
         err = max(float(np.abs(p[k] - po[k]).max()) for k in p)
+        # the reference's tolerance.  One Adam step moves each element by at most ~lr whatever the gradient, so this
+        # bounds the step and cannot detect a gradient error (see test_update_composition_gpu.py)
         assert err < 3e-3, (it, err)
         if it == 1:
             model.update_target()

@@ -143,7 +143,10 @@ def test_train_step_matches_oracle(name):
         p, po = model.get_params(), oracle.params_np()
         err = max(float(np.abs(p[k] - po[k]).max()) for k in p)
         worst = max(worst, err)
-        assert err < 3e-3, (it, err)                                       # test_microbatches.py:31-32 tolerance
+        # test_microbatches.py:31-32 tolerance.  Adam moves each element by at most ~lr per step whatever the
+        # gradient, so this bounds the step and cannot detect a gradient error; every tensor's gradient and the Adam
+        # step are checked in test_update_composition_gpu.py
+        assert err < 3e-3, (it, err)
     print(f"[{name}] max |param - oracle| after 3 steps = {worst:.3e}")
 
 

@@ -81,7 +81,9 @@ def test_bench_shaped_multichunk_multiminibatch_update_matches_oracle():
     p, po = model.get_params(), oracle.params_np()
     err = max(float(np.abs(p[n_] - po[n_]).max()) for n_ in p)
     print(f"bench-shaped update: {k} minibatches x 3 chunks, max |param - oracle| = {err:.3e}")
-    assert err < 3e-3, err                                              # ppo2/test_microbatches.py:31-32 tolerance
+    # ppo2/test_microbatches.py:31-32 tolerance.  Adam moves each element by at most ~lr per step whatever the
+    # gradient, so this bounds the steps and cannot detect a gradient error (see test_update_composition_gpu.py)
+    assert err < 3e-3, err
 
 
 @pytest.mark.parametrize("B", [8192])
