@@ -87,6 +87,33 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// ------------------------------------------------------------------ thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+  uint32_t n;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+  return n;
+}
+// every thread of every CTA of the cluster arrives (release) and waits (acquire)
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at `bar`'s shared-memory offset in CTA `rank` of the cluster.  Default (CTA-scope) release:
+// a cluster-scope release compiles to a GPU-wide MEMBAR in front of every arrival.  Releasing a stage needs none:
+// the reads it orders are the caller's wgmma operand reads, complete once wgmma.wait_group returns.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(rank)
+      : "memory");
+}
+
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -105,6 +132,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
+}
+// tma_load_2d into the same shared-memory offset of every CTA of the cluster in `mask` (bit r: rank r); each
+// destination's barrier at `bar`'s offset receives the box's bytes
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0,
+                                                      int c1, uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
 }
 // 1-D bulk copy global -> shared (no tensor map)
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {

@@ -11,7 +11,8 @@
 //                                       dX[m, :] = ( sum_t dY[m - sh_t, :] * W_t ) * (saved activation > 0)
 //   conv_shift_wgrad_kernel (MN-major): G[t, c, n] += alpha * sum_m X[m + sh_t, c] * dY[m, n]         wgrad
 //                                       (a CTA keeps the accumulators of up to 2*QW taps x 64 channels in registers;
-//                                        X and dY are read once per such group of taps)
+//                                        where clusters tile the SMs, the CTAs of the tap groups of one row range
+//                                        form a cluster and share each X / dY stage by TMA multicast)
 //
 // Warp roles: warps 0-7 are two consumer warpgroups (they issue the wgmma.mma_async chains, and run the epilogue --
 // or, in the wgrad, the fused bias-gradient sums -- from their own registers) | warp 8 TMA loads | uint8-fed first
@@ -500,6 +501,14 @@ struct ShiftWgradParams {
 
 // blockIdx.x: a run of k-blocks (reduction rows); blockIdx.y: a group of 2*QW 64-row accumulator chunks
 // q = (tap, h) of G.  Both operands are MN-major: X[rows, 64 channels] (shifted per tap) and dY[rows, N].
+//
+// TMA-fed instances may run as clusters of (1, g, 1) CTAs: g chunk groups of the same row range, so the same k-blocks
+// (every CTA of a cluster has the same blockIdx.x, hence the same kb0..kb1).  A stage is then loaded once per cluster:
+// its TMA boxes (the KH X halves, then the dY tile) are dealt round-robin to the cluster's producers, each box
+// multicast into every CTA.  Each CTA's full barrier still expects the whole stage's bytes; its empty barrier counts the
+// 8 consumer warps of every CTA (8*g arrivals), since a producer's boxes overwrite the stage in all of them.  The
+// cluster synchronises after the barriers are initialised (peers arrive on them and multicast into them) and before
+// exit (a peer's consumers may still arrive on this CTA's empty barriers).
 template <int BN, int KH, bool U8>
 __global__ void __launch_bounds__(sh_threads(U8), 1)
 conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmD,
@@ -529,18 +538,20 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   const int kb0 = blockIdx.x * p.kb_per_cta;
   const int kb1 = min(kb0 + p.kb_per_cta, p.kb_total);
   const int nchunks = p.taps * p.kx * KH;
+  const uint32_t ncta = U8 ? 1u : cluster_nctarank();        // the uint8-fed instance never runs as a cluster
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], U8 ? 1 + Ring::UPT : 1);
       // ring: a k-block also reads the first unit of the next stage; both groups finish k-blocks in order, so the
       // next stage's own k-block releasing it implies this one is done too
-      mbar_init(&empty_bar[s], SH_CONSUMER_WARPS);
+      mbar_init(&empty_bar[s], SH_CONSUMER_WARPS * ncta);
       if (U8) mbar_init(&head_bar[s], 1);
     }
     fence_barrier_init();
   }
-  __syncthreads();
+  if (ncta > 1) cluster_sync();
+  else __syncthreads();
 
   if (warp == SH_TMA_WARP) {
     if (elect_one()) {
@@ -548,18 +559,27 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
       tma_prefetch_desc(&tmD);
     }
     __syncwarp();
+    const uint32_t rank = U8 ? 0u : cluster_ctarank();
+    const uint16_t mask = (uint16_t)((1u << ncta) - 1u);
     int s = 0;
     uint32_t ph = 0;
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&empty_bar[s], ph ^ 1);
       if (elect_one()) {
         uint8_t* sa = smem + s * A_PITCH;
+        uint8_t* sb = smem + B_BASE + s * B_PITCH;
         mbar_arrive_expect_tx(&full_bar[s], (uint32_t)((U8 ? 0 : KH * SH_WABYTES) + B_BYTES));
-        if (!U8) {
-#pragma unroll
-          for (int h = 0; h < KH; ++h) tma_load_2d(sa + h * SH_WABYTES, &tmX, &full_bar[s], h * 64, kb * KR);
+        if (U8) {
+          tma_load_2d(sb, &tmD, &full_bar[s], 0, kb * KR);
+        } else {
+          // box b < KH: X half b; box KH: the dY tile.  This CTA loads boxes rank, rank + ncta, ...
+          for (int b = (int)rank; b <= KH; b += (int)ncta) {
+            void* dst = b < KH ? (void*)(sa + b * SH_WABYTES) : (void*)sb;
+            const CUtensorMap* tm = b < KH ? &tmX : &tmD;
+            if (ncta == 1) tma_load_2d(dst, tm, &full_bar[s], b < KH ? b * 64 : 0, kb * KR);
+            else tma_load_2d_multicast(dst, tm, &full_bar[s], b < KH ? b * 64 : 0, kb * KR, mask);
+          }
         }
-        tma_load_2d(smem + B_BASE + s * B_PITCH, &tmD, &full_bar[s], 0, kb * KR);
       }
       __syncwarp();
       if (++s == STAGES) { s = 0; ph ^= 1; }
@@ -628,7 +648,11 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
       }
       wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[s]);
+      if (U8 || ncta == 1) {
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+      } else if (lane < (int)ncta) {
+        mbar_arrive_cluster(&empty_bar[s], (uint32_t)lane);     // lane r releases the stage in CTA r of the cluster
+      }
 #pragma unroll
       for (int i = 0; i < QW; ++i)
 #pragma unroll
@@ -668,6 +692,7 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
       }
     }
   }
+  if (ncta > 1) cluster_sync();
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -706,6 +731,18 @@ static int launch_fwd(const CUtensorMap& tmX, const CUtensorMap& tmW, const Shif
   return check_launch("conv_shift_fwd_kernel");
 }
 
+// CTAs per cluster of the weight gradient: the largest divisor of the chunk-group count (grid.y) up to the portable
+// cluster size 8
+static int wgrad_cluster(int groups) {
+  int g = groups < 8 ? groups : 8;
+  while (groups % g) --g;
+  return g;
+}
+
+// grid.x: row ranges (k-block runs); grid.y: chunk groups.  The chunk groups of a row range run as one cluster when
+// clusters of that size tile the SMs.  Otherwise they do not cluster: a cluster's CTAs share one GPC, so clusters of 3
+// fit only 117 of an H100's 132 SMs at this kernel's shared memory, and the SMs left idle cost more than the operand
+// reads a cluster saves (measured: c3 of cfg-2 slower as clusters of 3).
 template <int BN, int KH, bool U8 = false>
 static int launch_wgrad(const CUtensorMap& tmX, const CUtensorMap& tmD, const ShiftWgradParams& p, dim3 grid,
                         cudaStream_t st) {
@@ -717,6 +754,7 @@ static int launch_wgrad(const CUtensorMap& tmX, const CUtensorMap& tmD, const Sh
       (U8 ? U8Ring<KR, STAGES>::BYTES + STAGES * B_REGION : STAGES * (KH * SH_WABYTES + B_REGION)) + 1024 + 512;
   static_assert(SMEM <= 227 * 1024, "conv_shift_wgrad: shared memory budget");
   static bool attr = false;
+  static int co_resident[9] = {};                 // clusters of g CTAs that fit on the device at once, per g
   auto kern = conv_shift_wgrad_kernel<BN, KH, U8>;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
@@ -726,8 +764,38 @@ static int launch_wgrad(const CUtensorMap& tmX, const CUtensorMap& tmD, const Sh
     }
     attr = true;
   }
-  kern<<<grid, sh_threads(U8), SMEM, st>>>(tmX, tmD, p);
-  return check_launch("conv_shift_wgrad_kernel");
+  int g = U8 ? 1 : wgrad_cluster((int)grid.y);
+  cudaLaunchAttribute cl;
+  cl.id = cudaLaunchAttributeClusterDimension;
+  cl.val.clusterDim.x = 1;
+  cl.val.clusterDim.y = (unsigned)g;
+  cl.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(sh_threads(U8));
+  cfg.dynamicSmemBytes = SMEM;
+  cfg.stream = st;
+  cfg.attrs = &cl;
+  cfg.numAttrs = 1;
+  if (g > 1) {
+    if (co_resident[g] == 0) {
+      cudaError_t e = cudaOccupancyMaxActiveClusters(&co_resident[g], kern, &cfg);
+      if (e != cudaSuccess) {
+        set_last_error("conv_shift_wgrad: cluster occupancy (%d CTAs): %s", g, cudaGetErrorString(e));
+        co_resident[g] = 0;
+        return B200RL_ERR_CUDA;
+      }
+    }
+    if (co_resident[g] * g < device_num_sms()) g = 1;
+  }
+  cfg.numAttrs = g > 1 ? 1 : 0;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tmX, tmD, p);
+  const int rc = check_launch("conv_shift_wgrad_kernel");
+  if (rc == B200RL_OK && e != cudaSuccess) {
+    set_last_error("conv_shift_wgrad_kernel: %s", cudaGetErrorString(e));
+    return B200RL_ERR_CUDA;
+  }
+  return rc;
 }
 
 static int ilog2(int v) { int l = 0; while ((1 << l) < v) ++l; return l; }
