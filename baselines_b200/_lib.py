@@ -45,7 +45,7 @@ SIGNATURES = {
     "b200rl_cast_transpose": [_p, _i, _i, _p, _ll, _p, _ll, _f, _p],
     "b200rl_cast_transpose_batch": [_p, _i, _i, _i, _p],
     "b200rl_cast_f32_f16": [_p, _p, _ll, _i, _ll, _ll, _f, _p],
-    "b200rl_obs_encode": [_p, _p, _ll, _i, _i, _i, _p, _p, _f, _f, _i, _p, _i, _p, _p],
+    "b200rl_obs_encode": [_p, _p, _ll, _i, _i, _i, _p, _p, _f, _f, _i, _p, _i, _p, _p, _p],
     "b200rl_tree_set": [_p, _p, _ll, _p, _p, _i, _p],
     "b200rl_tree_range_sum": [_p, _ll, _ll, _ll, _p, _p],
     "b200rl_per_sample": [_p, _p, _ll, _ll, _p, _i, _d, _p, _p, _p, _p],

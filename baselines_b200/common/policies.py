@@ -287,6 +287,10 @@ class PolicyNet:
         B = t.shape[0]
         return t.reshape(B, -1).to(torch.float32).to(self.device, non_blocking=True).contiguous()
 
+    def check_obs_range(self, flag=None):
+        """ValueError if an observation encoded since the last check was beyond fp16 (nn.Tower.check_obs_range)."""
+        self.tower_pi.check_obs_range(flag)
+
     def forward(self, x, B, src_idx=None, masks=True):
         """Towers + heads for B samples of x (optionally gathered through src_idx); masks=False: no backward follows."""
         if self.fuse0:

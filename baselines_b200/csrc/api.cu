@@ -64,7 +64,7 @@ int cast_transpose_impl(const float*, int, int, void*, long long, void*, long lo
 int cast_f32_f16_impl(const float*, void*, long long, int, long long, long long, float, cudaStream_t);
 int cast_transpose_batch_impl(const void*, int, int, int, cudaStream_t);
 int obs_encode_impl(const float*, const long long*, long long, int, int, int, const float*, const float*, float, float,
-                    int, const int*, int, void*, cudaStream_t);
+                    int, const int*, int, void*, int*, cudaStream_t);
 int tree_set_impl(double*, double*, long long, const long long*, const double*, int, cudaStream_t);
 int tree_range_sum_impl(const double*, long long, long long, long long, double*, cudaStream_t);
 int per_sample_impl(const double*, const double*, long long, long long, const double*, int, double, long long*,
@@ -246,9 +246,9 @@ int b200rl_cast_f32_f16(const float* src, void* dst, long long rows, int cols, l
 // common/input.py:43-63 encode_observation (Discrete :54-55, MultiDiscrete :58-61), policies.py:182-185
 int b200rl_obs_encode(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim, int in_pad,
                       const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n,
-                      const int* seg_off, int nseg, void* out, void* stream) {
+                      const int* seg_off, int nseg, void* out, int* overflow, void* stream) {
   return obs_encode_impl(x, src_idx, B, raw_dim, in_dim, in_pad, mean, inv_std, clip_lo, clip_hi, onehot_n, seg_off,
-                         nseg, out, S(stream));
+                         nseg, out, overflow, S(stream));
 }
 
 int b200rl_tree_set(double* sum_tree, double* min_tree, long long capacity, const long long* idx, const double* vals,

@@ -3,7 +3,12 @@
 //
 // The reference keeps observations in float32 end to end (tf.to_float, no narrowing).  The tensor cores take fp16
 // operands, so every encoded value v is emitted as an fp16 PAIR
-//     hi = fp16(v),  lo = fp16(v - hi)          (v - hi is exact in fp32; |v - (hi + lo)| <= 2^-22 |v|)
+//     hi = fp16(v),  lo = fp16(v - hi)          (v - hi is exact in fp32)
+// whose sum hi + lo differs from v by at most 2^-22 |v| while lo is an fp16 normal (|v| >= 2^-3 roughly) and by at most
+// 2^-25 (half of lo's subnormal spacing 2^-24) below that.  fp16 ends at 65504: an encoded |v| >= 65520 rounds hi to
+// +-inf (and lo to -+inf), which the first GEMM turns into NaN.  Such values set *overflow (when given); the host
+// raises at its next synchronisation (common/policies.py PolicyNet.check_obs_range) instead of acting on NaN.  Values
+// below the limit are encoded exactly as without the flag.
 // laid out side by side as one operand row [hi(0..in_pad) | lo(0..in_pad)].  The first GEMM runs over K = 2*in_pad
 // against the weight matrix stacked twice ([W ; W]), i.e. x.W = hi.W + lo.W accumulated in fp32: the observation
 // itself is no longer quantised to 11 bits.  Discrete observations become exact one-hot rows (lo = 0); a MultiDiscrete
@@ -25,6 +30,7 @@ struct ObsEncodeParams {
   const int* seg_off;        // optional [nseg + 1] one-hot block offsets (MultiDiscrete); null: one block [0, onehot_n)
   int nseg;
   __half* out;               // [B, 2 * in_pad]
+  int* overflow;             // optional: set to 1 when an encoded value has |v| >= 65520 (beyond fp16)
 };
 
 __global__ void __launch_bounds__(256) obs_encode_kernel(const ObsEncodeParams p) {
@@ -66,6 +72,12 @@ __global__ void __launch_bounds__(256) obs_encode_kernel(const ObsEncodeParams p
         }
         v[j] = t;
       }
+      if (p.overflow) {
+        bool over = false;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) over |= fabsf(v[j]) >= 65520.0f;    // NaN compares false: it passes through
+        if (over) *p.overflow = 1;
+      }
     }
     __align__(16) __half hi[8], lo[8];
 #pragma unroll
@@ -81,7 +93,7 @@ __global__ void __launch_bounds__(256) obs_encode_kernel(const ObsEncodeParams p
 
 int obs_encode_impl(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim, int in_pad,
                     const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n,
-                    const int* seg_off, int nseg, void* out, cudaStream_t stream) {
+                    const int* seg_off, int nseg, void* out, int* overflow, cudaStream_t stream) {
   B200RL_REQUIRE(x && out && B > 0, "obs_encode: null operand");
   B200RL_REQUIRE(in_pad % 8 == 0 && in_pad >= in_dim && in_dim > 0, "obs_encode: in_pad must be a multiple of 8 >= in_dim");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "obs_encode: output must be 16-byte aligned");
@@ -94,7 +106,7 @@ int obs_encode_impl(const float* x, const long long* src_idx, long long B, int r
   else
     B200RL_REQUIRE(raw_dim == in_dim, "obs_encode: raw_dim != in_dim");
   ObsEncodeParams p{x, src_idx, B, raw_dim, in_dim, in_pad, mean, inv_std, clip_lo, clip_hi, onehot_n,
-                    onehot_n > 0 ? seg_off : nullptr, nseg, reinterpret_cast<__half*>(out)};
+                    onehot_n > 0 ? seg_off : nullptr, nseg, reinterpret_cast<__half*>(out), overflow};
   const long long total = B * (in_pad / 8);
   long long blocks = (total + 255) / 256;
   if (blocks > 16LL * device_num_sms()) blocks = 16LL * device_num_sms();

@@ -238,8 +238,11 @@ class DQNModel:
             out = self.q.forward(x, B)[:B].clone()
             A = out[:, :self.nA]
             if self.q.dueling:
-                return (out[:, self.nA:self.nA + 1] + (A - A.mean(dim=1, keepdim=True))).cpu().numpy()
-            return A.cpu().numpy()
+                out = (out[:, self.nA:self.nA + 1] + (A - A.mean(dim=1, keepdim=True))).cpu().numpy()
+            else:
+                out = A.cpu().numpy()
+            self.q.trunk.check_obs_range()
+            return out
 
     def train_device(self, obs_t, obs_tp1, actions, rewards, dones, weights, idx, B, lr=None):
         """One step of build_graph.py:380-444 on device-resident arrays.  obs_* / actions / rewards / dones are the
@@ -286,8 +289,9 @@ def build_act(model):
             model.eps = float(update_eps)
         with torch.cuda.device(model.device):
             x = torch.as_tensor(np.ascontiguousarray(ob)).to(model.device)
-            a = model.act_device(x, x.shape[0], model.eps if stochastic else 0.0)
-            return a.cpu().numpy()
+            a = model.act_device(x, x.shape[0], model.eps if stochastic else 0.0).cpu().numpy()
+            model.q.trunk.check_obs_range()
+            return a
     return act
 
 

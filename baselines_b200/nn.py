@@ -477,6 +477,8 @@ class Tower:
         self.ld_hfc = [l.Np for l in self.fcs]         # row pitch of hfc[i] / dzfc[i] (a fused first layer widens [0])
         if self.kind == "mlp":
             self.x0 = torch.zeros(cap, 2 * self.in_pad, **f16)      # [hi | lo] operand rows of the float32 observations
+            # set by the encoder when an observation value is beyond fp16 (|v| >= 65520); see check_obs_range
+            self.obs_overflow = torch.zeros(1, dtype=torch.int32, device=dev)
             self.ob_seg = ops.segment_table(self.onehot_nvec, dev) if self.onehot_nvec else None
         # where the heads write d(loss)/d(latent pre-activation)
         if self.fcs:
@@ -576,8 +578,22 @@ class Tower:
         nm = self.obs_norm
         ops.obs_encode(x, self.x0, B, self.raw_dim, self.in_dim, self.in_pad, src_idx=src_idx,
                        mean=nm[0] if nm else None, inv_std=nm[1] if nm else None,
-                       clip=(nm[2], nm[3]) if nm else (0.0, 0.0), onehot_n=self.onehot_n, seg_off=self.ob_seg)
+                       clip=(nm[2], nm[3]) if nm else (0.0, 0.0), onehot_n=self.onehot_n, seg_off=self.ob_seg,
+                       overflow=self.obs_overflow)
         return self.x0
+
+    def check_obs_range(self, flag=None):
+        """Raise ValueError when an encoded observation value was beyond fp16 since the last check: its hi/lo pair is
+        +-inf and the network output NaN.  Reads the device flag (a synchronisation) unless the caller passes a host
+        copy of it; clears the flag before raising."""
+        if self.kind != "mlp":
+            return
+        if flag is None:
+            flag = int(self.obs_overflow.item())
+        if flag:
+            self.obs_overflow.zero_()
+            raise ValueError("observation values must satisfy |v| < 65520 after normalisation: the encoder splits "
+                             "each float32 value into two fp16 halves, and fp16 ends at 65504")
 
     def forward(self, x, B, src_idx=None, encoded=None, masks=True, skip_first=False):
         """encoded (mlp only): operand rows another tower already produced from the same observations.

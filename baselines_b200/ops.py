@@ -397,17 +397,20 @@ def cast_f32_f16(src, dst, rows, cols, ld_src, ld_dst, scale=1.0):
 
 
 def obs_encode(x, out, B, raw_dim, in_dim, in_pad, src_idx=None, mean=None, inv_std=None, clip=(-5.0, 5.0), onehot_n=0,
-               seg_off=None):
+               seg_off=None, overflow=None):
     """float32 observation rows -> fp16 [hi | lo] operand rows (input.py:43-63, policies.py:182-185, ppo2.py:165).
-    onehot_n with seg_off (segment_table(nvec)): MultiDiscrete rows of len(nvec) integers -> concatenated one-hot."""
+    onehot_n with seg_off (segment_table(nvec)): MultiDiscrete rows of len(nvec) integers -> concatenated one-hot.
+    overflow: optional int32 device scalar, set to 1 when an encoded value has |v| >= 65520 (beyond fp16)."""
     _chk(x, torch.float32, "x")
     _chk(out, torch.float16, "out")
     _chk(src_idx, torch.int64, "src_idx")
     _chk(mean, torch.float32, "mean")
     _chk(inv_std, torch.float32, "inv_std")
+    _chk(overflow, torch.int32, "overflow")
     so, nseg = _seg_args(seg_off)
     _lib.call("b200rl_obs_encode", _ptr(x), _ptr(src_idx), int(B), int(raw_dim), int(in_dim), int(in_pad), _ptr(mean),
-              _ptr(inv_std), float(clip[0]), float(clip[1]), int(onehot_n), so, nseg, _ptr(out), _stream(),
+              _ptr(inv_std), float(clip[0]), float(clip[1]), int(onehot_n), so, nseg, _ptr(out), _ptr(overflow),
+              _stream(),
               label="obs_encode", nbytes=float(B) * (4.0 * raw_dim + 4.0 * in_pad))
 
 

@@ -82,7 +82,9 @@ class Model(object):
             a, v, n = self._bufs(B)
             nz = None if noise is None else torch.as_tensor(np.ascontiguousarray(noise), dtype=torch.float32).to(self.device)
             self.step_device(x, a, v, n, noise=nz)
-            return self.net.actions_to_numpy(a), v.cpu().numpy(), None, n.cpu().numpy()
+            out = self.net.actions_to_numpy(a), v.cpu().numpy(), None, n.cpu().numpy()
+            self.net.check_obs_range()
+            return out
 
     def value(self, ob, *args, **kwargs):
         with torch.cuda.device(self.device):
@@ -90,7 +92,9 @@ class Model(object):
             B = x.shape[0]
             _, v, _ = self._bufs(B)
             self.value_device(x, v)
-            return v.cpu().numpy()
+            out = v.cpu().numpy()
+            self.net.check_obs_range()
+            return out
 
     def _bufs(self, B):
         if B <= self._act_v.shape[0]:
@@ -182,7 +186,9 @@ class Model(object):
             a = torch.as_tensor(np.ascontiguousarray(actions), dtype=self.net.action_dtype).to(dev).contiguous()
             f = lambda z: torch.as_tensor(np.ascontiguousarray(z), dtype=torch.float32).to(dev)
             st = self.train_rollout(float(lr), float(cliprange), x, a, f(returns), f(values), f(neglogpacs), None)
-            return [float(s) for s in st.cpu().numpy()]
+            out = [float(s) for s in st.cpu().numpy()]
+            self.net.check_obs_range()
+            return out
 
     # ------------------------------------------------------------------------------------ checkpoints
     def save(self, save_path):

@@ -98,6 +98,12 @@ class Runner:
             self._f32_pin = torch.zeros(nenv, net.tower_pi.raw_dim, dtype=torch.float32)
             if pin:
                 self._f32_pin = self._f32_pin.pin_memory()
+        # host copy of the encoder's out-of-range flag (vector observations), read after a synchronisation the runner
+        # makes anyway: per step with a host env, at the start of the next rollout with a device env
+        self._over_pin = torch.zeros(1, dtype=torch.int32)
+        if pin:
+            self._over_pin = self._over_pin.pin_memory()
+        self._over_ev = torch.cuda.Event()
         self._f32_sync = torch.cuda.Event()
         self._ro_copied = torch.cuda.Event()          # end-of-rollout H2D copies of the pinned reward / done staging
         self._cur = torch.zeros((nenv,) + store_shape, dtype=self.rollout.obs.dtype, device=self.device)
@@ -212,6 +218,11 @@ class Runner:
             # the previous rollout's asynchronous upload of _rew_host / _done_host must have read the staging buffers
             # before this rollout overwrites row 0 (callers need not synchronise between run_device calls)
             self._ro_copied.synchronize()
+            if not self.u8:                    # the previous rollout's flag (device envs)
+                self._over_ev.synchronize()
+                flag = int(self._over_pin[0])
+                self._over_pin.zero_()
+                model.net.check_obs_range(flag)
             if self.fs:
                 ro.obs[0].copy_(self._cur)
             chunked = self.fs and self.act_chunks > 1 and nz is None
@@ -230,7 +241,11 @@ class Runner:
                     continue
                 self._done_host[t] = torch.from_numpy(self.dones.astype(np.uint8))       # mb_dones.append(self.dones)
                 self._act_pin.copy_(ro.actions[t], non_blocking=True)
+                if not self.u8:
+                    self._over_pin.copy_(model.net.tower_pi.obs_overflow, non_blocking=True)
                 torch.cuda.current_stream().synchronize()
+                if not self.u8:
+                    model.net.check_obs_range(int(self._over_pin[0]))
                 actions = self._act_pin.numpy()
                 if self.model.net.pd == "mcat":
                     actions = actions.astype(np.int32)                      # distributions.py:222 tf.int32
@@ -257,6 +272,9 @@ class Runner:
             model.value_device(self._cur, ro.last_values, persistent=True)
             if self.device_env:
                 ro.last_dones.copy_(self._dev_dones)
+                if not self.u8:
+                    self._over_pin.copy_(model.net.tower_pi.obs_overflow, non_blocking=True)
+                    self._over_ev.record()
             else:
                 ro.rewards.copy_(self._rew_host, non_blocking=True)
                 ro.dones.copy_(self._done_host, non_blocking=True)

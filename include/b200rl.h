@@ -197,13 +197,15 @@ int b200rl_cast_f32_f16(const float* src, void* dst, long long rows, int cols, l
 /* Vector-observation encoding: common/input.py:43-63 (Box -> to_float, Discrete -> one_hot), the optional
  * clip((x - mean) / std, lo, hi) of common/policies.py:182-185, and the minibatch row gather of ppo2/ppo2.py:165.
  * x: float32 [*, raw_dim]; out: fp16 [B, 2*in_pad] = [hi | lo] with hi = fp16(v), lo = fp16(v - hi), so the first
- * GEMM (K = 2*in_pad against [W ; W]) sees the float32 observation to 2^-22 instead of an fp16-rounded copy.
+ * GEMM (K = 2*in_pad against [W ; W]) sees the float32 observation to 2^-22 relative (2^-25 absolute once lo is
+ * fp16-subnormal, |v| < ~2^-3) instead of an fp16-rounded copy.  overflow (optional device int): set to 1 when an
+ * encoded value has |v| >= 65520, which fp16 cannot hold (hi = +-inf); the caller must not use that output.
  * onehot_n > 0: x holds the Discrete value (raw_dim = 1), out row = one_hot(x, n).
  * onehot_n > 0 with seg_off (device int32 [nseg + 1]): x holds a MultiDiscrete value (raw_dim = nseg integers), out
  * row = concat_s one_hot(x[s], seg_off[s+1] - seg_off[s]) of width onehot_n = seg_off[nseg] (input.py:58-61). */
 int b200rl_obs_encode(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim, int in_pad,
                       const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n,
-                      const int* seg_off, int nseg, void* out, void* stream);
+                      const int* seg_off, int nseg, void* out, int* overflow, void* stream);
 
 /* prioritized replay: common/segment_tree.py:76-86 (__setitem__), :51-74 (reduce), :105-131
  * (find_prefixsum_idx); deepq/replay_buffer.py:107-115 (_sample_proportional), :157-165 (weights),

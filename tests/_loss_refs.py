@@ -236,3 +236,47 @@ def adam_tf(p, g, m, v, lr_t, beta1, beta2, eps):
 def clip_scale(sumsq, clip):
     """tf.clip_by_global_norm / tf.clip_by_norm factor clip / max(||g||, clip); 1 when clip <= 0."""
     return 1.0 if clip <= 0 else clip / max(float(np.sqrt(sumsq)), clip)
+
+
+# ------------------------------------------------------------------------------------------------ sampler streams
+_M32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(seed, rows, ctr, stream):
+    """The acting samplers' Philox4x32-10 (csrc/policy_heads.cu philox4) on the host: counter (row lo, row hi, ctr,
+    stream), key = seed.  rows: int array; returns uint32 [len(rows), 4]."""
+    r = np.asarray(rows, np.uint64)
+    c = [r & _M32, r >> np.uint64(32), np.full_like(r, ctr), np.full_like(r, stream)]
+    k0, k1 = np.uint64(seed & 0xFFFFFFFF), np.uint64((seed >> 32) & 0xFFFFFFFF)
+    for _ in range(10):
+        p0, p1 = np.uint64(0xD2511F53) * c[0], np.uint64(0xCD9E8D57) * c[2]
+        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & _M32, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & _M32]
+        k0, k1 = (k0 + np.uint64(0x9E3779B9)) & _M32, (k1 + np.uint64(0xBB67AE85)) & _M32
+    return np.stack(c, 1).astype(np.uint32)
+
+
+def philox_uniforms(seed, B, n, offset):
+    """float32 [B, n]: uniform j of row b of an acting pass at stream position `offset` -- word j % 4 of counter j // 4,
+    mapped to the open interval as u01_open does (fp32 arithmetic, as on the device)."""
+    out = np.empty((B, n), np.float32)
+    for c in range(-(-n // 4)):
+        w = philox4x32_10(seed, np.arange(B), c, offset)
+        for i in range(4):
+            if 4 * c + i < n:
+                out[:, 4 * c + i] = ((w[:, i] >> 8).astype(np.float32) + np.float32(0.5)) * np.float32(2.0 ** -24)
+    return out
+
+
+def dqn_act_draws(seed, step, B, nA):
+    """The DQN act kernel's splitmix64 draws (csrc/replay.cu dqn_act_kernel) for rows 0..B-1 at `step`: (u float32 in
+    (0, 1), the random action in [0, nA))."""
+    m = (1 << 64) - 1
+    us, rs = np.empty(B, np.float32), np.empty(B, np.int64)
+    for b in range(B):
+        x = (seed + 0x9E3779B97F4A7C15 * ((step * 1315423911 + b + 1) & m)) & m
+        x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & m
+        x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & m
+        x ^= x >> 31
+        us[b] = (np.float32(x >> 40) + np.float32(0.5)) * np.float32(2.0 ** -24)
+        rs[b] = (x & 0xFFFFFF) % nA
+    return us, rs

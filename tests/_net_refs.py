@@ -14,8 +14,9 @@ rnd=True evaluates what the kernels evaluate:
   * tanh' taken as 1 - s^2 from the stored fp16 activation s;
   * every stored pre-activation gradient (the data-gradient GEMMs' fp16 outputs) rounded to fp16 in the backward;
   * ReLU decisions taken from `masks` (name -> 0/1 tensor shaped like the pre-activation) where the caller supplies
-    them, e.g. from the kernels' own stored activations;
-  * mlp observations kept in float32: the encoder's fp16 hi/lo split loses at most 2^-22 relative.
+    them, e.g. from the kernels' own stored activations; for a tanh layer `masks[name]` is the stored activation itself,
+    which replaces the mirror's in the forward (the backward keeps the mirror's 1 - s^2);
+  * mlp observations kept in float32: the encoder's fp16 hi/lo split loses at most max(2^-22 |v|, 2^-25).
 
 absolute=True evaluates the same network on |x|, |W|, |b| and |seed| with the ReLU masks and stored tanh activations of
 a signed run (`ref_acts`): a tanh layer outputs |s| and passes the gradient through |1 - s^2|.  Its outputs and
@@ -147,6 +148,9 @@ class _Net:
                 a = pre + (a - pre).detach()
             return a + (a.half().double() - a).detach() if self.rnd else a
         s = _StoredTanh.apply(pre, self.rnd, name in self.no_dact)
+        m = self.masks.get(name)
+        if m is not None:                               # the kernels' stored activation (forward value only)
+            s = s + (m.double() - s).detach()
         self.acts[name] = s.detach()
         return s
 

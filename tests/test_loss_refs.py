@@ -174,3 +174,23 @@ def test_adam_and_moments_helpers():
     d = (R - V).astype(np.float64)
     assert math.isclose(mean, d.mean(), rel_tol=1e-13) and math.isclose(std, d.std(), rel_tol=1e-13)
     assert lr.clip_scale(25.0, 5.0) == 1.0 and lr.clip_scale(100.0, 5.0) == 0.5 and lr.clip_scale(1e9, 0.0) == 1.0
+
+
+def test_philox_helper_known_answers_and_uniform_layout():
+    """Philox4x32-10 known-answer vectors (Salmon et al., SC'11, Random123 kat_vectors), then the u01 mapping."""
+    got = lr.philox4x32_10(0, [0], 0, 0)[0]
+    assert [int(v) for v in got] == [0x6627E8D5, 0xE169C58D, 0xBC57AC4C, 0x9B00DBD8]
+    c = 0xFFFFFFFF
+    got = lr.philox4x32_10(c | (c << 32), [c | (c << 32)], c, c)[0]
+    assert [int(v) for v in got] == [0x408F276D, 0x41C83B0E, 0xA20BC7C6, 0x6D5451FD]
+    u = lr.philox_uniforms(7, 3, 6, 2)
+    w = lr.philox4x32_10(7, [1], 1, 2)[0]
+    assert u[1, 5] == np.float32(((int(w[1]) >> 8) + 0.5) / 2 ** 24)
+    assert u.dtype == np.float32 and (u > 0).all() and (u < 1).all()
+
+
+def test_dqn_act_draws_helper():
+    u, r = lr.dqn_act_draws(123, 4, 64, 6)
+    assert ((u > 0) & (u < 1)).all() and ((r >= 0) & (r < 6)).all()
+    u2, r2 = lr.dqn_act_draws(123, 5, 64, 6)
+    assert not np.array_equal(r, r2)                     # the stream moves with the step

@@ -189,3 +189,20 @@ def test_encode_obs_matches_oracle_normalisation():
     got = N.encode_obs(obs, mean=mean, inv_std=np.float32(1.0) / std)
     want = nets.encode_observation(obs, torch.float32, rms=rms).double().numpy()
     assert np.allclose(got, want, rtol=2 ** -22, atol=0) and (np.abs(want) == 5).any()
+
+
+@pytest.mark.parametrize("name", ["mlp13_cat15_l3_h20", "mlp11_gauss3_copy_l1_h32"])
+def test_policy_mirror_takes_stored_tanh_activations(name):
+    """A tanh layer's entry in `masks` replaces its stored activation in the forward: the mirror's own activations
+    reproduce its outputs exactly, and a changed activation reaches the heads."""
+    cfg, params, x, nout, rng = _ppo_case(name)
+    mcfg, ident = N.ppo_mirror_cfg(cfg), N.ppo_identity(cfg)
+    z, zv = np.zeros((len(x), nout)), np.zeros(len(x))
+    ref = N.policy_ref(params, mcfg, x, z, zv, rnd=True, identity=ident)
+    tanh_acts = {k: a for k, a in ref.acts.items() if "mlp_fc" in k}
+    same = N.policy_ref(params, mcfg, x, z, zv, rnd=True, masks=tanh_acts, identity=ident)
+    assert torch.equal(same.pi, ref.pi) and torch.equal(same.v, ref.v)
+    last = [k for k in tanh_acts if k.startswith("ppo2_model/pi/")][-1]
+    moved = dict(tanh_acts, **{last: tanh_acts[last] * 0.5})
+    other = N.policy_ref(params, mcfg, x, z, zv, rnd=True, masks=moved, identity=ident)
+    assert not torch.equal(other.pi, ref.pi)
