@@ -48,8 +48,9 @@ SIGNATURES = {
     "b200rl_obs_encode": [_p, _p, _ll, _i, _i, _i, _p, _p, _f, _f, _i, _p, _i, _p, _p, _p],
     "b200rl_tree_set": [_p, _p, _ll, _p, _p, _i, _p],
     "b200rl_tree_range_sum": [_p, _ll, _ll, _ll, _p, _p],
-    "b200rl_per_sample": [_p, _p, _ll, _ll, _p, _i, _d, _p, _p, _p, _p],
-    "b200rl_per_priorities": [_p, _i, _d, _d, _p, _p, _p],
+    "b200rl_per_sample": [_p, _p, _ll, _ll, _p, _i, _d, _p, _p, _p, _p, _p],
+    "b200rl_per_priorities": [_p, _i, _d, _d, _p, _p, _p, _p],
+    "b200rl_per_pow": [_p, _i, _d, _p, _p],
     "b200rl_dqn_td": [_p, _ll, _p, _ll, _p, _ll, _p, _ll, _p, _ll, _p, _ll, _i, _p, _p, _p, _p, _p, _f, _i, _p, _p,
                       _ll, _p, _ll, _p, _i, _p],
     "b200rl_dqn_act": [_p, _ll, _p, _ll, _i, _f, _ull, _ull, _p, _p, _p, _i, _p],

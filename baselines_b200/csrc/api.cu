@@ -68,8 +68,9 @@ int obs_encode_impl(const float*, const long long*, long long, int, int, int, co
 int tree_set_impl(double*, double*, long long, const long long*, const double*, int, cudaStream_t);
 int tree_range_sum_impl(const double*, long long, long long, long long, double*, cudaStream_t);
 int per_sample_impl(const double*, const double*, long long, long long, const double*, int, double, long long*,
-                    double*, float*, cudaStream_t);
-int per_priorities_impl(const float*, int, double, double, double*, double*, cudaStream_t);
+                    double*, float*, int*, cudaStream_t);
+int per_priorities_impl(const float*, int, double, double, double*, double*, int*, cudaStream_t);
+int per_pow_impl(const double*, int, double, double*, cudaStream_t);
 int dqn_td_impl(const float*, long long, const float*, long long, const float*, long long, const float*, long long,
                 const float*, long long, const float*, long long, int, const long long*, const long long*,
                 const float*, const float*, const float*, float, int, float*, void*, long long, void*, long long,
@@ -261,13 +262,16 @@ int b200rl_tree_range_sum(const double* tree, long long capacity, long long star
 }
 int b200rl_per_sample(const double* sum_tree, const double* min_tree, long long capacity, long long n_stored,
                       const double* uniforms, int batch, double beta, long long* idx_out, double* w_out,
-                      float* w_out_f32, void* stream) {
+                      float* w_out_f32, int* bad, void* stream) {
   return per_sample_impl(sum_tree, min_tree, capacity, n_stored, uniforms, batch, beta, idx_out, w_out, w_out_f32,
-                         S(stream));
+                         bad, S(stream));
 }
 int b200rl_per_priorities(const float* td, int n, double eps, double alpha, double* powered, double* max_priority,
-                          void* stream) {
-  return per_priorities_impl(td, n, eps, alpha, powered, max_priority, S(stream));
+                          int* bad, void* stream) {
+  return per_priorities_impl(td, n, eps, alpha, powered, max_priority, bad, S(stream));
+}
+int b200rl_per_pow(const double* x, int n, double y, double* out, void* stream) {
+  return per_pow_impl(x, n, y, out, S(stream));
 }
 int b200rl_dqn_td(const float* a_t, long long lda_t, const float* s_t, long long lds_t, const float* a_on,
                   long long lda_on, const float* s_on, long long lds_on, const float* a_tg, long long lda_tg,

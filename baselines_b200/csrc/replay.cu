@@ -6,7 +6,15 @@
 // recomputed as op(left child, right child), so after a batch of writes the trees are bit-identical
 // to the reference's sequential updates (last write to a duplicated index wins, as in the python loop).
 // Sampling is latency bound (batch x log2(capacity) dependent 8-byte reads that stay in L2).
+//
+// Priorities follow the reference's dtypes: its new priorities are |td| + eps on the float32 TD errors, so float32
+// values, and the leaves are float64 powers of them (priority ** alpha, NumPy 1.x scalar promotion).  Every pow here
+// (leaves, the add path's max_priority ** alpha, importance weights) is the correctly rounded pow_cr of pow_cr.cuh, so
+// the leaves and weights do not depend on which libm rounds them.  A priority that is not > 0 (the reference's
+// `assert priority > 0`, e.g. a NaN TD error) sets a sticky device flag that the buffer raises on; sampling never
+// returns an index outside the stored range, even from such a tree.
 #include "common.cuh"
+#include "pow_cr.cuh"
 
 namespace b200rl {
 
@@ -86,11 +94,16 @@ __global__ void tree_range_sum_kernel(const double* __restrict__ tree, long long
   if (threadIdx.x == 0 && blockIdx.x == 0) out[0] = fold_sum(tree, start, end_inclusive, 1, 0, capacity - 1);
 }
 
-// proportional stratified sampling + importance weights (replay_buffer.py:107-115,157-165)
+using powcr::pow_cr;
+
+// proportional stratified sampling + importance weights (replay_buffer.py:107-115,157-165).
+// bad (optional): set to 1 when the tree holds a priority that is not > 0 (NaN root sum, zero minimum) or the descent
+// ends past the stored range, which only such a tree can make it do; that slot returns index 0 instead.
 __global__ void __launch_bounds__(256)
 per_sample_kernel(const double* __restrict__ sum_tree, const double* __restrict__ min_tree, long long capacity,
                   long long n_stored, const double* __restrict__ uniforms, int batch, double beta,
-                  long long* __restrict__ idx_out, double* __restrict__ w_out, float* __restrict__ w_out_f32) {
+                  long long* __restrict__ idx_out, double* __restrict__ w_out, float* __restrict__ w_out_f32,
+                  int* __restrict__ bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= batch) return;
   // NOTE the reference's quirk: sum(0, len-1) has an EXCLUSIVE end, so the last stored element is dropped
@@ -103,27 +116,40 @@ per_sample_kernel(const double* __restrict__ sum_tree, const double* __restrict_
     if (left > mass) node = 2 * node;
     else { mass = __dsub_rn(mass, left); node = 2 * node + 1; }
   }
-  const long long leaf = node - capacity;
-  idx_out[i] = leaf;
+  long long leaf = node - capacity;
   const double total = sum_tree[1];
+  if (leaf >= n_stored || !(total > 0.0) || !(min_tree[1] > 0.0)) {
+    if (bad) *bad = 1;
+    if (leaf >= n_stored) { leaf = 0; node = capacity; }
+  }
+  idx_out[i] = leaf;
   const double p_min = min_tree[1] / total;
-  const double max_w = pow(p_min * (double)n_stored, -beta);
+  const double max_w = pow_cr(p_min * (double)n_stored, -beta);
   const double p = sum_tree[node] / total;
-  const double w = pow(p * (double)n_stored, -beta) / max_w;
+  const double w = pow_cr(p * (double)n_stored, -beta) / max_w;
   w_out[i] = w;
   if (w_out_f32) w_out_f32[i] = (float)w;
 }
 
-// new priorities from TD errors: (|td| + eps)^alpha, plus running max of the un-powered priority
+// new priorities from TD errors, deepq.py:302 + replay_buffer.py:186-191: p = float32(|td| + float32(eps)) (float32
+// TD errors plus a python float stay float32), leaf = p^alpha in float64, running max of p over every entry (duplicates
+// included).  bad: set to 1 when some p is not > 0 (NaN or zero), where the reference asserts.
 __global__ void __launch_bounds__(256)
 per_priorities_kernel(const float* __restrict__ td, int n, double eps, double alpha, double* __restrict__ powered,
-                      double* __restrict__ max_priority) {
+                      double* __restrict__ max_priority, int* __restrict__ bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double p = fabs((double)td[i]) + eps;
-  powered[i] = pow(p, alpha);
+  const double p = (double)__fadd_rn(fabsf(td[i]), __double2float_rn(eps));
+  powered[i] = pow_cr(p, alpha);
+  if (!(p > 0.0)) { *bad = 1; return; }
   // atomic max on a positive double == atomic max on its bit pattern as signed 64-bit
   atomicMax(reinterpret_cast<long long*>(max_priority), __double_as_longlong(p));
+}
+
+// out[i] = x[i]^y with the same pow as the leaves (the add path's max_priority ** alpha)
+__global__ void per_pow_kernel(const double* __restrict__ x, int n, double y, double* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = pow_cr(x[i], y);
 }
 
 // ------------------------------------------------------------------------------------------ DQN TD step
@@ -240,20 +266,26 @@ int tree_range_sum_impl(const double* tree, long long capacity, long long start,
 
 int per_sample_impl(const double* sum_tree, const double* min_tree, long long capacity, long long n_stored,
                     const double* uniforms, int batch, double beta, long long* idx_out, double* w_out,
-                    float* w_out_f32, cudaStream_t stream) {
+                    float* w_out_f32, int* bad, cudaStream_t stream) {
   B200RL_REQUIRE(sum_tree && min_tree && uniforms && idx_out && w_out && batch > 0, "per_sample: bad args");
   B200RL_REQUIRE(n_stored >= 2 && n_stored <= capacity, "per_sample: need 2 <= n_stored <= capacity");
   B200RL_REQUIRE(beta > 0, "per_sample: beta must be > 0");
   per_sample_kernel<<<ceil_div(batch, 256), 256, 0, stream>>>(sum_tree, min_tree, capacity, n_stored, uniforms, batch,
-                                                              beta, idx_out, w_out, w_out_f32);
+                                                              beta, idx_out, w_out, w_out_f32, bad);
   return check_launch("per_sample_kernel");
 }
 
 int per_priorities_impl(const float* td, int n, double eps, double alpha, double* powered, double* max_priority,
-                        cudaStream_t stream) {
-  B200RL_REQUIRE(td && powered && max_priority && n > 0, "per_priorities: bad args");
-  per_priorities_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(td, n, eps, alpha, powered, max_priority);
+                        int* bad, cudaStream_t stream) {
+  B200RL_REQUIRE(td && powered && max_priority && bad && n > 0, "per_priorities: bad args");
+  per_priorities_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(td, n, eps, alpha, powered, max_priority, bad);
   return check_launch("per_priorities_kernel");
+}
+
+int per_pow_impl(const double* x, int n, double y, double* out, cudaStream_t stream) {
+  B200RL_REQUIRE(x && out && n > 0, "per_pow: bad args");
+  per_pow_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(x, n, y, out);
+  return check_launch("per_pow_kernel");
 }
 
 int dqn_td_impl(const float* a_t, long long lda_t, const float* s_t, long long lds_t, const float* a_on,

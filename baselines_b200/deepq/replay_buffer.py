@@ -153,6 +153,15 @@ class PrioritizedReplayBuffer(ReplayBuffer):
         self._maxp_dev = torch.ones(1, dtype=torch.float64, device=dev)
         self._arange = torch.arange(self._stage_cap, dtype=torch.int64, device=dev)
         self._new_val = torch.zeros(self._stage_cap, dtype=torch.float64, device=dev)
+        # the reference asserts `priority > 0` (replay_buffer.py:186).  The kernels set a sticky device flag instead;
+        # it is copied to pinned memory without waiting and raised on by the first sample / update call that finds the
+        # copy complete, which is the first one after the host has synchronised with the stream (deepq.learn: after the
+        # next act), so the train loop never waits for it
+        self._bad_dev = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._bad_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self._bad_copied = torch.cuda.Event()
+        self._bad_pending = False
+        self._bad_seen = False
 
     @property
     def _max_priority(self):
@@ -165,6 +174,20 @@ class PrioritizedReplayBuffer(ReplayBuffer):
     def _set_priorities(self, idx_t, vals_t):
         ops.tree_set(self._it_sum, self._it_min, self._cap, idx_t, vals_t)
 
+    def _copy_bad_flag(self):
+        with torch.cuda.device(self.device):
+            self._bad_host.copy_(self._bad_dev, non_blocking=True)
+            self._bad_copied.record()
+        self._bad_pending = True
+
+    def _check_priorities(self):
+        if self._bad_pending and self._bad_copied.query():
+            self._bad_pending = False
+            self._bad_seen = bool(int(self._bad_host[0]))                        # the device flag is sticky
+        if self._bad_seen:
+            raise AssertionError("assert priority > 0 failed: an update wrote a priority that is not > 0 "
+                                 "(NaN or zero |td| + eps); the sum / min trees are invalid")
+
     def add(self, *args, **kwargs):
         """replay_buffer.py:100-105: new transitions enter with max_priority ** alpha.  max_priority only changes in
         update_priorities, which flushes the staged transitions first, so every staged transition shares one value and
@@ -172,20 +195,21 @@ class PrioritizedReplayBuffer(ReplayBuffer):
         return super().add(*args, **kwargs)
 
     def _on_flush_range(self, lo, n):
-        torch.pow(self._maxp_dev, self._alpha, out=self._new_val[:1])          # scalar bookkeeping, stays on the device
+        ops.per_pow(self._maxp_dev, self._alpha, self._new_val[:1])             # scalar bookkeeping, stays on the device
         self._set_priorities(self._arange[:n] + lo, self._new_val[:1].expand(n).contiguous())
 
     def add_batch(self, *args, **kwargs):
         idx = super().add_batch(*args, **kwargs)
         it = torch.from_numpy(np.asarray(idx, dtype=np.int64)).to(self.device)
-        vals = torch.pow(self._maxp_dev, self._alpha).expand(len(idx)).contiguous()
-        self._set_priorities(it, vals)
+        ops.per_pow(self._maxp_dev, self._alpha, self._new_val[:1])
+        self._set_priorities(it, self._new_val[:1].expand(len(idx)).contiguous())
         return idx
 
     def sample_device(self, batch_size, beta, uniforms=None):
         """Stratified proportional sampling + importance weights on device (replay_buffer.py:107-115,157-165).
         Returns (idx int64[B], weights float32[B], weights float64[B]) device tensors."""
         assert beta > 0
+        self._check_priorities()
         self._flush()
         if uniforms is None:
             uniforms = [random.random() for _ in range(batch_size)]              # replay_buffer.py:112
@@ -193,18 +217,21 @@ class PrioritizedReplayBuffer(ReplayBuffer):
         idx = torch.empty(batch_size, dtype=torch.int64, device=self.device)
         w64 = torch.empty(batch_size, dtype=torch.float64, device=self.device)
         w32 = torch.empty(batch_size, dtype=torch.float32, device=self.device)
-        ops.per_sample(self._it_sum, self._it_min, self._cap, self._n, u, beta, idx, w64, w32)
+        ops.per_sample(self._it_sum, self._it_min, self._cap, self._n, u, beta, idx, w64, w32, self._bad_dev)
         return idx, w32, w64
 
     def sample(self, batch_size, beta):
         """Reference return tuple: (obs_t, act, rew, obs_tp1, done, weights float64, idxes)."""
         idx, _, w64 = self.sample_device(batch_size, beta)
+        self._copy_bad_flag()
         idxes = idx.cpu().numpy()
+        self._check_priorities()
         return tuple(list(self._encode_sample(idxes)) + [w64.cpu().numpy(), list(idxes)])
 
     def update_priorities(self, idxes, priorities):
         """replay_buffer.py:169-191.  priority ** alpha is evaluated with python floats like the reference."""
         assert len(idxes) == len(priorities)
+        self._check_priorities()
         self._flush()
         pr = [float(p) for p in priorities]
         assert all(p > 0 for p in pr)
@@ -215,8 +242,11 @@ class PrioritizedReplayBuffer(ReplayBuffer):
         self._max_priority = max(self._max_priority, max(pr))
 
     def update_priorities_device(self, idx, td_errors, eps):
-        """new_priorities = |td| + eps (deepq.py:302); p ** alpha and the running max are computed on device."""
+        """new_priorities = |td| + eps in float32 (deepq.py:302); p ** alpha and the running max are computed on device.
+        A priority that is not > 0 raises AssertionError here or in a later sample / update call (see __init__)."""
+        self._check_priorities()
         self._flush()
         powered = torch.empty(idx.numel(), dtype=torch.float64, device=self.device)
-        ops.per_priorities(td_errors, eps, self._alpha, powered, self._maxp_dev)
+        ops.per_priorities(td_errors, eps, self._alpha, powered, self._maxp_dev, self._bad_dev)
         self._set_priorities(idx, powered)
+        self._copy_bad_flag()

@@ -426,18 +426,33 @@ def tree_range_sum(tree, capacity, start, end, out):
     _lib.call("b200rl_tree_range_sum", _ptr(tree), int(capacity), int(start), int(end), _ptr(out), _stream())
 
 
-def per_sample(sum_tree, min_tree, capacity, n_stored, uniforms, beta, idx_out, w_out, w_out_f32=None):
+def per_sample(sum_tree, min_tree, capacity, n_stored, uniforms, beta, idx_out, w_out, w_out_f32=None, bad=None):
+    """bad: optional int32 device scalar, set to 1 when the tree holds a priority that is not > 0 (the slot that would
+    leave the stored range returns index 0)."""
     _chk(uniforms, torch.float64, "uniforms")
     _chk(idx_out, torch.int64, "idx_out")
     _chk(w_out, torch.float64, "w_out")
+    _chk(bad, torch.int32, "bad")
     _lib.call("b200rl_per_sample", _ptr(sum_tree), _ptr(min_tree), int(capacity), int(n_stored), _ptr(uniforms),
-              uniforms.numel(), float(beta), _ptr(idx_out), _ptr(w_out), _ptr(w_out_f32), _stream())
+              uniforms.numel(), float(beta), _ptr(idx_out), _ptr(w_out), _ptr(w_out_f32), _ptr(bad), _stream())
 
 
-def per_priorities(td, eps, alpha, powered, max_priority):
+def per_priorities(td, eps, alpha, powered, max_priority, bad):
+    """p = float32(|td| + float32(eps)); powered = p ** alpha (float64); max_priority = max(max_priority, p).
+    bad: int32 device scalar, set to 1 when some p is not > 0 (NaN or zero)."""
     _chk(td, torch.float32, "td")
+    _chk(powered, torch.float64, "powered")
+    _chk(max_priority, torch.float64, "max_priority")
+    _chk(bad, torch.int32, "bad")
     _lib.call("b200rl_per_priorities", _ptr(td), td.numel(), float(eps), float(alpha), _ptr(powered),
-              _ptr(max_priority), _stream())
+              _ptr(max_priority), _ptr(bad), _stream())
+
+
+def per_pow(x, y, out):
+    """out = x ** y (float64), correctly rounded: the pow of the replay leaves and weights."""
+    _chk(x, torch.float64, "x")
+    _chk(out, torch.float64, "out")
+    _lib.call("b200rl_per_pow", _ptr(x), x.numel(), float(y), _ptr(out), _stream())
 
 
 def dqn_td(a_t, lda_t, s_t, lds_t, a_on, lda_on, s_on, lds_on, a_tg, lda_tg, s_tg, lds_tg, nA, idx, actions,

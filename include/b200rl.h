@@ -209,16 +209,22 @@ int b200rl_obs_encode(const float* x, const long long* src_idx, long long B, int
 
 /* prioritized replay: common/segment_tree.py:76-86 (__setitem__), :51-74 (reduce), :105-131
  * (find_prefixsum_idx); deepq/replay_buffer.py:107-115 (_sample_proportional), :157-165 (weights),
- * :169-191 (update_priorities). */
+ * :169-191 (update_priorities).  Every pow is correctly rounded (csrc/pow_cr.cuh).
+ * per_priorities: p = float32(|td| + float32(eps)), powered = p^alpha, max_priority = max(max_priority, p); bad
+ * (device int, required) is set to 1 when some p is not > 0 (NaN or zero), where the reference asserts.
+ * per_sample: bad (optional) is set to 1 when the tree holds a priority that is not > 0 or a descent ends past
+ * n_stored; such a slot returns index 0, so an index never leaves the stored range.
+ * per_pow: out[i] = x[i]^y, the pow of the leaves (the add path's max_priority ** alpha). */
 int b200rl_tree_set(double* sum_tree, double* min_tree, long long capacity, const long long* idx, const double* vals,
                     int n, void* stream);
 int b200rl_tree_range_sum(const double* tree, long long capacity, long long start, long long end, double* out,
                           void* stream);
 int b200rl_per_sample(const double* sum_tree, const double* min_tree, long long capacity, long long n_stored,
                       const double* uniforms, int batch, double beta, long long* idx_out, double* w_out,
-                      float* w_out_f32, void* stream);
+                      float* w_out_f32, int* bad, void* stream);
 int b200rl_per_priorities(const float* td, int n, double eps, double alpha, double* powered, double* max_priority,
-                          void* stream);
+                          int* bad, void* stream);
+int b200rl_per_pow(const double* x, int n, double y, double* out, void* stream);
 
 /* DQN: deepq/build_graph.py:388-413 (double-Q target, Huber tf_util.py:39-45, importance weights),
  * deepq/models.py:38-40 (dueling), build_graph.py:184-191 (epsilon-greedy). s_* == NULL -> no dueling. */

@@ -441,8 +441,11 @@ def test_per_trace_vs_reference_golden(ops):
     assert state["maxp"] == float(g["max_priority"])
 
 
-def test_per_large_tree_vs_oracle(ops):
+def test_per_large_tree_vs_oracle_float32_priorities(ops):
+    """Trees, indices and weights at 2^14 leaves against the oracle; new priorities from float32 TD errors are the
+    float32 values fl32(|td| + fl32(eps)) of the reference's graph, powered with the correctly rounded pow."""
     from oracle.segment_tree import PrioritizedSampler
+    from _replay_refs import cr_pow, leaf_values, reference_priorities
     size, batch = 1 << 14, 512
     rng = np.random.RandomState(8)
     per = PrioritizedSampler(size, 0.6)
@@ -464,14 +467,19 @@ def test_per_large_tree_vs_oracle(ops):
     ops.per_sample(s, m, cap, size, dev(u), 0.4, idx, w, wf)
     want = per.sample_idx(u)
     assert np.array_equal(idx.cpu().numpy(), want)
-    assert np.allclose(w.cpu().numpy(), per.weights(want, 0.4), rtol=1e-13)
+    assert np.allclose(w.cpu().numpy(), per.weights(want, 0.4), rtol=1e-13)    # the oracle's weights use libm pow
+    total = per.sum_tree.sum()
+    want_w = (cr_pow(np.array([per.sum_tree.get(i) for i in want]) / total * size, -0.4)
+              / cr_pow(per.min_tree.min() / total * size, -0.4))
+    assert np.array_equal(w.cpu().numpy(), want_w) and np.array_equal(wf.cpu().numpy(), want_w.astype(np.float32))
     td = torch.randn(batch, device="cuda")
     powered = torch.zeros(batch, dtype=torch.float64, device="cuda")
     maxp = torch.ones(1, dtype=torch.float64, device="cuda")
-    ops.per_priorities(td, 1e-6, 0.6, powered, maxp)
-    pw = (np.abs(td.cpu().numpy().astype(np.float64)) + 1e-6)
-    assert np.allclose(powered.cpu().numpy(), pw ** 0.6, rtol=1e-14)
-    assert float(maxp[0]) == max(1.0, float(pw.max()))
+    bad = torch.zeros(1, dtype=torch.int32, device="cuda")
+    ops.per_priorities(td, 1e-6, 0.6, powered, maxp, bad)
+    pw = reference_priorities(td.cpu().numpy(), 1e-6)                                # float32 priorities
+    assert np.array_equal(powered.cpu().numpy(), leaf_values(pw, 0.6))
+    assert float(maxp[0]) == max(1.0, float(pw.max())) and int(bad[0]) == 0
 
 
 def test_dqn_td_vs_oracle(ops):
