@@ -10,9 +10,10 @@
 //                                       and, with negative shifts over a zero-bordered dY, the data gradient
 //                                       dX[m, :] = ( sum_t dY[m - sh_t, :] * W_t ) * (saved activation > 0)
 //   conv_shift_wgrad_kernel (MN-major): G[t, c, n] += alpha * sum_m X[m + sh_t, c] * dY[m, n]         wgrad
-//                                       (a CTA keeps the accumulators of up to 2*QW taps x 64 channels in registers;
-//                                        where clusters tile the SMs, the CTAs of the tap groups of one row range
-//                                        form a cluster and share each X / dY stage by TMA multicast)
+//                                       (G's 64-row chunks, tap x 64 channels, are dealt evenly to the warpgroups of
+//                                        a row range, at most QW each, and accumulate in registers; where clusters
+//                                        tile the SMs, the CTAs of one row range form a cluster and share each X / dY
+//                                        stage by TMA multicast)
 //
 // Warp roles: warps 0-7 are two consumer warpgroups (they issue the wgmma.mma_async chains, and run the epilogue --
 // or, in the wgrad, the fused bias-gradient sums -- from their own registers) | warp 8 TMA loads | uint8-fed first
@@ -30,6 +31,8 @@
 // or multiply a zero of the zero-bordered dY (wgrad / dgrad) -- so dY tensors live on the conv's INPUT grid.
 // Replaces tf.nn.conv2d (a2c/utils.py:56) and its gradients (ppo2/model.py:102) of the reference.
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -59,8 +62,9 @@ __host__ __device__ constexpr int sh_wres_bytes(int KH, bool u8) {
 static constexpr int SH_BAR_BYTES = 512;             // forward kernel: mbarrier block after the weights
 static constexpr int SH_WROWS_K = 96;                // wgrad: 64 + max shift span (<= 32)
 static constexpr int SH_WABYTES = SH_WROWS_K * 128;
-// wgrad: 64-channel accumulator chunks per consumer warpgroup (2 * QW * N/2 registers per thread)
-__host__ __device__ constexpr int sh_wgrad_qw(int BN, bool u8) { return u8 ? 2 : (BN == 64 ? 2 : 4); }
+// wgrad: at most QW 64-channel accumulator chunks per consumer warpgroup (QW * N/2 accumulator registers per thread).
+// N = 64 over 64 channels: QW = 3, so that a 3x3 conv's 9 chunks fit one 2-CTA cluster and X / dY are read once.
+__host__ __device__ constexpr int sh_wgrad_qw(int BN, int KH, bool u8) { return u8 ? 2 : BN == 32 ? 4 : KH == 1 ? 3 : 2; }
 
 // Ordered MMA issue of the two consumer warpgroups (barrier 0 is __syncthreads, 1 joins the consumer warps in the
 // wgrad).  Group g waits on barrier SH_ORDER_BAR + g for its turn and hands the turn over with an arrive on the other
@@ -519,7 +523,7 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
   constexpr int B_BYTES = KR * BROWB;
   constexpr int B_REGION = (B_BYTES + 1023) & ~1023;
   constexpr int STAGES = (KH == 1) ? 8 : 6;
-  constexpr int QW = sh_wgrad_qw(BN, U8);
+  constexpr int QW = sh_wgrad_qw(BN, KH, U8);
   static_assert(!U8 || KH == 1, "the uint8-fed layer has 64 space-to-depth channels");
   // TMA-fed: stage = [A halves | B], 1024 B aligned.  uint8-fed: [rolling A ring (KR-row blocks) | B stages]
   using Ring = U8Ring<KR, STAGES>;
@@ -589,7 +593,11 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
                                     warp - (SH_TMA_WARP + 1), lane);
   } else {
     const int wg = warp >> 2, t = threadIdx.x & 127;
-    const int q0 = (int)blockIdx.y * 2 * QW + wg * QW;         // this warpgroup's first accumulator chunk
+    // The chunks are dealt to the 2 * gridDim.y warpgroups of the grid in contiguous runs whose lengths differ by at
+    // most one (c3's 9 chunks: 3 + 2 | 2 + 2), so no warpgroup issues MMAs for a chunk it does not own.
+    const int nwg = 2 * (int)gridDim.y, w = 2 * (int)blockIdx.y + wg;
+    const int q0 = w * (nchunks / nwg) + min(w, nchunks % nwg);     // this warpgroup's first accumulator chunk
+    const int nq = nchunks / nwg + (w < nchunks % nwg ? 1 : 0);     // its chunk count, 0 .. QW (warpgroup-uniform)
     // A descriptor start of chunk q relative to the stage: half h, rows shifted by the tap's shift
     int a_rel[QW];
 #pragma unroll
@@ -606,59 +614,84 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
     const int cq = lane % LPR, rg = lane / LPR;
     const int chunk = (cq * 8) >> 4, within = (cq * 8) & 15;
     float bsum[4] = {0.f, 0.f, 0.f, 0.f};
-    // Each k-block's MMAs start a fresh accumulator (part) that is then added to acc in fp32 registers: a CTA reduces
-    // ~10^4 rows, and one chain of that many tensor-core accumulations loses ~1e-5 relative against an fp32 sum.
-    float acc[QW][BN / 2], part[QW][BN / 2];
+    auto bias_sums = [&](int st) {
+      const uint8_t* sb = smem + B_BASE + st * B_PITCH;
+#pragma unroll 4
+      for (int r = warp * RG + rg; r < KR; r += SH_CONSUMER_WARPS * RG) {
+        const int sw = (BROWB == 128) ? (r & 7) : ((r >> 1) & 3);
+        const uint2 v = *reinterpret_cast<const uint2*>(sb + r * BROWB + ((chunk ^ sw) << 4) + within);
+        bsum[0] += __half2float(__ushort_as_half((unsigned short)(v.x & 0xffffu)));
+        bsum[1] += __half2float(__ushort_as_half((unsigned short)(v.x >> 16)));
+        bsum[2] += __half2float(__ushort_as_half((unsigned short)(v.y & 0xffffu)));
+        bsum[3] += __half2float(__ushort_as_half((unsigned short)(v.y >> 16)));
+      }
+    };
+    auto release = [&](int st) {
+      __syncwarp();
+      if (U8 || ncta == 1) {
+        if (lane == 0) mbar_arrive(&empty_bar[st]);
+      } else if (lane < (int)ncta) {
+        mbar_arrive_cluster(&empty_bar[st], (uint32_t)lane);   // lane r releases the stage in CTA r of the cluster
+      }
+    };
+    // Each (k-block, chunk) MMA group starts a fresh accumulator (part) that is then added to acc in fp32 registers: a
+    // CTA reduces ~10^4 rows, and one chain of that many tensor-core accumulations loses ~1e-5 relative against an fp32
+    // sum.  With NP = 2 part buffers the chunks of a k-block alternate between them, so chunk i's acc += part runs while
+    // chunk i+1's MMAs execute (wgmma_wait<1>).  QW = 3 leaves registers for one buffer only (288 threads cap the kernel
+    // at 168 registers): each chunk then waits for its own MMAs, and the other warpgroup's MMAs fill the tensor pipe.
+    constexpr int NP = (QW + 2) * (BN / 2) <= 128 ? 2 : 1;
+    float acc[QW][BN / 2], part[NP][BN / 2];
 #pragma unroll
     for (int i = 0; i < QW; ++i)
 #pragma unroll
       for (int e = 0; e < BN / 2; ++e) acc[i][e] = 0.0f;
-    int s = 0;
-    uint32_t ph = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      const int s1 = (s + 1 == STAGES) ? 0 : s + 1;
-      mbar_wait(&full_bar[s], ph);
-      if (U8) mbar_wait(&head_bar[s1], s1 == 0 ? ph ^ 1 : ph);   // the shifted taps read into the next block's first unit
-      const uint32_t a_base = smem_u32(smem + s * A_PITCH);
-      const uint32_t b_base = smem_u32(smem + B_BASE + s * B_PITCH);
-      wgmma_fence();
+    auto add_part = [&](float(&a)[BN / 2], const float(&pt)[BN / 2]) {
 #pragma unroll
-      for (int i = 0; i < QW; ++i) {
-        // chunks past the last one repeat it (a_rel is clamped) and are dropped by the epilogue: a wgmma under a
-        // thread-dependent branch would make the compiler serialise every wgmma of the kernel
+      for (int e = 0; e < BN / 2; ++e) a[e] += pt[e];
+    };
+    // the warpgroup's k-block loop for NQ chunks (a compile-time count, so that every register index is static)
+    auto consume = [&](auto nq_c) {
+      constexpr int NQ = decltype(nq_c)::value;
+      int s = 0;
+      uint32_t ph = 0;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        const int s1 = (s + 1 == STAGES) ? 0 : s + 1;
+        mbar_wait(&full_bar[s], ph);
+        if (U8) mbar_wait(&head_bar[s1], s1 == 0 ? ph ^ 1 : ph);   // the shifted taps read into the next block's first unit
+        const uint32_t a_base = smem_u32(smem + s * A_PITCH);
+        const uint32_t b_base = smem_u32(smem + B_BASE + s * B_PITCH);
+        if (NQ == 0 && do_bias) bias_sums(s);
 #pragma unroll
-        for (int k = 0; k < KR / 16; ++k) {
-          const uint64_t adesc = make_sdesc(a_base + a_rel[i] + k * 16 * 128, 8 * 1024, 1024, 1);
-          const uint64_t bdesc = make_sdesc(b_base + k * 16 * BROWB, 8 * 8 * BROWB, 8 * BROWB, LAYOUT_B);
-          wgmma_f16<BN, 1, 1>(part[i], adesc, bdesc, k > 0 ? 1u : 0u);
+        for (int i = 0; i < NQ; ++i) {
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < KR / 16; ++k) {
+            const uint64_t adesc = make_sdesc(a_base + a_rel[i] + k * 16 * 128, 8 * 1024, 1024, 1);
+            const uint64_t bdesc = make_sdesc(b_base + k * 16 * BROWB, 8 * 8 * BROWB, 8 * BROWB, LAYOUT_B);
+            wgmma_f16<BN, 1, 1>(part[i % NP], adesc, bdesc, k > 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          if (i == 0 && do_bias) bias_sums(s);
+          wgmma_wait<NP - 1>();                                    // chunk i - (NP - 1) has retired
+          if (i >= NP - 1) add_part(acc[i - (NP - 1)], part[(i - (NP - 1)) % NP]);
         }
-      }
-      wgmma_commit();
-      if (do_bias) {
-        const uint8_t* sb = smem + B_BASE + s * B_PITCH;
-#pragma unroll 4
-        for (int r = warp * RG + rg; r < KR; r += SH_CONSUMER_WARPS * RG) {
-          const int sw = (BROWB == 128) ? (r & 7) : ((r >> 1) & 3);
-          const uint2 w = *reinterpret_cast<const uint2*>(sb + r * BROWB + ((chunk ^ sw) << 4) + within);
-          bsum[0] += __half2float(__ushort_as_half((unsigned short)(w.x & 0xffffu)));
-          bsum[1] += __half2float(__ushort_as_half((unsigned short)(w.x >> 16)));
-          bsum[2] += __half2float(__ushort_as_half((unsigned short)(w.y & 0xffffu)));
-          bsum[3] += __half2float(__ushort_as_half((unsigned short)(w.y >> 16)));
+        if constexpr (NP == 2 && NQ > 0) {
+          wgmma_wait<0>();
+          add_part(acc[NQ - 1], part[(NQ - 1) % NP]);
         }
+        release(s);
+        s = s1;
+        if (s == 0) ph ^= 1;
       }
-      wgmma_wait<0>();
-      __syncwarp();
-      if (U8 || ncta == 1) {
-        if (lane == 0) mbar_arrive(&empty_bar[s]);
-      } else if (lane < (int)ncta) {
-        mbar_arrive_cluster(&empty_bar[s], (uint32_t)lane);     // lane r releases the stage in CTA r of the cluster
-      }
-#pragma unroll
-      for (int i = 0; i < QW; ++i)
-#pragma unroll
-        for (int e = 0; e < BN / 2; ++e) acc[i][e] += part[i][e];
-      s = s1;
-      if (s == 0) ph ^= 1;
+    };
+    static_assert(QW >= 2 && QW <= 4, "conv_shift_wgrad: 2..4 chunks per warpgroup");
+    switch (nq) {                                              // warpgroup-uniform
+      case 0: consume(std::integral_constant<int, 0>{}); break;
+      case 1: consume(std::integral_constant<int, 1>{}); break;
+      case 2: consume(std::integral_constant<int, 2>{}); break;
+      default:
+        if constexpr (QW >= 3) if (nq == 3) consume(std::integral_constant<int, 3>{});
+        if constexpr (QW >= 4) if (nq == 4) consume(std::integral_constant<int, 4>{});
     }
     if (do_bias) {
       __shared__ float s_bsum[SH_CONSUMER_WARPS][64];
@@ -681,7 +714,7 @@ conv_shift_wgrad_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_co
     if (kb1 > kb0) {
 #pragma unroll
       for (int i = 0; i < QW; ++i) {
-        if (q0 + i < nchunks) {
+        if (i < nq) {
 #pragma unroll
           for (int e = 0; e < BN / 2; ++e) {
             const int cn = acc_col(t, e);
@@ -903,7 +936,7 @@ int conv_shift_wgrad_impl(const void* X, long long rows, int C, const void* dY, 
   if (max_ctas > 0 && max_ctas < ctas) ctas = max_ctas;
   if (ctas > p.kb_total) ctas = p.kb_total;
   p.kb_per_cta = (p.kb_total + ctas - 1) / ctas;
-  const int qw = sh_wgrad_qw(N, u8_x != nullptr);
+  const int qw = sh_wgrad_qw(N, KH, u8_x != nullptr);
   const dim3 grid((p.kb_total + p.kb_per_cta - 1) / p.kb_per_cta, (taps * kx * KH + 2 * qw - 1) / (2 * qw));
   p.u8 = make_u8src(u8_x, u8_idx, u8_H, u8_W, u8_C, u8_s);
   p.grows = (long long)taps * kx * KH * 64;
