@@ -54,6 +54,8 @@ SIGNATURES = {
     "b200rl_dqn_td": [_p, _ll, _p, _ll, _p, _ll, _p, _ll, _p, _ll, _p, _ll, _i, _p, _p, _p, _p, _p, _f, _i, _p, _p,
                       _ll, _p, _ll, _p, _i, _p],
     "b200rl_dqn_act": [_p, _ll, _p, _ll, _i, _f, _ull, _ull, _p, _p, _p, _i, _p],
+    "b200rl_lstm_seq_fwd": [_p, _ll, _p, _p, _p, _p, _p, _p, _p, _ll, _p, _p, _p, _i, _i, _i, _p],
+    "b200rl_lstm_seq_bwd": [_p, _ll, _p, _p, _p, _p, _p, _p, _p, _p, _ll, _i, _i, _i, _p],
 }
 
 _lib = None

@@ -12,6 +12,9 @@ from .. import _lib, nn, ops
 from . import spaces
 
 
+RECURRENT_NETWORKS = ("lstm", "cnn_lstm")
+
+
 class PolicyBuilder:
     """What `build_policy(env, network, **kwargs)` returns (reference: a `policy_fn` closure,
     policies.py:126).  Carries the architecture; `Model` instantiates it on a device."""
@@ -20,9 +23,17 @@ class PolicyBuilder:
                  **network_kwargs):
         if callable(network) and not isinstance(network, str):
             raise NotImplementedError("custom network callables build TF graphs in the reference; this learner "
-                                      "supports the registry names 'cnn', 'mlp', 'conv_only'")
+                                      "supports the registry names 'cnn', 'mlp', 'conv_only', 'lstm', 'cnn_lstm'")
+        if network in ("lnlstm", "cnn_lnlstm") or (network in RECURRENT_NETWORKS and network_kwargs.get("layer_norm")):
+            raise NotImplementedError(f"network={network!r}: layer-normalised LSTMs are not implemented "
+                                      "(supported recurrent networks: 'lstm', 'cnn_lstm' without layer_norm)")
+        if network in ("impala_cnn", "impala_cnn_lstm"):
+            raise NotImplementedError(f"network={network!r}: the IMPALA residual tower is not implemented")
         if value_network not in (None, "shared", "copy"):
             raise NotImplementedError("value_network must be None/'shared'/'copy' (policies.py:154-166)")
+        if value_network == "copy" and network in RECURRENT_NETWORKS:
+            # the reference leaves this a TODO (policies.py:165): the copied value tower would need its own state
+            raise NotImplementedError("value_network='copy' is not supported with recurrent networks")
         self.ob_space, self.ac_space = ob_space, ac_space
         self.network = network
         self.value_network = "copy" if value_network == "copy" else None
@@ -58,8 +69,8 @@ class PolicyNet:
         if spaces.is_multi_binary(ob_space):
             raise NotImplementedError("MultiBinary observations have no encoding in common/input.py:43-63")
         self.ob_onehot = int(ob_space.n) if spaces.is_discrete(ob_space) else 0
-        if (self.ob_onehot or self.ob_nvec) and builder.network != "mlp":
-            raise NotImplementedError("Discrete / MultiDiscrete observations need a vector network ('mlp')")
+        if (self.ob_onehot or self.ob_nvec) and builder.network not in ("mlp", "lstm"):
+            raise NotImplementedError("Discrete / MultiDiscrete observations need a vector network ('mlp', 'lstm')")
         # the action distribution (distributions.py:278-290 make_pdtype): 'cat' Categorical (Discrete), 'mcat'
         # MultiCategorical (MultiDiscrete), 'bern' Bernoulli (MultiBinary), 'gauss' DiagGaussian (Box)
         self.nvec = None
@@ -94,6 +105,9 @@ class PolicyNet:
         # creation order == the reference's variable creation order (it fixes the ortho_init RNG stream)
         self.tower_pi = nn.Tower(store, kind, self.ob_shape, "pi", f"{scope}/pi", rng, cap, **kw)
         self.tower_vf = nn.Tower(store, kind, self.ob_shape, "vf", f"{scope}/vf", rng, cap, **kw) if self.copy_vf else None
+        # recurrent networks (models.py lstm / cnn_lstm): the state is [nenv, 2 * nlstm] = [c | h] (utils.py:96)
+        self.recurrent = self.tower_pi.lstm is not None
+        self.nlstm = self.tower_pi.lstm.H if self.recurrent else 0
         L = self.tower_pi.latent_dim
         # distributions.py:351-355 (_matching_fc): when the latent is already nout wide the 'pi' layer is skipped and
         # the latent IS the logits / mean.  Here the head keeps a frozen identity block (its gradient is zeroed before
@@ -291,8 +305,9 @@ class PolicyNet:
         """ValueError if an observation encoded since the last check was beyond fp16 (nn.Tower.check_obs_range)."""
         self.tower_pi.check_obs_range(flag)
 
-    def forward(self, x, B, src_idx=None, masks=True):
-        """Towers + heads for B samples of x (optionally gathered through src_idx); masks=False: no backward follows."""
+    def forward(self, x, B, src_idx=None, masks=True, seq=None):
+        """Towers + heads for B samples of x (optionally gathered through src_idx); masks=False: no backward follows.
+        seq (recurrent networks): how the B rows form sequences (nn.Seq)."""
         if self.fuse0:
             tp, tv = self.tower_pi, self.tower_vf
             a = tp.fcs[0]
@@ -305,7 +320,7 @@ class PolicyNet:
             self.head_pi.forward(lat, ldl, B, self.pi_out, self.ld_pi, mode=ops.MODE_F32_STORE)
             self.head_vf.forward(latv, ldlv, B, self.v_out, self.ld_v, mode=ops.MODE_F32_STORE)
             return
-        lat, ldl = self.tower_pi.forward(x, B, src_idx, masks=masks)
+        lat, ldl = self.tower_pi.forward(x, B, src_idx, masks=masks, seq=seq)
         self._lat_pi, self._ld_lat_pi = lat, ldl
         if self.head is not None:
             self.head.forward(lat, ldl, B, self.headout, self.ld_ho, mode=ops.MODE_F32_STORE)
@@ -317,11 +332,11 @@ class PolicyNet:
             self.head_pi.forward(lat, ldl, B, self.pi_out, self.ld_pi, mode=ops.MODE_F32_STORE)
             self.head_vf.forward(latv, ldlv, B, self.v_out, self.ld_v, mode=ops.MODE_F32_STORE)
 
-    def act(self, x, B, actions, values, neglogp, noise=None, seed=0):
+    def act(self, x, B, actions, values, neglogp, noise=None, seed=0, seq=None):
         """PolicyWithValue.step (policies.py:77-96) into caller-provided device tensors.  The sampler's stream position
         is a device counter advanced after every pass, so the sequence can be replayed from a CUDA graph."""
         _lib.phase = "@act"
-        self.forward(x, B, masks=False)
+        self.forward(x, B, masks=False, seq=seq)
         if self.pd in ("cat", "mcat"):
             ops.cat_step(self.pi_out, self.ld_pi, self.nout, self.v_out, self.ld_v, actions, values, neglogp, B,
                          uniforms=noise, seed=seed, offset_dev=self.rng_ctr, seg_off=self.seg_off)
@@ -353,14 +368,14 @@ class PolicyNet:
         ops.colsum(tv.dzfc[0], b.gb, B, b.N, N2, alpha=alpha)
 
     def loss_backward(self, x, B, src_idx, actions, returns, old_values, old_neglogp, cliprange, ent_coef, vf_coef,
-                      inv_M):
+                      inv_M, seq=None):
         """One chunk of ppo2/model.py:57-114: forward, loss statistics, full backward into store.grads
         (gradients of the MEAN loss: every wgrad carries alpha = 1/M).  cliprange None: read it from `clip_dev`
         (written with ops.set_scalars by the caller) -- the form a captured launch sequence uses."""
         clip_dev = self.clip_dev if cliprange is None else None
         cliprange = 0.0 if cliprange is None else cliprange
         _lib.phase = "@train"
-        self.forward(x, B, src_idx)
+        self.forward(x, B, src_idx, seq=seq)
         if self.pd in ("cat", "mcat"):
             ops.cat_loss(self.pi_out, self.ld_pi, self.nout, self.v_out, self.ld_v, actions, src_idx, returns,
                          old_values, old_neglogp, self.adv_st, cliprange, ent_coef, vf_coef, self.dpi, self.ld_dpi,

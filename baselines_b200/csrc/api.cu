@@ -77,6 +77,10 @@ int dqn_td_impl(const float*, long long, const float*, long long, const float*, 
                 double*, int, cudaStream_t);
 int dqn_act_impl(const float*, long long, const float*, long long, int, float, unsigned long long,
                  unsigned long long, const float*, const unsigned long long*, long long*, int, cudaStream_t);
+int lstm_seq_fwd_impl(const float*, long long, const void*, const uint8_t*, const long long*, const float*,
+                      const long long*, float*, void*, long long, void*, float*, float*, int, int, int, cudaStream_t);
+int lstm_seq_bwd_impl(const void*, long long, const float*, const float*, const uint8_t*, const long long*,
+                      const float*, const long long*, const void*, void*, long long, int, int, int, cudaStream_t);
 
 }  // namespace b200rl
 
@@ -286,6 +290,21 @@ int b200rl_dqn_act(const float* a, long long lda, const float* s, long long lds,
                    unsigned long long seed, unsigned long long step, const float* eps_dev,
                    const unsigned long long* step_dev, long long* actions, int B, void* stream) {
   return dqn_act_impl(a, lda, s, lds, nA, eps, seed, step, eps_dev, step_dev, actions, B, S(stream));
+}
+
+// a2c/utils.py:84-97 lstm() over a sequence; its gradient (ppo2/model.py:102 tf.gradients through the recurrence)
+int b200rl_lstm_seq_fwd(const float* xg, long long ldxg, const void* wh, const uint8_t* masks, const long long* mask_idx,
+                        const float* state_in, const long long* state_idx, float* state_out, void* h_out,
+                        long long ldh, void* hprev_out, float* gates_out, float* c_out, int T, int B, int H,
+                        void* stream) {
+  return lstm_seq_fwd_impl(xg, ldxg, wh, masks, mask_idx, state_in, state_idx, state_out, h_out, ldh, hprev_out,
+                           gates_out, c_out, T, B, H, S(stream));
+}
+int b200rl_lstm_seq_bwd(const void* dh, long long lddh, const float* gates, const float* c, const uint8_t* masks,
+                        const long long* mask_idx, const float* state_in, const long long* state_idx, const void* whT,
+                        void* dz, long long lddz, int T, int B, int H, void* stream) {
+  return lstm_seq_bwd_impl(dh, lddh, gates, c, masks, mask_idx, state_in, state_idx, whT, dz, lddz, T, B, H,
+                           S(stream));
 }
 
 }  // extern "C"

@@ -39,6 +39,9 @@ class QNet:
                                   tf_style="contrib", **network_kwargs)
         elif kind == "mlp":
             self.trunk = nn.Tower(store, "mlp", ob_shape, "trunk", scope, rng, cap, init="ortho", **network_kwargs)
+        elif kind in ("lstm", "cnn_lstm", "lnlstm", "cnn_lnlstm"):
+            raise NotImplementedError(f"network={kind!r}: recurrent Q networks are not implemented (deepq acts on "
+                                      "single observations)")
         else:
             raise ValueError(f"unknown network {kind!r}")
         L = self.trunk.latent_dim

@@ -127,6 +127,35 @@ class IdentityEnv(Env):
         return [seed]
 
 
+class FixedSequenceEnv(Env):
+    """A memory task (common/tests/envs/fixed_sequence_env.py): the observation is always 0 (Discrete(1)); at step t
+    of an episode the action that earns reward 1 is the t-th entry of one sequence of `episode_len` actions, drawn once
+    when the env is built from a RandomState seeded 0.  Only a policy that counts steps (a recurrent one) can follow it.
+    The episode ends after `episode_len` steps; seed() reseeds the env's generator but keeps the sequence."""
+
+    def __init__(self, n_actions=10, episode_len=100):
+        self.action_space = spaces.Discrete(n_actions)
+        self.observation_space = spaces.Discrete(1)
+        self.np_random = np.random.RandomState(0)
+        self.episode_len = episode_len
+        self.sequence = [int(self.np_random.randint(0, n_actions)) for _ in range(episode_len)]
+        self.time = 0
+
+    def reset(self):
+        self.time = 0
+        return 0
+
+    def step(self, actions):
+        rew = 1 if actions == self.sequence[self.time] else 0
+        self.time += 1
+        done = bool(self.episode_len) and self.time >= self.episode_len
+        return 0, rew, done, {}
+
+    def seed(self, seed=None):
+        self.np_random.seed(seed)
+        return [seed]
+
+
 class DiscreteIdentityEnv(IdentityEnv):
     def __init__(self, dim, episode_len=None, delay=0, zero_first_rewards=True):
         self.action_space = spaces.Discrete(dim)

@@ -283,6 +283,78 @@ class Conv(Linear):
                       shuffle=(self.H, self.W, self.C, s), tag="dgrad." + self.name)
 
 
+LSTM_SIZES = (64, 128)     # nlstm instances of csrc/lstm.cu
+
+Seq = namedtuple("Seq", "T B masks mask_idx state state_idx state_out")
+Seq.__doc__ = """How the rows of one LSTM pass form sequences: T time-major steps of B environments (row t*B + b); masks
+uint8 "done before step t" of row r at masks[mask_idx[r]] (mask_idx None: masks[r]); environment b starts from row
+state_idx[b] (None: b) of the float32 [*, 2H] state; state_out: where the final state goes (None: not kept)."""
+
+
+class LSTM:
+    """The cell of a2c/utils.py:84-97 lstm() over a sequence: the input projection x.wx + b is one GEMM over all rows (a
+    Linear, MODE_F32_STORE), the recurrence csrc/lstm.cu.  Variables wx [nin, 4H], wh [H, 4H], b [4H] under
+    `<tf_prefix>/lstm/` in the reference's [i | f | o | u] gate layout; wx and wh take ortho_init(1.0) in that order
+    (utils.py:89-91)."""
+
+    def __init__(self, store, prefix, tf_prefix, nin, H, winit, split_in=False):
+        if H not in LSTM_SIZES:
+            raise NotImplementedError(f"nlstm={H}: the LSTM sequence kernels are built for nlstm in {LSTM_SIZES}")
+        self.store, self.H, self.nin = store, H, nin
+        w_x = winit((nin, 4 * H), 1.0)
+        w_h = winit((H, 4 * H), 1.0)
+        self.wx = Linear(store, f"{prefix}/lstm/wx", nin, 4 * H, None, w_x, tf_w=f"{tf_prefix}/lstm/wx:0",
+                         tf_b=f"{tf_prefix}/lstm/b:0", split_in=split_in)
+        self.wh_name = store.add(f"{prefix}/lstm/wh", w_h)
+        store.map_tf(f"{tf_prefix}/lstm/wh:0", self.wh_name, (H, 4 * H))
+
+    def materialize(self, cap):
+        dev, H = self.store.device, self.H
+        self.wx.materialize()
+        self.wh = self.store.views[self.wh_name]
+        self.gwh = self.store.gviews[self.wh_name]
+        f16, f32 = dict(dtype=torch.float16, device=dev), dict(dtype=torch.float32, device=dev)
+        self.wh16 = torch.zeros(H, 4 * H, **f16)          # forward operand (Wh)
+        self.whT16 = torch.zeros(4 * H, H, **f16)         # backward operand (Wh^T)
+        self.xg = torch.zeros(cap, 4 * H, **f32)          # x.wx + b, overwritten in place by the gate activations
+        self.c = torch.zeros(cap, H, **f32)
+        self.h = torch.zeros(cap, H, **f16)               # the latent
+        self.hprev = torch.zeros(cap, H, **f16)           # masked h_{t-1}: the A operand of dWh
+        self.dh = torch.zeros(cap, H, **f16)              # d loss / d h_t, written by the heads' data gradient
+        self.dz = torch.zeros(cap, 4 * H, **f16)
+
+    def refresh(self):
+        self.wx.refresh()
+        ops.cast_transpose(self.wh, self.H, 4 * self.H, self.wh16, 4 * self.H, self.whT16, self.H)
+
+    def forward(self, x, ldx, seq, train=True):
+        """x: [T*B, *] fp16 input rows (time-major).  train=False: only h and the state (acting / value passes)."""
+        H, rows = self.H, seq.T * seq.B
+        self.wx.forward(x, ldx, rows, self.xg, 4 * H, mode=ops.MODE_F32_STORE, act=ops.ACT_NONE)
+        ops.lstm_seq_fwd(self.xg, 4 * H, self.wh16, seq.masks, seq.state, self.h, H, seq.T, seq.B, H,
+                         mask_idx=seq.mask_idx, state_idx=seq.state_idx, state_out=seq.state_out,
+                         hprev_out=self.hprev if train else None, gates_out=self.xg if train else None,
+                         c_out=self.c if train else None)
+        self._x, self._ldx, self._seq = x, ldx, seq
+        return self.h, H
+
+    def backward(self, alpha, dx=None, ldo=0, saved=None, ld_saved=0, act=ops.ACT_NONE):
+        """self.dh -> dz; dWh += alpha hprev^T dz, dWx += alpha x^T dz, db += alpha colsum(dz); dx = (dz Wx^T) act'(saved)
+        when dx is given."""
+        H, seq = self.H, self._seq
+        rows = seq.T * seq.B
+        ops.lstm_seq_bwd(self.dh, H, self.xg, self.c, seq.masks, seq.state, self.whT16, self.dz, 4 * H, seq.T, seq.B, H,
+                         mask_idx=seq.mask_idx, state_idx=seq.state_idx)
+        tiles = -(-H // 128) * -(-4 * H // 256)
+        kb = -(-rows // 64)
+        split = max(1, min(kb // 2 if kb >= 2 else 1, -(-2 * ops.num_sms() // tiles)))
+        ops.gemm(self.hprev, self.dz, self.gwh, M=H, N=4 * H, K=rows, lda=H, ldb=4 * H, ldc=4 * H, mn_major=True,
+                 mode=ops.MODE_F32_ATOMIC, alpha=alpha, split_k=split, tag="wgrad.lstm/wh")
+        self.wx.wgrad(self._x, self._ldx, self.dz, 4 * H, rows, alpha)
+        if dx is not None:
+            self.wx.dgrad(self.dz, 4 * H, rows, dx, ldo, saved=saved, ld_saved=ld_saved, act=act)
+
+
 ConvLayerPlan = namedtuple("ConvLayerPlan", "path s2d geom implicit_dgrad kx")
 ConvLayerPlan.__doc__ = """How one conv layer runs.  path: "shift" (csrc/conv_shift.cu), "implicit" (TMA im2col GEMM over the
 input viewed as geom = (H, W, C, R, S, stride_h, stride_w, pad_t, pad_l)) or "explicit" (im2col + GEMM).  s2d: the
@@ -395,16 +467,25 @@ class Tower:
 
     def __init__(self, store, kind, ob_shape, prefix, tf_prefix, rng, cap, init="ortho", num_layers=2,
                  num_hidden=64, convs=NATURE_CONVS, same_pad=False, fc_hidden=512, tf_style="a2c", onehot_n=0,
-                 onehot_nvec=None):
+                 onehot_nvec=None, nlstm=128, layer_norm=False):
+        """kind: cnn, conv_only, mlp, or the recurrent lstm (the observation encoding of mlp, then an LSTM; models.py
+        lstm) and cnn_lstm (cnn, then an LSTM; models.py cnn_lstm).  The recurrent towers' forward and backward take
+        the rows as sequences (Seq)."""
+        if layer_norm:
+            raise NotImplementedError("layer-normalised LSTMs (lnlstm, cnn_lnlstm) are not implemented")
         self.kind, self.cap, self.store = kind, cap, store
+        self.base = {"lstm": "mlp", "cnn_lstm": "cnn"}.get(kind, kind)      # the tower below the LSTM
+        if kind == "lstm":
+            num_layers = 0                              # models.py lstm: flatten(X) straight into the cell
         self.convs, self.fcs = [], []
+        self.lstm = None
         winit = (lambda shape, scale: ortho_init(shape, scale, rng)) if init == "ortho" else \
                 (lambda shape, scale: xavier_uniform(shape, rng))
-        if kind in ("cnn", "conv_only"):
+        if self.base in ("cnn", "conv_only"):
             H, W, C = ob_shape
             self.in_u8 = True
             scale_in = 1.0 / 255.0                                           # models.py:19 folded into c1 weights
-            self.plan = plan_conv_stack(ob_shape, convs, same_pad, kind == "cnn")
+            self.plan = plan_conv_stack(ob_shape, convs, same_pad, self.base == "cnn")
             self.shift_mode = self.plan.shift
             for i, ((nm, nf, rf, stride), lp) in enumerate(zip(convs, self.plan.layers)):
                 if tf_style == "a2c":
@@ -418,7 +499,7 @@ class Tower:
                 self.convs.append(conv)
                 H, W, C = conv.OH, conv.OW, nf
             self.flat = H * W * C
-            if kind == "cnn":
+            if self.base == "cnn":
                 self.fcs.append(Linear(store, f"{prefix}/fc1", self.flat, fc_hidden, "relu",
                                        winit((self.flat, fc_hidden), math.sqrt(2)),
                                        tf_w=f"{tf_prefix}/fc1/w:0", tf_b=f"{tf_prefix}/fc1/b:0"))
@@ -426,7 +507,7 @@ class Tower:
             else:
                 self.latent_dim, self.latent_act = self.flat, ops.ACT_RELU
             self.in_dim = None
-        elif kind == "mlp":
+        elif self.base == "mlp":
             self.in_u8 = False
             self.shift_mode = False
             # Discrete(n) observations are one-hot encoded (common/input.py:54-55): raw rows hold the integer;
@@ -449,10 +530,21 @@ class Tower:
                 nin = num_hidden
             self.latent_dim, self.latent_act = nin, ops.ACT_TANH
         else:
-            raise ValueError(f"unknown network type {kind!r} (supported: cnn, conv_only, mlp)")
+            raise ValueError(f"unknown network type {kind!r} (supported: cnn, conv_only, mlp, lstm, cnn_lstm)")
         self.layers = self.convs + self.fcs
+        if kind in ("lstm", "cnn_lstm"):
+            # utils.py:89-91: wx and wh take ortho_init(1.0) after the layers below them (it fixes the RNG stream)
+            self.lstm = LSTM(store, prefix, tf_prefix, self.latent_dim, nlstm,
+                             lambda shape, scale: ortho_init(shape, scale, rng), split_in=self.base == "mlp")
+            self.latent_dim, self.latent_act = nlstm, ops.ACT_NONE
 
     def materialize(self):
+        self._materialize_layers()
+        if self.lstm is not None:
+            self.lstm.materialize(self.cap)
+            self.dlatent, self.ld_dlatent = self.lstm.dh, self.lstm.H
+
+    def _materialize_layers(self):
         dev, cap = self.store.device, self.cap
         f16 = dict(dtype=torch.float16, device=dev)
         for l in self.layers:
@@ -475,7 +567,7 @@ class Tower:
         self.hfc = [torch.empty(cap, l.Np, **f16) for l in self.fcs]
         self.dzfc = [torch.empty(cap, l.Np, **f16) for l in self.fcs]
         self.ld_hfc = [l.Np for l in self.fcs]         # row pitch of hfc[i] / dzfc[i] (a fused first layer widens [0])
-        if self.kind == "mlp":
+        if self.base == "mlp":
             self.x0 = torch.zeros(cap, 2 * self.in_pad, **f16)      # [hi | lo] operand rows of the float32 observations
             # set by the encoder when an observation value is beyond fp16 (|v| >= 65520); see check_obs_range
             self.obs_overflow = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -483,7 +575,7 @@ class Tower:
         # where the heads write d(loss)/d(latent pre-activation)
         if self.fcs:
             self.dlatent, self.ld_dlatent = self.dzfc[-1], self.fcs[-1].Np
-        else:
+        elif self.convs:
             self.dlatent, self.ld_dlatent = self.dzconv[-1], self.flat
 
     # ---- shift-GEMM conv stack ---------------------------------------------------------------------------------
@@ -571,6 +663,8 @@ class Tower:
             l.refresh()
         if self.convs and self.shift_mode:
             self._refresh_shift()
+        if self.lstm is not None:
+            self.lstm.refresh()
 
     # x: uint8 [*,H,W,C] images (cnn) or fp16 [*, in_pad] rows (mlp); src_idx gathers samples from it
     def encode(self, x, B, src_idx=None):
@@ -586,7 +680,7 @@ class Tower:
         """Raise ValueError when an encoded observation value was beyond fp16 since the last check: its hi/lo pair is
         +-inf and the network output NaN.  Reads the device flag (a synchronisation) unless the caller passes a host
         copy of it; clears the flag before raising."""
-        if self.kind != "mlp":
+        if self.base != "mlp":
             return
         if flag is None:
             flag = int(self.obs_overflow.item())
@@ -595,10 +689,11 @@ class Tower:
             raise ValueError("observation values must satisfy |v| < 65520 after normalisation: the encoder splits "
                              "each float32 value into two fp16 halves, and fp16 ends at 65504")
 
-    def forward(self, x, B, src_idx=None, encoded=None, masks=True, skip_first=False):
+    def forward(self, x, B, src_idx=None, encoded=None, masks=True, skip_first=False, seq=None):
         """encoded (mlp only): operand rows another tower already produced from the same observations.
-        masks=False (acting passes: no backward follows): the convs skip their 1-bit ReLU mask output.
-        skip_first (mlp only): hfc[0] was already produced by a fused first layer (common/policies.py)."""
+        masks=False (acting passes: no backward follows): the convs skip their 1-bit ReLU mask output, the LSTM its
+        saved gates.  skip_first (mlp only): hfc[0] was already produced by a fused first layer (common/policies.py).
+        seq (lstm, cnn_lstm): how the B rows form sequences (Seq, seq.T * seq.B == B)."""
         assert B <= self.cap
         if self.convs and self.shift_mode:
             h, ldh = self._forward_shift(x, B, src_idx, masks)
@@ -633,6 +728,9 @@ class Tower:
             if not (skip_first and i == 0):
                 l.forward(h, ldh, B, self.hfc[i], self.ld_hfc[i])
             h, ldh = self.hfc[i], self.ld_hfc[i]
+        if self.lstm is not None:
+            assert seq is not None and seq.T * seq.B == B, "recurrent towers take their rows as sequences"
+            h, ldh = self.lstm.forward(h, ldh, seq, train=masks)
         return h, ldh                                    # latent [B, latent_dim] fp16, row pitch ldh
 
     # consumes self.dlatent: fp16 [B, ld_dlatent] gradient w.r.t. the latent PRE-activation
@@ -640,6 +738,14 @@ class Tower:
         """skip_first_wgrad (mlp): the caller computes the first layer's weight gradient (fused over two towers)."""
         nfc = len(self.fcs)
         dz, lddz = self.dlatent, self.ld_dlatent
+        if self.lstm is not None:
+            if not self.fcs:                            # lstm: the input is the encoded observation
+                self.lstm.backward(alpha)
+                return
+            l = self.fcs[-1]                            # cnn_lstm: dx is fc1's output gradient through its ReLU
+            self.lstm.backward(alpha, dx=self.dzfc[-1], ldo=self.ld_hfc[-1], saved=self.hfc[-1],
+                               ld_saved=self.ld_hfc[-1], act=l.act)
+            dz, lddz = self.dzfc[-1], self.ld_hfc[-1]
         for i in reversed(range(nfc)):
             l = self.fcs[i]
             if i == 0 and skip_first_wgrad and not self.convs:

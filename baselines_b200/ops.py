@@ -468,3 +468,38 @@ def dqn_act(a, lda, s, lds, nA, eps, seed, step, actions, B, eps_dev=None, step_
     _chk(step_dev, torch.int64, "step_dev")
     _lib.call("b200rl_dqn_act", _ptr(a), int(lda), _ptr(s), int(lds), int(nA), float(eps), int(seed), int(step),
               _ptr(eps_dev), _ptr(step_dev), _ptr(actions), int(B), _stream())
+
+
+def lstm_seq_fwd(xg, ldxg, wh, masks, state_in, h_out, ldh, T, B, H, *, mask_idx=None, state_idx=None, state_out=None,
+                 hprev_out=None, gates_out=None, c_out=None):
+    """LSTM recurrence (a2c/utils.py:84-97) over T time-major steps of B environments: xg float32 [T*B, ldxg] (x.Wx + b),
+    wh fp16 [H, 4H], masks uint8 (done before the step; gathered through mask_idx), state_in float32 [*, 2H] = [c | h]
+    (gathered through state_idx).  See include/b200rl.h for the optional outputs."""
+    for t, dt, nm in ((xg, torch.float32, "xg"), (wh, torch.float16, "wh"), (masks, torch.uint8, "masks"),
+                      (mask_idx, torch.int64, "mask_idx"), (state_in, torch.float32, "state_in"),
+                      (state_idx, torch.int64, "state_idx"), (state_out, torch.float32, "state_out"),
+                      (h_out, torch.float16, "h_out"), (hprev_out, torch.float16, "hprev_out"),
+                      (gates_out, torch.float32, "gates_out"), (c_out, torch.float32, "c_out")):
+        _chk(t, dt, nm)
+    rows = T * B
+    _lib.call("b200rl_lstm_seq_fwd", _ptr(xg), int(ldxg), _ptr(wh), _ptr(masks), _ptr(mask_idx), _ptr(state_in),
+              _ptr(state_idx), _ptr(state_out), _ptr(h_out), int(ldh), _ptr(hprev_out), _ptr(gates_out), _ptr(c_out),
+              int(T), int(B), int(H), _stream(), label="lstm_seq_fwd",
+              flops=8.0 * rows * H * H,
+              nbytes=16.0 * rows * H + 8.0 * H * H * -(-B // 8) + 2.0 * rows * H
+              + (2.0 * rows * H + 16.0 * rows * H + 4.0 * rows * H if gates_out is not None else 0))
+
+
+def lstm_seq_bwd(dh, lddh, gates, c, masks, state_in, whT, dz, lddz, T, B, H, *, mask_idx=None, state_idx=None):
+    """Backward of lstm_seq_fwd: dz fp16 [T*B, lddz] = d loss / d (pre-activation gates) from dh fp16 [T*B, lddh]
+    (d loss / d h_t) and the forward's gates / c, walking t downwards with the dh carry through whT fp16 [4H, H]."""
+    for t, dt, nm in ((dh, torch.float16, "dh"), (gates, torch.float32, "gates"), (c, torch.float32, "c"),
+                      (masks, torch.uint8, "masks"), (mask_idx, torch.int64, "mask_idx"),
+                      (state_in, torch.float32, "state_in"), (state_idx, torch.int64, "state_idx"),
+                      (whT, torch.float16, "whT"), (dz, torch.float16, "dz")):
+        _chk(t, dt, nm)
+    rows = T * B
+    _lib.call("b200rl_lstm_seq_bwd", _ptr(dh), int(lddh), _ptr(gates), _ptr(c), _ptr(masks), _ptr(mask_idx),
+              _ptr(state_in), _ptr(state_idx), _ptr(whT), _ptr(dz), int(lddz), int(T), int(B), int(H), _stream(),
+              label="lstm_seq_bwd", flops=8.0 * rows * H * H,
+              nbytes=2.0 * rows * H + 16.0 * rows * H + 8.0 * rows * H + 8.0 * rows * H + 8.0 * H * H * -(-B // 8))

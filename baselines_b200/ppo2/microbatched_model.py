@@ -28,6 +28,13 @@ class MicrobatchedModel(Model):
                          microbatch_size=microbatch_size, **kw)
         self._acc = torch.zeros_like(self.net.store.grads)
 
+    def train(self, lr, cliprange, obs, returns, masks, actions, values, neglogpacs, states=None):
+        assert states is None, "microbatches with recurrent models are not supported yet"    # microbatched_model.py:36
+        return super().train(lr, cliprange, obs, returns, masks, actions, values, neglogpacs)
+
+    def train_rollout_seq(self, *args, **kwargs):
+        raise AssertionError("microbatches with recurrent models are not supported yet")
+
     def train_rollout(self, lr, cliprange, obs, actions, returns, values, neglogpacs, src_idx):
         net, store, opt = self.net, self.net.store, self.opt
         M = int(src_idx.numel()) if src_idx is not None else int(returns.numel())

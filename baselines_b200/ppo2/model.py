@@ -12,7 +12,8 @@ import numpy as np
 import torch
 
 from .. import graphs, ops
-from ..common.policies import PolicyNet
+from ..common.policies import RECURRENT_NETWORKS, PolicyNet
+from ..nn import Seq
 from ..common import dist_util
 
 
@@ -31,6 +32,8 @@ class Model(object):
             chunk = int(microbatch_size)
         self.chunk = max(1, min(chunk, max(1, nbatch_train)))
         cap = max(nbatch_act, self.chunk)
+        if getattr(policy, "network", None) in RECURRENT_NETWORKS:
+            cap = max(cap, nsteps)                            # a train chunk is whole environments x nsteps
         with torch.cuda.device(self.device):
             # ortho_init consumes the GLOBAL numpy stream seeded by set_global_seeds (ppo2.py:80), like the reference
             self.net = PolicyNet(policy, cap, self.device, rng=np.random)
@@ -40,6 +43,14 @@ class Model(object):
             self._act_nlp = torch.zeros(nbatch_act, dtype=torch.float32, device=self.device)
         self.loss_names = ['policy_loss', 'value_loss', 'policy_entropy', 'approxkl', 'clipfrac']   # model.py:115
         self.initial_state = None
+        self.recurrent = self.net.recurrent
+        if self.recurrent:
+            # policies.py:90-92 / models.py lstm: zeros [nenv, 2 * nlstm] (float64, like np.zeros there)
+            self.initial_state = np.zeros((nbatch_act, 2 * self.net.nlstm))
+            with torch.cuda.device(self.device):
+                self._act_state = torch.zeros(nbatch_act, 2 * self.net.nlstm, dtype=torch.float32, device=self.device)
+                self._act_mask = torch.zeros(nbatch_act, dtype=torch.uint8, device=self.device)
+            self._seq_idx = self._seq_env = None      # fixed homes of a recurrent minibatch's row / environment indices
         self.act_model = self.train_model = self
         self._rng_seed = int(np.random.randint(0, 2 ** 31 - 1))
         self.graphs = graphs.GraphCache()
@@ -52,46 +63,89 @@ class Model(object):
         self.net.refresh()
 
     # ------------------------------------------------------------------------------------ act path
-    def step_device(self, obs_dev, actions, values, neglogp, noise=None, persistent=False):
+    def _act_seq(self, B, state, mask, advance):
+        """Recurrent networks: one step of B environments from the device state [B, 2H] float32 with the device mask
+        uint8 [B] (done before this step); advance: the new state is written back in place."""
+        if not self.recurrent:
+            return None
+        if state is None or mask is None:
+            raise ValueError("a recurrent policy acts with a state and a mask (S=, M=)")
+        return Seq(1, B, mask, None, state, None, state if advance else None)
+
+    def step_device(self, obs_dev, actions, values, neglogp, noise=None, persistent=False, state=None, mask=None):
         """PolicyWithValue.step (policies.py:77-96) on device tensors; obs_dev as produced by net.encode_obs.
         persistent=True: the caller passes the same buffers on every call (the Runner's rollout slots), so the launch
-        sequence is captured once per slot and replayed."""
+        sequence is captured once per slot and replayed.  Recurrent networks: state float32 [B, 2H] is advanced in
+        place, mask uint8 [B] is "done before this step"."""
         B = obs_dev.shape[0]
+        seq = self._act_seq(B, state, mask, True)
         if persistent and noise is None:
             key = ("act", obs_dev.data_ptr(), actions.data_ptr(), values.data_ptr(), neglogp.data_ptr(), B)
-            self.graphs.run(key, lambda: self.net.act(obs_dev, B, actions, values, neglogp, seed=self._rng_seed))
+            if seq is not None:
+                key += (state.data_ptr(), mask.data_ptr())
+            self.graphs.run(key, lambda: self.net.act(obs_dev, B, actions, values, neglogp, seed=self._rng_seed,
+                                                      seq=seq))
         else:
-            self.net.act(obs_dev, B, actions, values, neglogp, noise=noise, seed=self._rng_seed)
+            self.net.act(obs_dev, B, actions, values, neglogp, noise=noise, seed=self._rng_seed, seq=seq)
 
-    def value_device(self, obs_dev, values, persistent=False):
+    def value_device(self, obs_dev, values, persistent=False, state=None, mask=None):
+        """Recurrent networks: state / mask as in step_device; the state is not advanced (policies.py:98-119)."""
         B = obs_dev.shape[0]
+        seq = self._act_seq(B, state, mask, False)
 
         def body():
-            self.net.forward(obs_dev, B)
+            self.net.forward(obs_dev, B, masks=seq is None, seq=seq)
             values.copy_(self.net.v_out[:B, 0] if self.net.v_out.dim() == 2 else self.net.v_out[:B])
         if persistent:
-            self.graphs.run(("value", obs_dev.data_ptr(), values.data_ptr(), B), body)
+            key = ("value", obs_dev.data_ptr(), values.data_ptr(), B)
+            if seq is not None:
+                key += (state.data_ptr(), mask.data_ptr())
+            self.graphs.run(key, body)
         else:
             body()
 
+    def _host_state(self, B, S, M):
+        """Upload the reference's S (float [B, 2H]) and M (bool [B]) for a host-side step / value call."""
+        if not self.recurrent:
+            return None, None
+        if B > self._act_state.shape[0]:
+            st = torch.zeros(B, 2 * self.net.nlstm, dtype=torch.float32, device=self.device)
+            mk = torch.zeros(B, dtype=torch.uint8, device=self.device)
+        else:
+            st, mk = self._act_state[:B], self._act_mask[:B]
+        if S is None:
+            st.zero_()
+        else:
+            st.copy_(torch.from_numpy(np.ascontiguousarray(S, dtype=np.float32).reshape(B, -1)))
+        if M is None:
+            mk.zero_()
+        else:
+            mk.copy_(torch.from_numpy(np.asarray(M).astype(np.uint8).reshape(B)))
+        return st, mk
+
     def step(self, observation, S=None, M=None, noise=None, **_):
-        """numpy in / numpy out, like the reference: (actions, values, states=None, neglogpacs)."""
+        """numpy in / numpy out, like the reference: (actions, values, states, neglogpacs).  Recurrent networks take the
+        state S [B, 2H] and the mask M [B] (done before this step) and return the new state as float32; the others
+        return states=None."""
         with torch.cuda.device(self.device):
             x = self.net.encode_obs(np.asarray(observation))
             B = x.shape[0]
             a, v, n = self._bufs(B)
             nz = None if noise is None else torch.as_tensor(np.ascontiguousarray(noise), dtype=torch.float32).to(self.device)
-            self.step_device(x, a, v, n, noise=nz)
-            out = self.net.actions_to_numpy(a), v.cpu().numpy(), None, n.cpu().numpy()
+            st, mk = self._host_state(B, S, M)
+            self.step_device(x, a, v, n, noise=nz, state=st, mask=mk)
+            out = (self.net.actions_to_numpy(a), v.cpu().numpy(), None if st is None else st.cpu().numpy(),
+                   n.cpu().numpy())
             self.net.check_obs_range()
             return out
 
-    def value(self, ob, *args, **kwargs):
+    def value(self, ob, *args, S=None, M=None, **kwargs):
         with torch.cuda.device(self.device):
             x = self.net.encode_obs(np.asarray(ob))
             B = x.shape[0]
             _, v, _ = self._bufs(B)
-            self.value_device(x, v)
+            st, mk = self._host_state(B, S, M)
+            self.value_device(x, v, state=st, mask=mk)
             out = v.cpu().numpy()
             self.net.check_obs_range()
             return out
@@ -167,6 +221,69 @@ class Model(object):
             self._after_train_call()
             return self._stats_out / M
 
+    def train_rollout_seq(self, lr, cliprange, obs, actions, returns, values, neglogpacs, dones, states0, rows, envs,
+                          eager=False):
+        """One recurrent minibatch of ppo2/model.py:133-158 (ppo2.py:167-180): whole environments with their start
+        states.  obs/actions/returns/values/neglogpacs/dones: flat device buffers; states0: float32 [*, 2H] device;
+        rows: host int64 [E, T], the buffer offsets of environment e's steps; envs: host int64 [E], its rows of
+        states0.  The sequence kernels take time-major rows (t*E + e), so the launch order is built here; the loss is a
+        mean, so the order does not change it.  Chunks are whole environments (chunk // T of them).  Returns a device
+        float64[5] of the loss statistics.  eager: the buffers are the caller's temporaries (no graph capture)."""
+        net, store = self.net, self.net.store
+        rows = np.asarray(rows, dtype=np.int64)
+        envs = np.asarray(envs, dtype=np.int64).reshape(-1)
+        E, T = rows.shape
+        M = E * T
+        per = max(1, self.chunk // T)
+        chunks = [(e0, min(E, e0 + per)) for e0 in range(0, E, per)]
+        # per chunk, the time-major row offsets of its environments, chunk after chunk
+        order = np.concatenate([rows[e0:e1].T.reshape(-1) for e0, e1 in chunks])
+        with torch.cuda.device(self.device):
+            dev = self.device
+            if self._seq_idx is None or self._seq_idx.numel() < M or self._seq_env.numel() < E:
+                self._seq_idx = torch.empty(max(M, self.nbatch_train), dtype=torch.int64, device=dev)
+                self._seq_env = torch.empty(max(E, self.nbatch_train // max(T, 1), 1), dtype=torch.int64, device=dev)
+            self._seq_idx[:M].copy_(torch.from_numpy(order))
+            self._seq_env[:E].copy_(torch.from_numpy(envs))
+            ops.set_scalars(net.clip_dev, cliprange)
+            self.opt.begin_step(lr)
+            idx, env = self._seq_idx, self._seq_env
+            inv_M = 1.0 / M
+
+            def grads():
+                store.grads.zero_()
+                net.stats.zero_()
+                ops.adv_stats(returns, values, idx[:M], M, net.adv_st)                        # model.py:139
+                for e0, e1 in chunks:
+                    B, s = (e1 - e0) * T, e0 * T
+                    seq = Seq(T, e1 - e0, dones, idx[s:s + B], states0, env[e0:e1], None)
+                    net.loss_backward(obs, B, idx[s:s + B], actions, returns, values, neglogpacs, None,
+                                      self.ent_coef, self.vf_coef, inv_M, seq=seq)
+                net.freeze_identity()
+
+            def update():
+                self.opt.apply()
+                net.refresh()
+                self._stats_out.copy_(net.stats)
+
+            if eager:
+                grads()
+                self.dist.average_gradients(store)
+                update()
+                self._after_train_call()
+                return self._stats_out / M
+            key = ("train_seq", E, T, obs.data_ptr(), actions.data_ptr(), returns.data_ptr(), values.data_ptr(),
+                   neglogpacs.data_ptr(), dones.data_ptr(), states0.data_ptr(), idx.data_ptr(), env.data_ptr())
+            if self.dist.active and os.environ.get("B200RL_GRAPH_NCCL", "0") != "1":
+                self.graphs.run(key + ("grads",), grads)
+                self.dist.average_gradients(store)
+                self.graphs.run(key + ("update",), update)
+            else:
+                self.graphs.run(key, lambda: (grads(), self.dist.average_gradients(store), update()),
+                                allow_fallback=self.dist.active)
+            self._after_train_call()
+            return self._stats_out / M
+
     def _after_train_call(self):
         """mpi_adam_optimizer.py:41-42: every 100th compute_gradients call checks that the ranks still hold identical
         parameters (check_synced :53-68); a mismatch is a hard error there (assert) and here."""
@@ -177,15 +294,29 @@ class Model(object):
                                      "mpi_adam_optimizer.py:53-68) after {} train calls".format(self._train_calls))
 
     def train(self, lr, cliprange, obs, returns, masks, actions, values, neglogpacs, states=None):
-        """Reference signature (model.py:133); numpy minibatch in, list of 5 python floats out."""
-        if states is not None:
-            raise NotImplementedError("recurrent policies are outside the hot-path scope (SURVEY.md 2, #4)")
+        """Reference signature (model.py:133); numpy minibatch in, list of 5 python floats out.  Recurrent networks:
+        the rows are whole environments, env-major (row e * nsteps + t, ppo2.py:174-176), and states [nenv, 2H] are
+        their start states."""
+        if states is not None and not self.recurrent:
+            raise NotImplementedError("states are only taken by recurrent policies ('lstm', 'cnn_lstm')")
+        if states is None and self.recurrent:
+            raise ValueError("a recurrent policy trains from the start states of its minibatch (states=)")
         with torch.cuda.device(self.device):
             dev = self.device
             x = self.net.encode_obs(np.asarray(obs))
             a = torch.as_tensor(np.ascontiguousarray(actions), dtype=self.net.action_dtype).to(dev).contiguous()
             f = lambda z: torch.as_tensor(np.ascontiguousarray(z), dtype=torch.float32).to(dev)
-            st = self.train_rollout(float(lr), float(cliprange), x, a, f(returns), f(values), f(neglogpacs), None)
+            if self.recurrent:
+                T = self.nsteps
+                E = int(np.shape(states)[0])
+                assert x.shape[0] == E * T, "a recurrent minibatch is nenv whole sequences of nsteps"
+                m = torch.from_numpy(np.asarray(masks).astype(np.uint8).reshape(-1)).to(dev)
+                rows = np.arange(E * T, dtype=np.int64).reshape(E, T)
+                st = self.train_rollout_seq(float(lr), float(cliprange), x, a, f(returns), f(values), f(neglogpacs),
+                                            m, f(np.asarray(states).reshape(E, -1)), rows, np.arange(E),
+                                            eager=True)
+            else:
+                st = self.train_rollout(float(lr), float(cliprange), x, a, f(returns), f(values), f(neglogpacs), None)
             out = [float(s) for s in st.cpu().numpy()]
             self.net.check_obs_range()
             return out

@@ -127,7 +127,12 @@ def run_epochs(model, ro, lrnow, cliprangenow, nbatch, nbatch_train, noptepochs,
                      same minibatches as the reference; the 8-byte indices cross PCIe (default, $B200RL_SHUFFLE);
       shuffle="device" a keyed bijection evaluated by a kernel (ops.shuffle_indices): nothing is generated or uploaded
                      on the host -- at cfg-3 sizes (8.4 M samples x 10 epochs) the host shuffle alone costs ~1 s per
-                     update.  The key is drawn from the seeded numpy stream, so runs stay reproducible."""
+                     update.  The key is drawn from the seeded numpy stream, so runs stay reproducible.
+                     Feed-forward policies only: a recurrent one always shuffles on the host.
+    Recurrent policies (ppo2.py:167-180): the permutation is over environments (perms: [noptepochs][nenvs]); a
+    minibatch is nenvs / nminibatches whole environments with their rollout-start states."""
+    if getattr(model, "recurrent", False):
+        return _run_epochs_recurrent(model, ro, lrnow, cliprangenow, nbatch // nbatch_train, noptepochs, perms)
     out = []
     shuffle = shuffle or os.environ.get("B200RL_SHUFFLE", "host")
     inds = np.arange(nbatch) if (perms is not None or shuffle == "host") else None
@@ -147,4 +152,26 @@ def run_epochs(model, ro, lrnow, cliprangenow, nbatch, nbatch_train, noptepochs,
         for start in range(0, nbatch, nbatch_train):
             mb = src[start:start + nbatch_train]
             out.append(model.train_rollout(lrnow, cliprangenow, obs, actions, returns, values, neglogp, mb))
+    return out
+
+
+def _run_epochs_recurrent(model, ro, lrnow, cliprangenow, nminibatches, noptepochs, perms):
+    nenvs, T = ro.N, ro.T
+    assert nenvs % nminibatches == 0                                        # ppo2.py:168
+    envsperbatch = nenvs // nminibatches
+    envinds = np.arange(nenvs)
+    flatinds = np.arange(T)[None, :] * nenvs + envinds[:, None]             # [env, t] -> buffer offset t*N + env
+    obs, actions = ro.flat("obs"), ro.flat("actions")
+    returns, values, neglogp = ro.flat("returns"), ro.flat("values"), ro.flat("neglogpacs")
+    dones = ro.flat("dones")
+    out = []
+    for ep in range(noptepochs):
+        if perms is None:
+            np.random.shuffle(envinds)                                      # ppo2.py:172
+        else:
+            envinds = np.asarray(perms[ep])
+        for start in range(0, nenvs, envsperbatch):
+            mbenvinds = envinds[start:start + envsperbatch]                 # ppo2.py:174-176
+            out.append(model.train_rollout_seq(lrnow, cliprangenow, obs, actions, returns, values, neglogp, dones,
+                                               ro.states0, flatinds[mbenvinds], mbenvinds))
     return out

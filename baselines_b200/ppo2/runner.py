@@ -18,9 +18,10 @@ class Rollout:
     """Time-major [T, N] rollout arrays in HBM.  Flat env-major index i = e*T + t (runner.py:69-74) maps to
     buffer offset t*N + e."""
 
-    def __init__(self, T, N, obs_store_shape, obs_dtype, discrete, act_dim, device, act_dtype=None):
+    def __init__(self, T, N, obs_store_shape, obs_dtype, discrete, act_dim, device, act_dtype=None, state_dim=0):
         """discrete: int64 [T, N] actions (Discrete); otherwise [T, N, act_dim] rows of act_dtype (float32 for Box and
-        MultiBinary, int64 for MultiDiscrete)."""
+        MultiBinary, int64 for MultiDiscrete).  state_dim > 0 (recurrent policies): states0 float32 [N, state_dim] holds
+        the policy state at the start of the rollout (runner.py:31 mb_states)."""
         self.T, self.N, self.device = T, N, device
         f32 = dict(dtype=torch.float32, device=device)
         self.obs = torch.zeros((T, N) + tuple(obs_store_shape), dtype=obs_dtype, device=device)
@@ -34,6 +35,7 @@ class Rollout:
         self.returns = torch.zeros(T, N, **f32)
         self.last_values = torch.zeros(N, **f32)
         self.last_dones = torch.zeros(N, dtype=torch.uint8, device=device)
+        self.states0 = torch.zeros(N, state_dim, **f32) if state_dim else None
         self._arange = None
 
     @property
@@ -79,7 +81,8 @@ class Runner:
         # common/input.py:56-57); the encode kernel reads them through the minibatch indices
         store_shape = tuple(ob_space.shape) if self.u8 else (net.tower_pi.raw_dim,)
         self.rollout = Rollout(nsteps, nenv, store_shape, torch.uint8 if self.u8 else torch.float32, net.pd == "cat",
-                               net.act_dim, self.device, act_dtype=net.action_dtype)
+                               net.act_dim, self.device, act_dtype=net.action_dtype,
+                               state_dim=2 * net.nlstm if net.recurrent else 0)
         # pinned staging for the per-step host<->device traffic
         pin = torch.cuda.is_available()
         np_dtype = np.dtype(ob_space.dtype.name) if hasattr(ob_space.dtype, "name") else np.dtype(ob_space.dtype)
@@ -138,6 +141,23 @@ class Runner:
         self.states = model.initial_state
         self.dones = np.zeros(nenv, dtype=np.bool_)                            # runners.py:14
         self._dev_dones = torch.zeros(nenv, dtype=torch.uint8, device=self.device)
+        # recurrent policies (runner.py:31-36): the state lives on the device and is advanced in place by every acting
+        # pass; the mask of step t (done before step t) reaches the device before that step's pass
+        self.recurrent = net.recurrent
+        if self.recurrent:
+            st = np.zeros((nenv, 2 * net.nlstm), np.float32) if self.states is None else self.states
+            self._state_dev = torch.from_numpy(np.ascontiguousarray(st, dtype=np.float32)).to(self.device)
+            self._mask_dev = torch.zeros(nenv, dtype=torch.uint8, device=self.device)
+
+    def _rnn(self):
+        """step_device / value_device keywords of a recurrent policy: the state and this step's mask."""
+        if not self.recurrent:
+            return {}
+        if self.device_env:
+            self._mask_dev.copy_(self._dev_dones)
+        else:
+            self._mask_dev.copy_(torch.from_numpy(self.dones.astype(np.uint8)))
+        return dict(state=self._state_dev, mask=self._mask_dev)
 
     def _take_obs(self, obs):
         """`self.obs[:] = obs` of the reference (runner.py:38), except that an env which already hands out
@@ -225,14 +245,17 @@ class Runner:
                 model.net.check_obs_range(flag)
             if self.fs:
                 ro.obs[0].copy_(self._cur)
-            chunked = self.fs and self.act_chunks > 1 and nz is None
+            if self.recurrent:
+                ro.states0.copy_(self._state_dev)                              # runner.py:31 mb_states = self.states
+            # chunked acting overlaps step t+1's pass with the upload; a recurrent pass waits for step t+1's mask instead
+            chunked = self.fs and self.act_chunks > 1 and nz is None and not self.recurrent
             acted = False                      # step t's policy pass already issued (chunk-wise, with the upload)
             for t in range(T):
                 if not self.fs:
                     self._upload_obs(ro.obs[t])
                 if not acted:
                     model.step_device(ro.obs[t], ro.actions[t], ro.values[t], ro.neglogpacs[t],
-                                      noise=None if nz is None else nz[t], persistent=True)
+                                      noise=None if nz is None else nz[t], persistent=True, **self._rnn())
                 acted = False
                 if self.device_env:
                     ro.dones[t].copy_(self._dev_dones)
@@ -269,7 +292,7 @@ class Runner:
             # bootstrap value of the final observation (runner.py:50)
             if not self.fs:
                 self._upload_obs(self._cur)
-            model.value_device(self._cur, ro.last_values, persistent=True)
+            model.value_device(self._cur, ro.last_values, persistent=True, **self._rnn())   # runner.py:50
             if self.device_env:
                 ro.last_dones.copy_(self._dev_dones)
                 if not self.u8:
@@ -299,5 +322,9 @@ class Runner:
         actions = ro.to_reference_numpy("actions")
         if self.model.net.pd == "mcat":
             actions = actions.astype(np.int32)                              # distributions.py:222 tf.int32
+        states = None
+        if self.recurrent:
+            states = ro.states0.cpu().numpy()                               # the states at the start of the rollout
+            self.states = self._state_dev.cpu().numpy()
         return (obs, ro.to_reference_numpy("returns"), masks, actions,
-                ro.to_reference_numpy("values"), ro.to_reference_numpy("neglogpacs"), self.states, epinfos)
+                ro.to_reference_numpy("values"), ro.to_reference_numpy("neglogpacs"), states, epinfos)

@@ -238,6 +238,25 @@ int b200rl_dqn_act(const float* a, long long lda, const float* s, long long lds,
                    unsigned long long seed, unsigned long long step, const float* eps_dev,
                    const unsigned long long* step_dev, long long* actions, int B, void* stream);
 
+/* LSTM recurrence: a2c/utils.py:84-97 lstm() over T steps (the cell of common/models.py lstm / cnn_lstm) and its
+ * gradient (the BPTT TF derives for ppo2/model.py:102).  xg = x.Wx + b comes from b200rl_gemm_f16; rows are time-major
+ * (row t*B + b), gate columns the reference's [i | f | o | u] blocks, the state [*, 2H] = [c | h] float32.
+ * mask of row r = masks[mask_idx ? mask_idx[r] : r], "done before step t" (c and h are zeroed before the step);
+ * environment b starts from state_in row state_idx ? state_idx[b] : b.  H = 64 or 128.
+ * fwd: h_out fp16 [T*B, ldh]; optional state_out [B, 2H] (final c, h; may alias state_in when state_idx is NULL),
+ * hprev_out fp16 [T*B, H] (masked h_{t-1}), gates_out [T*B, 4H] (sigma(i), sigma(f), sigma(o), tanh(u); may alias xg
+ * when ldxg = 4H) and c_out [T*B, H], the last three for the backward.
+ * bwd: dz fp16 [T*B, lddz] = d loss / d (pre-activation gates) from dh (d loss / d h_t, fp16) and the forward's saved
+ * gates and c; whT = Wh^T fp16 [4H, H].  dWh = hprev^T dz, dWx = x^T dz, db = colsum(dz), dx = dz Wx^T follow on the
+ * GEMM. */
+int b200rl_lstm_seq_fwd(const float* xg, long long ldxg, const void* wh, const uint8_t* masks, const long long* mask_idx,
+                        const float* state_in, const long long* state_idx, float* state_out, void* h_out,
+                        long long ldh, void* hprev_out, float* gates_out, float* c_out, int T, int B, int H,
+                        void* stream);
+int b200rl_lstm_seq_bwd(const void* dh, long long lddh, const float* gates, const float* c, const uint8_t* masks,
+                        const long long* mask_idx, const float* state_in, const long long* state_idx, const void* whT,
+                        void* dz, long long lddz, int T, int B, int H, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
