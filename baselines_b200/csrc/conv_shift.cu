@@ -19,7 +19,12 @@
 // or, in the wgrad, the fused bias-gradient sums -- from their own registers) | warp 8 TMA loads | uint8-fed first
 // layer only: warps 9-16 are uint8 producers that cast raw frames into a rolling A ring instead of the TMA.  The
 // forward epilogue can also write 1 bit per output element (act > 0); the dgrad of the next layer reads that as its
-// ReLU mask.
+// ReLU mask, which the TMA warp stages with each A tile (one bulk copy of the tile's 128 mask rows on the stage's full
+// barrier), so the epilogue reads it from shared memory.
+//
+// Epilogue: bias / ReLU / alpha (or the mask) are applied to the fp32 accumulators and rounded to fp16 in registers;
+// each warp then moves its 16-row fragment through a small shared scratch (stmatrix) so that every lane holds 8
+// consecutive columns of one row, and the tile leaves as 16-byte stores (the ReLU bits as one 16-bit word per two lanes).
 //
 // "Ping-pong" schedule of the forward / dgrad: the two consumer warpgroups take whole 128-row tiles (even / odd) and
 // turns on the tensor cores.  Named barriers 2 and 3 order their MMA issue: a group issues its next tile only after
@@ -60,6 +65,11 @@ __host__ __device__ constexpr int sh_wres_bytes(int KH, bool u8) {
   return u8 ? SH_U8_WRES_BYTES : KH == 1 ? 80 * 1024 : 64 * 1024;
 }
 static constexpr int SH_BAR_BYTES = 512;             // forward kernel: mbarrier block after the weights
+// forward / dgrad kernel, after the barriers: the staged ReLU mask of each A stage (DACT: 128 rows x BN bits), then one
+// 16-row x 32-column fp16 epilogue scratch per consumer warp
+__host__ __device__ constexpr int sh_mask_stage_bytes(int BN, bool DACT) { return DACT ? SH_BM * BN / 8 : 0; }
+static constexpr int SH_EPI_WARP_BYTES = 16 * 64;
+static constexpr int SH_EPI_BYTES = SH_CONSUMER_WARPS * SH_EPI_WARP_BYTES;
 static constexpr int SH_WROWS_K = 96;                // wgrad: 64 + max shift span (<= 32)
 static constexpr int SH_WABYTES = SH_WROWS_K * 128;
 // wgrad: at most QW 64-channel accumulator chunks per consumer warpgroup (QW * N/2 accumulator registers per thread).
@@ -281,8 +291,8 @@ struct ShiftParams {
   __half* out;
   AddrMap omap;
   uint16_t* bits_out;           // optional (forward): bit k of word e/16 = (out element e + k) > 0, e = element offset
-  const uint16_t* saved_bits;   // optional (DACT): the same bit array of the saved activation (ReLU mask)
-  AddrMap smap;
+  const uint16_t* saved_bits;   // optional (DACT): the same bit array of the saved activation (ReLU mask), rows of
+                                // N bits at m * N (row-contiguous), 16-byte aligned
   const float* bias;
   int act, dact;           // dact = 1: multiply by the saved_bits mask (if any) instead of applying act
   float alpha;
@@ -290,6 +300,31 @@ struct ShiftParams {
 };
 
 // ------------------------------------------------------------------------------------------------ forward / dgrad
+// Epilogue transpose: the accumulator fragment of one warp (16 rows; thread t holds 2 columns of rows t/4 and t/4 + 8 per
+// 8-column block) goes through a per-warp scratch of 16 rows x 64 B so that each lane then holds 8 consecutive columns
+// of one row.  16-byte piece p of scratch row r lives at slot p ^ ((r >> 1) & 3): the 8 rows of one stmatrix matrix,
+// and the 8 lanes of a quarter-warp load, hit 8 distinct 16-byte slots of 128 B (no bank conflict).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+// (a plain uint4 store is split into four 4-byte stores by the compiler here)
+__device__ __forceinline__ void st_global_v4(void* p, const uint4& v) {
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
+// bits 2k, 2k + 1 of b8 -> 0xffff in the low / high half of the word (the mask of fp16 elements 2k, 2k + 1)
+__device__ __forceinline__ uint32_t mask_pair(uint32_t b8, int k) {
+  const uint32_t b = b8 >> (2 * k);
+  return ((b & 1u) | ((b & 2u) << 15)) * 0xffffu;
+}
+
 // Weights: [BN rows, taps*KH*64 columns (t, h, c)], all resident in shared memory as (t, h) sub-tiles of BN rows x 128 B.
 template <int BN, int KH, bool DACT, bool U8>
 __global__ void __launch_bounds__(sh_threads(U8), 1)
@@ -317,6 +352,9 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
   uint64_t* w_bar = bars + 2 * STAGES;
   uint64_t* head_bar = bars + 2 * STAGES + 1;        // U8: first unit of the stage's tile is in place
   static_assert((3 * STAGES + 1) * 8 <= SH_BAR_BYTES, "barrier block");
+  constexpr int MASK_STAGE = sh_mask_stage_bytes(BN, DACT);
+  uint8_t* smask = reinterpret_cast<uint8_t*>(bars) + SH_BAR_BYTES;   // DACT: the mask rows of stage s's tile
+  uint8_t* sepi = smask + STAGES * MASK_STAGE;                         // epilogue scratch, one per consumer warp
 
   __shared__ float s_bias[BN];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -370,10 +408,25 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
         mbar_wait(&empty_bar[s], ph ^ 1);
         if (elect_one()) {
           uint8_t* sa = smem + s * STAGE_BYTES;
-          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)STAGE_BYTES);
+          // DACT: the tile's mask words are one contiguous run (rows of BN bits), clamped to M; the bulk copy takes
+          // whole 16-byte pieces and this thread copies the last 4- or 8-byte rows of a short tail itself (before its
+          // arrive, which releases them to the consumers)
+          uint32_t mbytes = 0;
+          const uint8_t* msrc = nullptr;
+          if (DACT && p.saved_bits != nullptr) {
+            const long long left = p.M - (long long)tile * SH_BM;
+            mbytes = (uint32_t)(left < SH_BM ? left : SH_BM) * (BN / 8);
+            msrc = reinterpret_cast<const uint8_t*>(p.saved_bits) + (long long)tile * MASK_STAGE;
+#pragma unroll 1
+            for (uint32_t b = mbytes & ~15u; b < mbytes; b += 4)
+              *reinterpret_cast<uint32_t*>(smask + s * MASK_STAGE + b) = __ldg(reinterpret_cast<const uint32_t*>(msrc + b));
+            if (mbytes & 15u) __threadfence_block();          // the tail stores are performed before the arrive
+          }
+          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)STAGE_BYTES + (mbytes & ~15u));
           const int row0 = tile * SH_BM + p.min_shift;                  // may be negative: TMA zero-fills
 #pragma unroll
           for (int h = 0; h < KH; ++h) tma_load_2d(sa + h * SH_ABYTES, &tmX, &full_bar[s], h * 64, row0);
+          if (mbytes >= 16) bulk_load_1d(smask + s * MASK_STAGE, msrc, mbytes & ~15u, &full_bar[s]);
         }
         __syncwarp();
         if (++s == STAGES) { s = 0; ph ^= 1; }
@@ -389,11 +442,21 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
     // of each accumulator.  (wg is broadcast: the compiler then knows the tile loop is warp-uniform and keeps the
     // wgmma chain asynchronous.)
     const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), t = threadIdx.x & 127;
-    const int row0 = PINGPONG ? 0 : wg * 64, r0 = row0 + acc_row(t, 0);
+    const int row0 = PINGPONG ? 0 : wg * 64;
     const uint32_t w_base = smem_u32(wres);
     const float lo = (p.act == ACT_RELU) ? 0.0f : -INFINITY;
     const __half2 lo2 = __floats2half2_rn(lo, lo);
     const __half2 zero2 = __floats2half2_rn(0.0f, 0.0f);
+    // Epilogue: after the transpose, lane l holds columns 8 * (l >> 4) .. + 7 of each 16-column chunk of row
+    // er = l & 15 of the warp's 16 rows (rows 16 * (warp % 4) + er of each m64 accumulator).  That is also the row
+    // and piece whose address lane l hands to stmatrix for the chunk, so one scratch address per chunk parity.
+    const int er = lane & 15, ep = lane >> 4;
+    const int erow = row0 + 16 * (warp & 3) + er;                 // tile row of accumulator 0
+    uint32_t epi_addr[2];
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj)
+      epi_addr[jj] = smem_u32(sepi + warp * SH_EPI_WARP_BYTES) + er * 64 + (((2 * jj + ep) ^ ((er >> 1) & 3)) << 4);
+    const bool masked = DACT && p.saved_bits != nullptr;
     float acc[MH][BN / 2];
     mbar_wait(w_bar, 0);
     for (int i = PINGPONG ? wg : 0; i < tile_count; i += PINGPONG ? 2 : 1) {
@@ -426,58 +489,93 @@ conv_shift_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_cons
       wgmma_commit();
       if (PINGPONG && i + 1 < tile_count) order_pass(wg);         // the other group may issue tile i + 1
       wgmma_wait<0>();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&empty_bar[s]);
-        if (U8) mbar_arrive(&empty_bar[s1]);                      // the head unit this tile read
+      auto release = [&]() {
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&empty_bar[s]);
+          if (U8) mbar_arrive(&empty_bar[s1]);                    // the head unit this tile read
+        }
+      };
+      // DACT: this lane's mask rows (BN bits each).  The stage is released only after the epilogue has used them: an
+      // arrive does not wait for a shared-memory load still in flight, and while the other group's MMAs stream their
+      // operands from shared memory such a load can still be pending when the TMA warp refills the stage.
+      uint32_t mrow[MH][BN / 32];
+      if (masked) {
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) {
+          const uint32_t r = smem_u32(smask + s * MASK_STAGE) + (uint32_t)((erow + mh * 64) * (BN / 8));
+#pragma unroll
+          for (int i = 0; i < BN / 32; ++i) asm volatile("ld.shared.b32 %0, [%1];" : "=r"(mrow[mh][i]) : "r"(r + 4 * i));
+        }
+      } else {
+        release();
       }
 
 #pragma unroll
-      for (int q = 0; q < 2 * MH; ++q) {                              // accumulator mh, its row r0 + 8 * hr
-        const int mh = q >> 1, hr = q & 1;
-        const uint32_t m = (uint32_t)tile * SH_BM + mh * 64 + r0 + 8 * hr;   // M < 2^31 (checked on the host)
+      for (int mh = 0; mh < MH; ++mh) {
+        const uint32_t m = (uint32_t)tile * SH_BM + mh * 64 + erow;    // M < 2^31 (checked on the host)
         const uint32_t t2 = p.fwg.div(m);
         const int x = (int)(m - t2 * (uint32_t)p.Wg);
         const int n = (int)p.fhg.div(t2);
         const int y = (int)(t2 - (uint32_t)n * (uint32_t)p.Hg);
         const bool ok = ((long long)m < p.M) && (y < p.vy) && (x < p.vx);
         const long long obase = map_rowbase(p.omap, n, y, x);
-        const bool masked = DACT && p.saved_bits != nullptr && ok;
-        const long long sbase = masked ? map_rowbase(p.smap, n, y, x) : 0;
 #pragma unroll
-        for (int j = 0; j < BN / 16; ++j) {                  // 16-column chunks: two 8-column accumulator blocks
-          uint32_t mw = 0xffffu;                              // activation-derivative bits of the chunk (DACT)
-          // a 16-column chunk never straddles a class of the maps: column 16 * j + cc lies at coloff(16 * j) + cc
-          const long long ocol = map_coloff(p.omap, 16 * j);
-          const long long scol = DACT ? map_coloff(p.smap, 16 * j) : 0;
-          if (masked) mw = __ldg(p.saved_bits + ((sbase + scol) >> 4));
-          uint32_t bits = 0;
+        for (int ps = 0; ps < BN / 32; ++ps) {               // passes of 32 columns = two 16-column chunks
 #pragma unroll
           for (int jj = 0; jj < 2; ++jj) {
-            const int e = 4 * (2 * j + jj) + 2 * hr;
-            const int cc = 8 * jj + 2 * (t & 3);              // column within the chunk
-            const int c = 16 * j + cc;
-            __half2 o;
-            if (DACT) {
-              const uint32_t mb = mw >> cc;
-              o = __floats2half2_rn((mb & 1u) ? acc[mh][e] * p.alpha : 0.0f,
-                                    (mb & 2u) ? acc[mh][e + 1] * p.alpha : 0.0f);
-            } else {                                          // relu after the rounding: same result, one packed max
-              o = __hmax2(__floats2half2_rn(fmaf(acc[mh][e], p.alpha, s_bias[c]),
-                                            fmaf(acc[mh][e + 1], p.alpha, s_bias[c + 1])),
-                          lo2);
-              const uint32_t gt = __hgt2_mask(o, zero2);
-              bits |= ((gt & 1u) | ((gt >> 15) & 2u)) << cc;
+            // chunk 2 * ps + jj = 8-column blocks b, b + 1; stmatrix matrices (b, row t/4), (b, + 8), (b + 1, ...)
+            const int b = 2 * (2 * ps + jj);
+            uint32_t r[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const int e = 4 * (b + (k >> 1)) + 2 * (k & 1);
+              const int c = 8 * (b + (k >> 1)) + 2 * (t & 3);
+              __half2 o;
+              if (DACT) {                                     // the mask is applied to the fp16 words below
+                o = __floats2half2_rn(acc[mh][e] * p.alpha, acc[mh][e + 1] * p.alpha);
+              } else {                                        // relu after the rounding: same result, one packed max
+                o = __hmax2(__floats2half2_rn(fmaf(acc[mh][e], p.alpha, s_bias[c]),
+                                              fmaf(acc[mh][e + 1], p.alpha, s_bias[c + 1])),
+                            lo2);
+              }
+              r[k] = h2_bits(o);
             }
-            if (ok) *reinterpret_cast<__half2*>(p.out + obase + ocol + cc) = o;
+            stmatrix_x4(epi_addr[jj], r);
           }
-          if (!DACT && p.bits_out != nullptr) {               // the four lanes of a row assemble the chunk's 16 bits
-            bits |= __shfl_xor_sync(0xffffffffu, bits, 1);
-            bits |= __shfl_xor_sync(0xffffffffu, bits, 2);
-            if (ok && (t & 3) == 0) p.bits_out[(obase + ocol) >> 4] = (uint16_t)bits;
+          __syncwarp();
+#pragma unroll
+          for (int jj = 0; jj < 2; ++jj) {
+            const int j = 2 * ps + jj;
+            uint4 v = ld_shared_v4(epi_addr[jj]);            // columns 16 * j + 8 * ep .. + 7 of row er
+            // a 16-column chunk never straddles a class of the map: column 16 * j + cc lies at coloff(16 * j) + cc
+            const long long ocol = map_coloff(p.omap, 16 * j);
+            if (masked) {
+              // zeroing the rounded value gives what rounding 0.0f gives: +0
+              const uint32_t b8 = (mrow[mh][j >> 1] >> (16 * (j & 1) + 8 * ep)) & 0xffu;
+              v.x &= mask_pair(b8, 0);
+              v.y &= mask_pair(b8, 1);
+              v.z &= mask_pair(b8, 2);
+              v.w &= mask_pair(b8, 3);
+            }
+            if (ok) st_global_v4(p.out + obase + ocol + 8 * ep, v);
+            if (!DACT && p.bits_out != nullptr) {             // the two lanes of a row assemble the chunk's 16 bits
+              const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+              uint32_t bits = 0;
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const uint32_t gt = __hgt2_mask(*reinterpret_cast<const __half2*>(&w[k]), zero2);
+                bits |= ((gt & 1u) | ((gt >> 15) & 2u)) << (2 * k);
+              }
+              bits <<= 8 * ep;
+              bits |= __shfl_xor_sync(0xffffffffu, bits, 16);
+              if (ok && ep == 0) p.bits_out[(obase + ocol) >> 4] = (uint16_t)bits;
+            }
           }
+          __syncwarp();                                       // the scratch is rewritten by the next pass
         }
       }
+      if (masked) release();
     }
   }
 }
@@ -747,7 +845,7 @@ template <int BN, int KH, bool DACT, bool U8 = false>
 static int launch_fwd(const CUtensorMap& tmX, const CUtensorMap& tmW, const ShiftParams& p, cudaStream_t st) {
   constexpr int STAGES = U8 ? SH_U8_STAGES : sh_stages(KH);
   constexpr int SMEM = (U8 ? U8Ring<SH_BM, STAGES>::BYTES : STAGES * KH * sh_arows(KH) * 128) + sh_wres_bytes(KH, U8) +
-                       1024 + SH_BAR_BYTES;
+                       1024 + SH_BAR_BYTES + STAGES * sh_mask_stage_bytes(BN, DACT) + SH_EPI_BYTES;
   static_assert(SMEM + 1024 <= 227 * 1024, "conv_shift_fwd: shared memory budget (+ static bias array)");
   static bool attr = false;
   auto kern = conv_shift_fwd_kernel<BN, KH, DACT, U8>;
@@ -872,12 +970,16 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
   B200RL_REQUIRE(fill_map(p.omap, omap), "conv_shift_fwd: output map needs power-of-two Cq >= 16 and s");
   p.bits_out = reinterpret_cast<uint16_t*>(bits_out);
   p.saved_bits = reinterpret_cast<const uint16_t*>(saved_bits);
-  if (smap) B200RL_REQUIRE(fill_map(p.smap, smap), "conv_shift_fwd: saved map needs power-of-two Cq >= 16 and s");
-  // the epilogue stores column pairs as 4-byte words and writes the activation bits per 16-column chunk
+  // the epilogue stores 8-column pieces as 16-byte words and writes the activation bits per 16-column chunk
   B200RL_REQUIRE(((omap[1] | omap[2] | omap[3]) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 31) == 0,
                  "conv_shift_fwd: output strides must be multiples of 16 elements, base 32-byte aligned");
+  // a tile's mask is staged with its A tile as one contiguous run: the saved activation must be row-contiguous on
+  // the output grid, N elements per grid row
   if (saved_bits)
-    B200RL_REQUIRE(((smap[1] | smap[2] | smap[3]) & 15) == 0, "conv_shift_fwd: saved strides must be multiples of 16");
+    B200RL_REQUIRE(smap[0] == 0 && smap[3] == N && smap[2] == (long long)Wg * N && smap[1] == (long long)Hg * Wg * N &&
+                       (reinterpret_cast<uintptr_t>(saved_bits) & 15) == 0,
+                   "conv_shift_fwd: saved_bits needs the row-contiguous map (0, Hg*Wg*N, Wg*N, N) and a 16-byte aligned "
+                   "base");
   p.bias = bias; p.act = act; p.dact = dact; p.alpha = alpha;
   p.num_tiles = (int)((p.M + SH_BM - 1) / SH_BM);
   p.u8 = make_u8src(u8_x, u8_idx, u8_H, u8_W, u8_C, u8_s);
