@@ -56,6 +56,10 @@ SIGNATURES = {
     "b200rl_dqn_act": [_p, _ll, _p, _ll, _i, _f, _ull, _ull, _p, _p, _p, _i, _p],
     "b200rl_lstm_seq_fwd": [_p, _ll, _p, _p, _p, _p, _p, _p, _p, _ll, _p, _p, _p, _i, _i, _i, _p],
     "b200rl_lstm_seq_bwd": [_p, _ll, _p, _p, _p, _p, _p, _p, _p, _p, _ll, _i, _i, _i, _p],
+    "b200rl_ln_fwd": [_p, _ll, _p, _p, _p, _ll, _ll, _i, _i, _f, _p],
+    "b200rl_ln_bwd": [_p, _ll, _p, _ll, _p, _p, _ll, _p, _p, _ll, _i, _f, _f, _p],
+    "b200rl_param_perturb": [_p, _p, _p, _i, _ll, _p, _p, _ull, _p, _p],
+    "b200rl_dqn_param_noise_adapt": [_p, _p, _ll, _i, _i, _i, _p, _p, _p, _p],
 }
 
 _lib = None

@@ -166,7 +166,8 @@ class PolicyNet:
         # parameters (checkpoint names / layouts unchanged); their fp16 forward operands, outputs and output gradients
         # are the two halves of shared buffers.
         tp, tv = self.tower_pi, self.tower_vf
-        self.fuse0 = bool(tv is not None and tp.kind == "mlp" and tp.fcs[0].N == tv.fcs[0].N and
+        # With layer_norm the first layers write fp32 pre-activations into their norms' workspaces and run apart.
+        self.fuse0 = bool(tv is not None and tp.kind == "mlp" and tp.lns[0] is None and tp.fcs[0].N == tv.fcs[0].N and
                           tp.fcs[0].K == tv.fcs[0].K and tp.fcs[0].act == tv.fcs[0].act and
                           2 * tp.fcs[0].N in (64, 128, 256))
         if self.fuse0:

@@ -81,6 +81,14 @@ int lstm_seq_fwd_impl(const float*, long long, const void*, const uint8_t*, cons
                       const long long*, float*, void*, long long, void*, float*, float*, int, int, int, cudaStream_t);
 int lstm_seq_bwd_impl(const void*, long long, const float*, const float*, const uint8_t*, const long long*,
                       const float*, const long long*, const void*, void*, long long, int, int, int, cudaStream_t);
+int ln_fwd_impl(const float*, long long, const float*, const float*, void*, long long, long long, int, int, float,
+                cudaStream_t);
+int ln_bwd_impl(const void*, long long, const float*, long long, const float*, void*, long long, float*, float*,
+                long long, int, float, float, cudaStream_t);
+int param_perturb_impl(const float*, float*, const void*, int, long long, const float*, const float*,
+                       unsigned long long, const unsigned long long*, cudaStream_t);
+int dqn_param_noise_adapt_impl(const float*, const float*, long long, int, int, int, float*, const float*, float*,
+                               cudaStream_t);
 
 }  // namespace b200rl
 
@@ -305,6 +313,28 @@ int b200rl_lstm_seq_bwd(const void* dh, long long lddh, const float* gates, cons
                         void* dz, long long lddz, int T, int B, int H, void* stream) {
   return lstm_seq_bwd_impl(dh, lddh, gates, c, masks, mask_idx, state_in, state_idx, whT, dz, lddz, T, B, H,
                            S(stream));
+}
+
+// tf.contrib.layers.layer_norm after a fully connected layer (common/models.py:97-98, deepq/models.py:24-25,34-35)
+int b200rl_ln_fwd(const float* z, long long ld_z, const float* gamma, const float* beta, void* y, long long ld_y,
+                  long long rows, int N, int act, float eps, void* stream) {
+  return ln_fwd_impl(z, ld_z, gamma, beta, y, ld_y, rows, N, act, eps, S(stream));
+}
+int b200rl_ln_bwd(const void* du, long long ld_du, const float* z, long long ld_z, const float* gamma, void* dz,
+                  long long ld_dz, float* dgamma, float* dbeta, long long rows, int N, float alpha, float eps,
+                  void* stream) {
+  return ln_bwd_impl(du, ld_du, z, ld_z, gamma, dz, ld_dz, dgamma, dbeta, rows, N, alpha, eps, S(stream));
+}
+
+// deepq/build_graph.py:258-287: perturb_vars, mean_kl and the scale adaptation of parameter-space noise
+int b200rl_param_perturb(const float* src, float* dst, const void* jobs, int njobs, long long max_len,
+                         const float* scale_dev, const float* normals, unsigned long long seed,
+                         const unsigned long long* offset_dev, void* stream) {
+  return param_perturb_impl(src, dst, jobs, njobs, max_len, scale_dev, normals, seed, offset_dev, S(stream));
+}
+int b200rl_dqn_param_noise_adapt(const float* q, const float* q_adapt, long long ld, int nA, int dueling, int B,
+                                 float* scale_dev, const float* threshold_dev, float* mean_kl_dev, void* stream) {
+  return dqn_param_noise_adapt_impl(q, q_adapt, ld, nA, dueling, B, scale_dev, threshold_dev, mean_kl_dev, S(stream));
 }
 
 }  // extern "C"

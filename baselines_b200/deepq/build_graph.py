@@ -22,13 +22,13 @@ def _fc_name(j):
 class QNet:
     """Trunk + (dueling) streams with workspaces for `cap` samples.  Variables are created in the order
     trunk, action_value stream, state_value stream with the same RandomState, so the oracle's
-    init_q_params(seed) reproduces them."""
+    init_q_params(seed) reproduces them.  layer_norm (deepq/models.py:5,24-25,34-35): a LayerNorm between every hidden
+    fully_connected of the streams and its ReLU; build_q_func consumes the argument, so the trunk never sees it."""
 
     def __init__(self, ob_shape, num_actions, network, cap, device, rng, scope="deepq/q_func", hiddens=(256,),
                  dueling=True, layer_norm=False, **network_kwargs):
-        if layer_norm:
-            raise NotImplementedError("layer_norm is outside the hot-path scope")
         self.device, self.cap, self.nA, self.dueling = device, cap, int(num_actions), bool(dueling)
+        self.scope = scope
         self.hiddens = tuple(hiddens)
         store = self.store = nn.ParamStore(device)
         kind = network
@@ -45,19 +45,22 @@ class QNet:
         else:
             raise ValueError(f"unknown network {kind!r}")
         L = self.trunk.latent_dim
-        self.streams = []
+        self.streams, self.stream_lns = [], []          # stream_lns[si][j]: the norm of hidden layer j, or None
         for sname, nout in [("action_value", self.nA)] + ([("state_value", 1)] if self.dueling else []):
-            layers, nin = [], L
+            layers, lns, nin = [], [], L
             for j, h in enumerate(self.hiddens):
                 layers.append(nn.Linear(store, f"{sname}/{j}", nin, h, "relu", nn.xavier_uniform((nin, h), rng),
                                         tf_w=f"{scope}/{sname}/{_fc_name(j)}/weights:0",
                                         tf_b=f"{scope}/{sname}/{_fc_name(j)}/biases:0"))
+                lns.append(nn.LayerNorm(store, f"{sname}/ln{j}", h, "relu", f"{scope}/{sname}/{nn.ln_scope(j)}", cap)
+                           if layer_norm else None)
                 nin = h
             j = len(self.hiddens)
             layers.append(nn.Linear(store, f"{sname}/{j}", nin, nout, None, nn.xavier_uniform((nin, nout), rng),
                                     tf_w=f"{scope}/{sname}/{_fc_name(j)}/weights:0",
                                     tf_b=f"{scope}/{sname}/{_fc_name(j)}/biases:0"))
             self.streams.append(layers)
+            self.stream_lns.append(lns)
         store.finalize()
         self._materialize()
         self.refresh()
@@ -67,8 +70,8 @@ class QNet:
         f16 = dict(dtype=torch.float16, device=dev)
         self.trunk.materialize()
         L = self.trunk.latent_dim
-        for layers in self.streams:
-            for l in layers:
+        for layers, lns in zip(self.streams, self.stream_lns):
+            for l in layers + [n for n in lns if n is not None]:
                 l.materialize()
         ns = len(self.streams)
         self.first_widths = [layers[0].N for layers in self.streams]
@@ -117,11 +120,18 @@ class QNet:
 
     def forward(self, obs, B, idx=None, out=None):
         """q head outputs for B samples: out[:, :nA] action scores, out[:, nA] state score (dueling)."""
+        self.trunk_forward(obs, B, idx)
+        return self.streams_forward(B, self.out if out is None else out)
+
+    def trunk_forward(self, obs, B, idx=None):
         x, src = self.encode(obs, idx)
-        lat, ldl = self.trunk.forward(x, B, src)
-        self._lat, self._ld_lat = lat, ldl
-        out = self.out if out is None else out
-        for si, layers in enumerate(self.streams):
+        self._lat, self._ld_lat = self.trunk.forward(x, B, src)
+
+    def streams_forward(self, B, out, streams=None):
+        """The streams over the latent trunk_forward left.  streams: the layers to run (default: this network's own; a
+        perturbed copy's for parameter-space noise, through the same workspaces and norms)."""
+        lat, ldl = self._lat, self._ld_lat
+        for si, layers in enumerate(self.streams if streams is None else streams):
             h, ldh = lat, ldl
             nl = len(layers)
             for j, l in enumerate(layers):
@@ -130,10 +140,10 @@ class QNet:
                     l.forward(h, ldh, B, out[:, col:], self.ld_out, mode=ops.MODE_F32_STORE)
                 elif j == 0:
                     dst = self.h_cat[:, self.cat_off[si]:]
-                    l.forward(h, ldh, B, dst, self.cat_w)
+                    nn.linear_ln_forward(l, self.stream_lns[si][j], h, ldh, B, dst, self.cat_w)
                     h, ldh = dst, self.cat_w
                 else:
-                    l.forward(h, ldh, B, self.hid[si][j - 1], l.Np)
+                    nn.linear_ln_forward(l, self.stream_lns[si][j], h, ldh, B, self.hid[si][j - 1], l.Np)
                     h, ldh = self.hid[si][j - 1], l.Np
         return out
 
@@ -147,6 +157,8 @@ class QNet:
             dz, lddz = self.dout[:, col:], self.ld_dout
             for j in reversed(range(nl)):
                 l = layers[j]
+                if j < nl - 1 and self.stream_lns[si][j] is not None:
+                    self.stream_lns[si][j].backward(B, dz, lddz, inv_B)
                 if j == 0:
                     xin, ldx = self._lat, self._ld_lat
                 elif j == 1:
@@ -171,11 +183,108 @@ class QNet:
         tr.backward(B, inv_B)
 
 
+class StreamCopy:
+    """A perturbed copy of a QNet's stream `fully_connected` variables (build_graph.py:254,277 `perturbed_q_func`,
+    `adaptive_q_func`): compact fp32 weights and biases, their fp16 forward operands and the head outputs.  Only these
+    variables differ from q_func (default_param_noise_filter :131-143), so the trunk, the norms and the workspaces are
+    q_func's."""
+
+    def __init__(self, q, scope):
+        import copy
+        self.scope, dev = scope, q.device
+        self.tf_names, self.jobs, off = {}, [], 0              # tf name -> (offset, shape); (src, dst, len, perturb)
+        by_internal = {v[0]: k for k, v in q.store.tf_map.items()}
+        for layers in q.streams:
+            for l in layers:
+                for part, shape in (("/w", (l.K, l.N)), ("/b", (l.N,))):
+                    n = int(np.prod(shape))
+                    self.jobs.append((q.store.offsets[l.name + part], off, n, 1))
+                    self.tf_names[by_internal[l.name + part].replace(q.scope, scope, 1)] = (off, shape)
+                    off += (n + 3) // 4 * 4
+        self.numel = off
+        self.params = torch.zeros(off, dtype=torch.float32, device=dev)
+        self.streams, k = [], 0
+        for layers in q.streams:
+            mine = []
+            for l in layers:
+                c = copy.copy(l)
+                (ow, sw), (ob, sb) = [(j[1], j[2]) for j in self.jobs[k:k + 2]]
+                k += 2
+                c.w, c.b = self.params[ow:ow + sw].view(l.K, l.N), self.params[ob:ob + sb]
+                c.w_fwd = torch.zeros(l.N, l.Kf, dtype=torch.float16, device=dev)
+                mine.append(c)
+            self.streams.append(mine)
+        self.out = torch.zeros_like(q.out)
+        self.cast = ops.CastPlan(self._cast_layers, dev)
+
+    def _cast_layers(self):
+        for layers in self.streams:
+            for c in layers:
+                ops.cast_transpose(c.w, c.K, c.N, None, 0, c.w_fwd, c.Kf)
+
+    def export_tf(self):
+        host = self.params.cpu().numpy()
+        return {k: host[o:o + int(np.prod(sh))].reshape(sh).copy() for k, (o, sh) in self.tf_names.items()}
+
+    def import_tf(self, values):
+        for k, (o, sh) in self.tf_names.items():
+            if k in values:
+                a = np.ascontiguousarray(values[k], dtype=np.float32).reshape(-1)
+                self.params[o:o + a.size].copy_(torch.from_numpy(a).to(self.params.device))
+        self.cast.run()
+
+
+class ParamNoise:
+    """State of parameter-space noise (build_graph.py:246-287): the perturbed and the adaptive stream copies, the noise
+    scale (0.01), the KL threshold (0.05) and the last mean_kl as float32 device scalars, and the Philox position."""
+
+    def __init__(self, q, seed):
+        dev = q.device
+        self.q, self.seed = q, int(seed)
+        self.perturbed = StreamCopy(q, "deepq/perturbed_q_func")
+        self.adaptive = StreamCopy(q, "deepq/adaptive_q_func")
+        jobs = self.perturbed.jobs
+        self.jobs = torch.tensor(jobs, dtype=torch.int64, device=dev)
+        self.njobs, self.max_len = len(jobs), max(j[2] for j in jobs)
+        self.scale = torch.full((1,), 0.01, dtype=torch.float32, device=dev)
+        self.threshold = torch.full((1,), 0.05, dtype=torch.float32, device=dev)
+        self.mean_kl = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.ctr = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.normals = None                      # tests: float32 [numel] noise used instead of the Philox stream
+        for c in (self.perturbed, self.adaptive):           # until the first reset a copy is q_func
+            for s, d, n, _ in jobs:
+                c.params[d:d + n].copy_(q.store.params[s:s + n])
+            c.cast.run()
+
+    def perturb(self, copy_):
+        """perturb_vars (:258-272): copy_ <- q_func + N(0, scale^2), then its fp16 operands (one launch each)."""
+        ops.param_perturb(self.q.store.params, copy_.params, self.jobs, self.njobs, self.max_len, self.scale, self.seed,
+                          self.ctr, normals=self.normals)
+        ops.counter_add(self.ctr, 1)
+        copy_.cast.run()
+
+    def export_tf(self):
+        d = {"deepq/param_noise_scale:0": np.float32(self.scale.item()),
+             "deepq/param_noise_threshold:0": np.float32(self.threshold.item())}
+        d.update(self.perturbed.export_tf())
+        d.update(self.adaptive.export_tf())
+        return d
+
+    def import_tf(self, d):
+        """Files written without these keys leave the state as it is."""
+        if "deepq/param_noise_scale:0" in d:
+            self.scale.fill_(float(d["deepq/param_noise_scale:0"]))
+        if "deepq/param_noise_threshold:0" in d:
+            self.threshold.fill_(float(d["deepq/param_noise_threshold:0"]))
+        self.perturbed.import_tf(d)
+        self.adaptive.import_tf(d)
+
+
 class DQNModel:
     """Online + target QNet, optimiser and the train step."""
 
     def __init__(self, ob_space, num_actions, network, lr, gamma=1.0, grad_norm_clipping=None, double_q=True,
-                 batch_cap=512, device=None, seed=None, adam_eps=1e-8, **network_kwargs):
+                 batch_cap=512, device=None, seed=None, adam_eps=1e-8, param_noise=False, **network_kwargs):
         if not torch.cuda.is_available():
             raise RuntimeError("baselines_b200.deepq needs a CUDA device: no CPU fallback on the hot path")
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
@@ -205,6 +314,8 @@ class DQNModel:
         self.batch_cap = batch_cap
         self.eps = 0.0
         self._seed = int(np.random.randint(0, 2 ** 31 - 1))
+        with torch.cuda.device(self.device):
+            self.pn = ParamNoise(self.q, self._seed) if param_noise else None
         self.update_target()
 
     def update_target(self):
@@ -232,6 +343,46 @@ class DQNModel:
                         eps_dev=self._eps_dev, step_dev=self._step_dev)
             ops.counter_add(self._step_dev, 1)
         self.graphs.run(("act", B), body)
+        return self._act[:B]
+
+    def act_device_param_noise(self, obs_dev, B, eps, reset, update_scale):
+        """build_graph.py:290-313 on B observations, in this order: (1) eps (and the threshold, by the caller) are set;
+        (2) reset: perturbed <- q_func + N(0, scale^2) with the scale as it is before this call's update; (3)
+        update_scale: adaptive <- q_func + N(0, scale^2), the streams of q_func and of the adaptive copy, mean_kl and the
+        scale update; (4) epsilon-greedy over the PERTURBED scores.  (The reference's graph leaves the order of (2) and
+        (3) to the TF runtime.)  One trunk forward serves all three networks; the sequence is captured per
+        (B, reset, update_scale)."""
+        pn, q = self.pn, self.q
+        if B > self.batch_cap:
+            raise ValueError(f"act batch {B} exceeds batch_cap {self.batch_cap}")
+        if self._act_obs is None or self._act_obs.shape[1:] != obs_dev.shape[1:] or self._act_obs.dtype != obs_dev.dtype:
+            self._act_obs = torch.zeros((self.batch_cap,) + tuple(obs_dev.shape[1:]), dtype=obs_dev.dtype,
+                                        device=self.device)
+            self.graphs.clear()
+        self._act_obs[:B].copy_(obs_dev)
+        ops.set_scalars(self._eps_dev, eps)
+        x = self._act_obs[:B]
+
+        def body():
+            q.trunk_forward(x, B)
+            if reset:
+                pn.perturb(pn.perturbed)
+            if update_scale:
+                pn.perturb(pn.adaptive)
+                q.streams_forward(B, q.out)
+                q.streams_forward(B, pn.adaptive.out, pn.adaptive.streams)
+                ops.dqn_param_noise_adapt(q.out, pn.adaptive.out, q.ld_out, self.nA, q.dueling, B, pn.scale,
+                                          pn.threshold, pn.mean_kl)
+            out = q.streams_forward(B, pn.perturbed.out, pn.perturbed.streams)
+            S = out[:, self.nA:] if q.dueling else None
+            ops.dqn_act(out, q.ld_out, S, q.ld_out, self.nA, 0.0, self._seed, 0, self._act, B,
+                        eps_dev=self._eps_dev, step_dev=self._step_dev)
+            ops.counter_add(self._step_dev, 1)
+        # injected noise (tests) is a different pointer set: keep it out of the captured sequences
+        if pn.normals is None:
+            self.graphs.run(("act_pn", B, bool(reset), bool(update_scale)), body)
+        else:
+            body()
         return self._act[:B]
 
     def q_values(self, obs):
@@ -286,7 +437,11 @@ class DQNModel:
 
 def build_act(model):
     """act(ob, stochastic=True, update_eps=-1) -> actions (build_graph.py:146-199 semantics: eps is sticky and is
-    updated when update_eps >= 0; stochastic=False gives the greedy action)."""
+    updated when update_eps >= 0; stochastic=False gives the greedy action).  A model built with param_noise=True gets
+    build_act_with_param_noise's act (:290-313) instead."""
+    if model.pn is not None:
+        return build_act_with_param_noise(model)
+
     def act(ob, stochastic=True, update_eps=-1):
         if update_eps >= 0:
             model.eps = float(update_eps)
@@ -298,16 +453,37 @@ def build_act(model):
     return act
 
 
+def build_act_with_param_noise(model):
+    """act(ob, reset=False, update_param_noise_threshold=False, update_param_noise_scale=False, stochastic=True,
+    update_eps=-1) with the reference's sticky values (build_graph.py:290-313): eps is replaced when update_eps >= 0,
+    the threshold when update_param_noise_threshold >= 0 -- so the default False (== 0.0) sets it to 0, as the
+    reference's givens do.  Actions are epsilon-greedy over the perturbed network (DQNModel.act_device_param_noise)."""
+    def act(ob, reset=False, update_param_noise_threshold=False, update_param_noise_scale=False, stochastic=True,
+            update_eps=-1):
+        if update_eps >= 0:
+            model.eps = float(update_eps)
+        with torch.cuda.device(model.device):
+            if update_param_noise_threshold >= 0:
+                ops.set_scalars(model.pn.threshold, float(update_param_noise_threshold))
+            x = torch.as_tensor(np.ascontiguousarray(ob)).to(model.device)
+            a = model.act_device_param_noise(x, x.shape[0], model.eps if stochastic else 0.0, bool(reset),
+                                             bool(update_param_noise_scale)).cpu().numpy()
+            model.q.trunk.check_obs_range()
+            return a
+    return act
+
+
 def build_train(make_obs_ph=None, q_func=None, num_actions=None, optimizer=None, grad_norm_clipping=None, gamma=1.0,
                 double_q=True, scope="deepq", reuse=None, param_noise=False, param_noise_filter_func=None, *,
                 ob_space=None, network="mlp", lr=5e-4, batch_cap=512, seed=None, **network_kwargs):
     """Same return value as the reference's build_train (build_graph.py:317-449):
     (act, train, update_target, debug).  `make_obs_ph` / `q_func` / `optimizer` are TF objects in the reference and
     are ignored here; the architecture comes from (ob_space, network, **network_kwargs)."""
-    if param_noise:
-        raise NotImplementedError("param_noise is outside the hot-path scope")
+    if param_noise_filter_func is not None:
+        raise NotImplementedError("param_noise_filter_func is a predicate over TF variables; the default filter "
+                                  "(the fully_connected variables, build_graph.py:131-143) is the one implemented")
     model = DQNModel(ob_space, num_actions, network, lr, gamma=gamma, grad_norm_clipping=grad_norm_clipping,
-                     double_q=double_q, batch_cap=batch_cap, seed=seed, **network_kwargs)
+                     double_q=double_q, batch_cap=batch_cap, seed=seed, param_noise=param_noise, **network_kwargs)
     act = build_act(model)
 
     def train(obs_t, action, reward, obs_tp1, done, weight):

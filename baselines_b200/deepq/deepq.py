@@ -48,6 +48,8 @@ class ActWrapper(object):
         d["beta1_power:0"] = np.float32(opt.beta1 ** (opt.t + 1))
         d["beta2_power:0"] = np.float32(opt.beta2 ** (opt.t + 1))
         d["b200rl/adam_t"] = np.int64(opt.t)
+        if self.model.pn is not None:                 # the noise scale / threshold and the perturbed copies are variables too
+            d.update(self.model.pn.export_tf())
         dirname = os.path.dirname(path)
         if dirname:
             os.makedirs(dirname, exist_ok=True)
@@ -66,6 +68,8 @@ class ActWrapper(object):
         opt.t = _adam_step_from_checkpoint(d, opt.beta1, opt.beta2, opt.t)
         self.model.q.refresh()
         self.model.qt.refresh()
+        if self.model.pn is not None:
+            self.model.pn.import_tf(d)
 
     def save_act(self, path=None):
         """deepq.py:55-72: pickle of (model data, act params)."""
@@ -98,18 +102,22 @@ def load_act(path):
     return ActWrapper.load_act(path)
 
 
+def param_noise_threshold(eps, num_actions):
+    """deepq.py:274: the KL between a greedy policy and its eps-greedy version (Plappert et al. 2017, appendix C.1)."""
+    return -np.log(1.0 - eps + eps / float(num_actions))
+
+
 def learn(env, network, seed=None, lr=5e-4, total_timesteps=100000, buffer_size=50000, exploration_fraction=0.1,
           exploration_final_eps=0.02, train_freq=1, batch_size=32, print_freq=100, checkpoint_freq=10000,
           checkpoint_path=None, learning_starts=1000, gamma=1.0, target_network_update_freq=500,
           prioritized_replay=False, prioritized_replay_alpha=0.6, prioritized_replay_beta0=0.4,
           prioritized_replay_beta_iters=None, prioritized_replay_eps=1e-6, param_noise=False, callback=None,
           load_path=None, **network_kwargs):
-    if param_noise:
-        raise NotImplementedError("param_noise is outside the hot-path scope")
     set_global_seeds(seed)                                                    # deepq.py:190
     num_actions = env.action_space.n
     act_params = dict(ob_space=env.observation_space, num_actions=num_actions, network=network, lr=lr, gamma=gamma,
-                      grad_norm_clipping=10, batch_cap=max(batch_size, 1), **network_kwargs)   # deepq.py:200-208
+                      grad_norm_clipping=10, batch_cap=max(batch_size, 1), param_noise=param_noise,
+                      **network_kwargs)                                       # deepq.py:200-208
     model = DQNModel(**act_params)
     act = ActWrapper(build_act(model), act_params, model)
 
@@ -128,6 +136,7 @@ def learn(env, network, seed=None, lr=5e-4, total_timesteps=100000, buffer_size=
     episode_rewards = [0.0]
     saved_mean_reward = None
     obs = env.reset()
+    reset = True
     with tempfile.TemporaryDirectory() as td:
         td = checkpoint_path or td
         model_file = os.path.join(td, "model")
@@ -144,8 +153,17 @@ def learn(env, network, seed=None, lr=5e-4, total_timesteps=100000, buffer_size=
             if callback is not None:
                 if callback(locals(), globals()):
                     break
-            update_eps = exploration.value(t)
-            action = act(np.array(obs)[None], update_eps=update_eps)[0]
+            kwargs = {}
+            if not param_noise:
+                update_eps = exploration.value(t)
+            else:
+                # deepq.py:268-277: no epsilon; the KL threshold that makes the perturbed policy as far from the plain
+                # one as eps-greedy with eps = exploration.value(t) would be
+                update_eps = 0.0
+                kwargs = dict(reset=reset, update_param_noise_scale=True,
+                              update_param_noise_threshold=param_noise_threshold(exploration.value(t), num_actions))
+            action = act(np.array(obs)[None], update_eps=update_eps, **kwargs)[0]
+            reset = False
             new_obs, rew, done, _ = env.step(action)
             replay_buffer.add(obs, action, rew, new_obs, float(done))       # deepq.py:283
             obs = new_obs
@@ -153,6 +171,7 @@ def learn(env, network, seed=None, lr=5e-4, total_timesteps=100000, buffer_size=
             if done:
                 obs = env.reset()
                 episode_rewards.append(0.0)
+                reset = True
 
             if t > learning_starts and t % train_freq == 0:                   # deepq.py:292-303
                 rb = replay_buffer

@@ -208,6 +208,52 @@ class Linear:
                      ld_saved=ld_saved, mode=ops.MODE_F16_DACT, act=act, tag="dgrad." + self.name, remap=remap)
 
 
+LN_EPS = 1e-12      # variance_epsilon of tf.contrib.layers.layer_norm (tf.nn.batch_normalization inside it)
+
+
+def ln_scope(k):
+    """Name tf.contrib.layers.layer_norm gives its k-th use inside one variable scope."""
+    return "LayerNorm" if k == 0 else f"LayerNorm_{k}"
+
+
+class LayerNorm:
+    """y = act(gamma * (z - mean) / sqrt(var + LN_EPS) + beta) over each row of a layer's fp32 pre-activation z
+    (tf.contrib.layers.layer_norm(center=True, scale=True), common/models.py:97-98, deepq/models.py:24-25).  Variables
+    beta (zeros) then gamma (ones), [N] each, `<tf_scope>/{beta,gamma}:0`; neither draws from the RNG.  They stay fp32:
+    the operand refresh has nothing to cast."""
+
+    def __init__(self, store, name, N, act, tf_scope, cap):
+        self.store, self.name, self.N, self.act, self.cap = store, name, N, ops.ACT_CODES[act], cap
+        store.add(name + "/beta", np.zeros(N, np.float32))
+        store.add(name + "/gamma", np.ones(N, np.float32))
+        store.map_tf(f"{tf_scope}/beta:0", name + "/beta", (N,))
+        store.map_tf(f"{tf_scope}/gamma:0", name + "/gamma", (N,))
+
+    def materialize(self):
+        v, g = self.store.views, self.store.gviews
+        self.beta, self.gamma = v[self.name + "/beta"], v[self.name + "/gamma"]
+        self.gbeta, self.ggamma = g[self.name + "/beta"], g[self.name + "/gamma"]
+        # the layer's pre-activation: written by its GEMM (MODE_F32_STORE), read again by the backward
+        self.z = torch.empty(self.cap, _pad8(self.N), dtype=torch.float32, device=self.store.device)
+        self.ldz = _pad8(self.N)
+
+    def forward(self, M, y, ldy):
+        ops.ln_fwd(self.z, self.ldz, self.gamma, self.beta, y, ldy, M, self.N, self.act, LN_EPS)
+
+    def backward(self, M, du, lddu, alpha):
+        """du: d loss / d (gamma * xhat + beta), replaced in place by d loss / d z; the norm's gradients accumulate."""
+        ops.ln_bwd(du, lddu, self.z, self.ldz, self.gamma, du, lddu, self.ggamma, self.gbeta, M, self.N, alpha, LN_EPS)
+
+
+def linear_ln_forward(l, ln, x, ldx, M, out, ldo):
+    """out = l's activation of x: act(x W + b), or with a norm act(LN(x W + b)) through the norm's fp32 workspace."""
+    if ln is None:
+        l.forward(x, ldx, M, out, ldo)
+    else:
+        l.forward(x, ldx, M, ln.z, ln.ldz, mode=ops.MODE_F32_STORE, act=ops.ACT_NONE)
+        ln.forward(M, out, ldo)
+
+
 class Conv(Linear):
     """NHWC convolution lowered to im2col + wgmma GEMM (a2c/utils.py:37-56)."""
 
@@ -471,13 +517,15 @@ class Tower:
         """kind: cnn, conv_only, mlp, or the recurrent lstm (the observation encoding of mlp, then an LSTM; models.py
         lstm) and cnn_lstm (cnn, then an LSTM; models.py cnn_lstm).  The recurrent towers' forward and backward take
         the rows as sequences (Seq)."""
-        if layer_norm:
-            raise NotImplementedError("layer-normalised LSTMs (lnlstm, cnn_lnlstm) are not implemented")
+        if layer_norm and kind != "mlp":
+            raise NotImplementedError("layer_norm is an argument of 'mlp' (common/models.py:75); layer-normalised LSTMs "
+                                      "(lnlstm, cnn_lnlstm) are not implemented")
         self.kind, self.cap, self.store = kind, cap, store
         self.base = {"lstm": "mlp", "cnn_lstm": "cnn"}.get(kind, kind)      # the tower below the LSTM
         if kind == "lstm":
             num_layers = 0                              # models.py lstm: flatten(X) straight into the cell
         self.convs, self.fcs = [], []
+        self.lns = []                                   # per fc layer: its LayerNorm or None
         self.lstm = None
         winit = (lambda shape, scale: ortho_init(shape, scale, rng)) if init == "ortho" else \
                 (lambda shape, scale: xavier_uniform(shape, rng))
@@ -527,11 +575,15 @@ class Tower:
                                        winit((nin, num_hidden), math.sqrt(2)),
                                        tf_w=f"{tf_prefix}/mlp_fc{i}/w:0", tf_b=f"{tf_prefix}/mlp_fc{i}/b:0",
                                        split_in=(i == 0)))
+                if layer_norm:                                                # models.py:97-98
+                    self.lns.append(LayerNorm(store, f"{prefix}/mlp_ln{i}", num_hidden, "tanh",
+                                              f"{tf_prefix}/{ln_scope(i)}", cap))
                 nin = num_hidden
             self.latent_dim, self.latent_act = nin, ops.ACT_TANH
         else:
             raise ValueError(f"unknown network type {kind!r} (supported: cnn, conv_only, mlp, lstm, cnn_lstm)")
         self.layers = self.convs + self.fcs
+        self.lns = self.lns or [None] * len(self.fcs)
         if kind in ("lstm", "cnn_lstm"):
             # utils.py:89-91: wx and wh take ortho_init(1.0) after the layers below them (it fixes the RNG stream)
             self.lstm = LSTM(store, prefix, tf_prefix, self.latent_dim, nlstm,
@@ -547,7 +599,7 @@ class Tower:
     def _materialize_layers(self):
         dev, cap = self.store.device, self.cap
         f16 = dict(dtype=torch.float16, device=dev)
-        for l in self.layers:
+        for l in self.layers + [n for n in self.lns if n is not None]:
             l.materialize()
         if self.convs and self.shift_mode:
             self._materialize_shift(f16)
@@ -726,14 +778,15 @@ class Tower:
             self._mlp_in = h
         for i, l in enumerate(self.fcs):
             if not (skip_first and i == 0):
-                l.forward(h, ldh, B, self.hfc[i], self.ld_hfc[i])
+                linear_ln_forward(l, self.lns[i], h, ldh, B, self.hfc[i], self.ld_hfc[i])
             h, ldh = self.hfc[i], self.ld_hfc[i]
         if self.lstm is not None:
             assert seq is not None and seq.T * seq.B == B, "recurrent towers take their rows as sequences"
             h, ldh = self.lstm.forward(h, ldh, seq, train=masks)
         return h, ldh                                    # latent [B, latent_dim] fp16, row pitch ldh
 
-    # consumes self.dlatent: fp16 [B, ld_dlatent] gradient w.r.t. the latent PRE-activation
+    # consumes self.dlatent: fp16 [B, ld_dlatent] gradient w.r.t. the latent PRE-activation (with a norm: w.r.t. the
+    # normalised, scaled and shifted value the activation reads)
     def backward(self, B, alpha, skip_first_wgrad=False):
         """skip_first_wgrad (mlp): the caller computes the first layer's weight gradient (fused over two towers)."""
         nfc = len(self.fcs)
@@ -748,6 +801,8 @@ class Tower:
             dz, lddz = self.dzfc[-1], self.ld_hfc[-1]
         for i in reversed(range(nfc)):
             l = self.fcs[i]
+            if self.lns[i] is not None:
+                self.lns[i].backward(B, dz, lddz, alpha)
             if i == 0 and skip_first_wgrad and not self.convs:
                 return
             if i > 0:

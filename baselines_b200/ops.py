@@ -503,3 +503,44 @@ def lstm_seq_bwd(dh, lddh, gates, c, masks, state_in, whT, dz, lddz, T, B, H, *,
               _ptr(state_in), _ptr(state_idx), _ptr(whT), _ptr(dz), int(lddz), int(T), int(B), int(H), _stream(),
               label="lstm_seq_bwd", flops=8.0 * rows * H * H,
               nbytes=2.0 * rows * H + 16.0 * rows * H + 8.0 * rows * H + 8.0 * rows * H + 8.0 * H * H * -(-B // 8))
+
+
+def ln_fwd(z, ld_z, gamma, beta, y, ld_y, rows, N, act, eps):
+    """y fp16 = act(gamma * (z - mean) / sqrt(var + eps) + beta) per row of z float32 [rows, ld_z] (biased variance)."""
+    for t, dt, nm in ((z, torch.float32, "z"), (gamma, torch.float32, "gamma"), (beta, torch.float32, "beta"),
+                      (y, torch.float16, "y")):
+        _chk(t, dt, nm)
+    _lib.call("b200rl_ln_fwd", _ptr(z), int(ld_z), _ptr(gamma), _ptr(beta), _ptr(y), int(ld_y), int(rows), int(N),
+              int(act), float(eps), _stream(), label="ln_fwd", nbytes=6.0 * rows * N)
+
+
+def ln_bwd(du, ld_du, z, ld_z, gamma, dz, ld_dz, dgamma, dbeta, rows, N, alpha, eps):
+    """Backward of ln_fwd from du fp16 = d loss / d (gamma * xhat + beta): dz fp16 (may be du), dgamma += alpha *
+    sum_r du * xhat, dbeta += alpha * sum_r du (deterministic)."""
+    for t, dt, nm in ((du, torch.float16, "du"), (z, torch.float32, "z"), (gamma, torch.float32, "gamma"),
+                      (dz, torch.float16, "dz"), (dgamma, torch.float32, "dgamma"), (dbeta, torch.float32, "dbeta")):
+        _chk(t, dt, nm)
+    _lib.call("b200rl_ln_bwd", _ptr(du), int(ld_du), _ptr(z), int(ld_z), _ptr(gamma), _ptr(dz), int(ld_dz),
+              _ptr(dgamma), _ptr(dbeta), int(rows), int(N), float(alpha), float(eps), _stream(), label="ln_bwd",
+              nbytes=8.0 * rows * N)
+
+
+def param_perturb(src, dst, jobs, njobs, max_len, scale_dev, seed, offset_dev, normals=None):
+    """dst <- src (+ scale_dev[0] * N(0, 1) on the jobs marked perturb) per record {src_off, dst_off, len, perturb} of
+    the int64 device table `jobs`; the noise is the Philox stream at *offset_dev, or `normals` (indexed like dst)."""
+    for t, dt, nm in ((src, torch.float32, "src"), (dst, torch.float32, "dst"), (jobs, torch.int64, "jobs"),
+                      (scale_dev, torch.float32, "scale_dev"), (normals, torch.float32, "normals"),
+                      (offset_dev, torch.int64, "offset_dev")):
+        _chk(t, dt, nm)
+    _lib.call("b200rl_param_perturb", _ptr(src), _ptr(dst), _ptr(jobs), int(njobs), int(max_len), _ptr(scale_dev),
+              _ptr(normals), int(seed), _ptr(offset_dev), _stream(), label="param_perturb")
+
+
+def dqn_param_noise_adapt(q, q_adapt, ld, nA, dueling, B, scale_dev, threshold_dev, mean_kl_dev):
+    """mean_kl_dev[0] = mean KL(softmax(Q) || softmax(Q_adapt)) over B rows; scale_dev[0] *= or /= 1.01 against the
+    threshold (build_graph.py:279-287)."""
+    for t, nm in ((q, "q"), (q_adapt, "q_adapt"), (scale_dev, "scale_dev"), (threshold_dev, "threshold_dev"),
+                  (mean_kl_dev, "mean_kl_dev")):
+        _chk(t, torch.float32, nm)
+    _lib.call("b200rl_dqn_param_noise_adapt", _ptr(q), _ptr(q_adapt), int(ld), int(nA), int(bool(dueling)), int(B),
+              _ptr(scale_dev), _ptr(threshold_dev), _ptr(mean_kl_dev), _stream(), label="dqn_param_noise_adapt")

@@ -257,6 +257,34 @@ int b200rl_lstm_seq_bwd(const void* dh, long long lddh, const float* gates, cons
                         const long long* mask_idx, const float* state_in, const long long* state_idx, const void* whT,
                         void* dz, long long lddz, int T, int B, int H, void* stream);
 
+/* Row layer normalisation after a fully connected layer (tf.contrib.layers.layer_norm(center=True, scale=True):
+ * common/models.py:97-98, deepq/models.py:24-25,34-35), csrc/layer_norm.cu.  N a multiple of 8 in [8, 1024]; row
+ * pitches multiples of 8 elements; act 0 none, 1 relu, 2 tanh.
+ * fwd: y fp16 [rows, ld_y] = act(gamma * (z - mean) / sqrt(var + eps) + beta) of z fp32 [rows, ld_z] (the
+ * pre-activation a MODE_F32_STORE GEMM wrote), mean and biased variance per row.  A row's output depends on the row
+ * alone.
+ * bwd: du fp16 = d loss / d (gamma * xhat + beta); dz fp16 = d loss / d z (may be du's buffer);
+ * dgamma += alpha * sum_r du * xhat, dbeta += alpha * sum_r du, summed over fixed 128-row slices in row order and
+ * then over the slices in order.  The statistics are recomputed from z. */
+int b200rl_ln_fwd(const float* z, long long ld_z, const float* gamma, const float* beta, void* y, long long ld_y,
+                  long long rows, int N, int act, float eps, void* stream);
+int b200rl_ln_bwd(const void* du, long long ld_du, const float* z, long long ld_z, const float* gamma, void* dz,
+                  long long ld_dz, float* dgamma, float* dbeta, long long rows, int N, float alpha, float eps,
+                  void* stream);
+
+/* DQN parameter-space noise (deepq/build_graph.py:202-314), csrc/param_noise.cu.
+ * param_perturb: for each of njobs device records {src_off, dst_off, len, perturb} (4 x int64; max_len = the largest
+ * len): dst[dst_off + i] = src[src_off + i] + (perturb ? scale_dev[0] * n : 0), float32, n ~ N(0, 1) by Box-Muller over
+ * the Philox4x32-10 stream (seed, position *offset_dev), or normals[dst_off + i] when normals is given.
+ * dqn_param_noise_adapt: q, q_adapt = head outputs [B, ld] ([A | S] when dueling) of the plain and the adaptively
+ * perturbed network; mean_kl_dev[0] = mean_b KL(softmax(Q_b) || softmax(Q_adapt_b)), summed in a fixed order, then
+ * scale_dev[0] <- mean_kl < threshold_dev[0] ? scale * 1.01f : scale / 1.01f (:281-287).  One CTA. */
+int b200rl_param_perturb(const float* src, float* dst, const void* jobs, int njobs, long long max_len,
+                         const float* scale_dev, const float* normals, unsigned long long seed,
+                         const unsigned long long* offset_dev, void* stream);
+int b200rl_dqn_param_noise_adapt(const float* q, const float* q_adapt, long long ld, int nA, int dueling, int B,
+                                 float* scale_dev, const float* threshold_dev, float* mean_kl_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
