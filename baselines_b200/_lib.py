@@ -60,6 +60,11 @@ SIGNATURES = {
     "b200rl_ln_bwd": [_p, _ll, _p, _ll, _p, _p, _ll, _p, _p, _ll, _i, _f, _f, _p],
     "b200rl_param_perturb": [_p, _p, _p, _i, _ll, _p, _p, _ull, _p, _p],
     "b200rl_dqn_param_noise_adapt": [_p, _p, _ll, _i, _i, _i, _p, _p, _p, _p],
+    "b200rl_vecnorm_moments": [_p, _i, _ll, _i, _p, _p],
+    "b200rl_vecnorm_combine": [_p, _p, _i, _ll, _i, _d, _p],
+    "b200rl_vecnorm_normalize": [_p, _i, _ll, _i, _p, _d, _p, _p],
+    "b200rl_vecnorm_rewards": [_p, _i, _p, _ll, _p, _p, _d, _d, _d, _p, _p],
+    "b200rl_vecnorm_add_latency": [_i, _ll, _p, _p],
 }
 
 _lib = None

@@ -269,35 +269,175 @@ class VecFrameStack(VecEnvWrapper):
 class VecNormalize(VecEnvWrapper):
     """vec_normalize.py:4-49: running normalisation of observations and of rewards (by the std of the discounted
     return), both clipped.  Host numpy, float64 statistics (the reference's use_tf=True variant only changes where
-    the three statistics are stored)."""
+    the three statistics are stored).
+
+    reset()/step_wait() are the reference's host implementation.  The device Runner does not call them: it sees
+    `normalize_device`, pulls the RAW batches with reset_raw()/step_raw() (or, over a device env, the HBM tensors of
+    reset_raw_device()/step_raw_device()) and applies the same update, bit for bit, with the b200rl_vecnorm kernels
+    (dev_reset / dev_step).  From then on the statistics and `ret` live on the device; `ob_rms`, `ret_rms` and `ret`
+    read them back when accessed (and what is assigned through them is uploaded before the next device step), and a
+    host reset()/step_wait() continues from the device state."""
+    normalize_device = True
 
     def __init__(self, venv, ob=True, ret=True, clipob=10., cliprew=10., gamma=0.99, epsilon=1e-8, use_tf=False):
         super().__init__(venv)
         from .running_mean_std import RunningMeanStd
-        self.ob_rms = RunningMeanStd(shape=self.observation_space.shape) if ob else None
-        self.ret_rms = RunningMeanStd(shape=()) if ret else None
+        self._ob_rms = RunningMeanStd(shape=self.observation_space.shape) if ob else None
+        self._ret_rms = RunningMeanStd(shape=()) if ret else None
         self.clipob, self.cliprew, self.gamma, self.epsilon = clipob, cliprew, gamma, epsilon
-        self.ret = np.zeros(self.num_envs)
+        self._ret = np.zeros(self.num_envs)
+        self._dev = None                 # _VecNormDevice once a device Runner has stepped through this wrapper
+        self._on_device = False          # the device copy is the current state (the host copy is stale)
 
+    # ---- the statistics, wherever they currently live
+    @property
+    def ob_rms(self):
+        self._pull()
+        return self._ob_rms
+
+    @ob_rms.setter
+    def ob_rms(self, v):
+        self._pull()
+        self._ob_rms = v
+
+    @property
+    def ret_rms(self):
+        self._pull()
+        return self._ret_rms
+
+    @ret_rms.setter
+    def ret_rms(self, v):
+        self._pull()
+        self._ret_rms = v
+
+    @property
+    def ret(self):
+        self._pull()
+        return self._ret
+
+    @ret.setter
+    def ret(self, v):
+        self._pull()
+        self._ret = np.asarray(v, dtype=np.float64)
+
+    def _pull(self):
+        """Make the host copy current (device -> host) and the host its owner."""
+        if self._on_device:
+            self._dev.download(self)
+            self._on_device = False
+
+    def _push(self, device):
+        """Make the device copy current (host -> device) and the device its owner."""
+        if self._dev is None or not self._dev.fits(self, device):
+            self._pull()
+            self._dev = _VecNormDevice(self, device)
+        if not self._on_device:
+            self._dev.upload(self)
+            self._on_device = True
+        return self._dev
+
+    # ---- host implementation
     def _obfilt(self, obs):
-        if self.ob_rms is None:
+        if self._ob_rms is None:
             return obs
-        self.ob_rms.update(obs)
-        return np.clip((obs - self.ob_rms.mean) / np.sqrt(self.ob_rms.var + self.epsilon), -self.clipob, self.clipob)
+        self._ob_rms.update(obs)
+        return np.clip((obs - self._ob_rms.mean) / np.sqrt(self._ob_rms.var + self.epsilon), -self.clipob, self.clipob)
 
     def step_wait(self):
         obs, rews, news, infos = self.venv.step_wait()
-        self.ret = self.ret * self.gamma + rews
+        self._pull()
+        self._ret = self._ret * self.gamma + rews
         obs = self._obfilt(obs)
-        if self.ret_rms is not None:
-            self.ret_rms.update(self.ret)
-            rews = np.clip(rews / np.sqrt(self.ret_rms.var + self.epsilon), -self.cliprew, self.cliprew)
-        self.ret[np.asarray(news, dtype=np.bool_)] = 0.
+        if self._ret_rms is not None:
+            self._ret_rms.update(self._ret)
+            rews = np.clip(rews / np.sqrt(self._ret_rms.var + self.epsilon), -self.cliprew, self.cliprew)
+        self._ret[np.asarray(news, dtype=np.bool_)] = 0.
         return obs, rews, news, infos
 
     def reset(self):
-        self.ret = np.zeros(self.num_envs)
+        self._pull()
+        self._ret = np.zeros(self.num_envs)
         return self._obfilt(self.venv.reset())
+
+    # ---- raw access and the device implementation (ppo2 Runner)
+    def reset_raw(self):
+        return self.venv.reset()
+
+    def step_raw(self, actions):
+        """(raw obs, raw rews, news, infos): the wrapped env's step; normalisation is left to the caller."""
+        self.venv.step_async(actions)
+        return self.venv.step_wait()
+
+    def reset_raw_device(self):
+        return self.venv.reset_device()
+
+    def step_raw_device(self, actions):
+        return self.venv.step_device(actions)
+
+    def dev_reset(self, obs, out):
+        """reset() on the device: ret = 0, out float32 [N, D] = the filtered observations obs [N, ...] (float32 or
+        float64 CUDA tensor), ob_rms updated."""
+        dev = self._push(obs.device)
+        dev.ret.zero_()
+        self._dev_obfilt(dev, obs, out)
+
+    def dev_step(self, obs, rews, news, obs_out, rew_out):
+        """step_wait() on the device from the raw step: obs [N, ...] and rews [N] (float32 or float64), news uint8 [N];
+        writes the float32 observations [N, D] and rewards [N] the Runner stores."""
+        from .. import ops
+        dev = self._push(obs.device)
+        ops.vecnorm_rewards(rews, news, dev.ret, dev.rt, self.gamma, self.epsilon, self.cliprew, rew_out)
+        self._dev_obfilt(dev, obs, obs_out)
+
+    def _dev_obfilt(self, dev, obs, out):
+        from .. import ops
+        if dev.ob is not None:
+            ops.vecnorm_moments(obs, dev.ws)
+            ops.vecnorm_combine(dev.ob, dev.ws, obs.shape[0], self.epsilon, obs.dtype == torch.float32)
+        ops.vecnorm_normalize(obs, dev.ob, self.clipob, out)
+
+
+class _VecNormDevice:
+    """Device copy of VecNormalize's state: float64 [mean(D) | var(D) | std(D) | count] per RunningMeanStd (the
+    layout of the b200rl_vecnorm kernels), ret [N], and the batch-moment workspace."""
+
+    def __init__(self, vn, device):
+        self.device = device
+        f64 = dict(dtype=torch.float64, device=device)
+        D = int(np.prod(vn.observation_space.shape))
+        self.ob = torch.zeros(3 * D + 1, **f64) if vn._ob_rms is not None else None
+        self.rt = torch.zeros(4, **f64) if vn._ret_rms is not None else None
+        self.ret = torch.zeros(vn.num_envs, **f64)
+        self.ws = torch.zeros(2 * D, **f64)
+
+    def fits(self, vn, device):
+        return self.device == device and (self.ob is None) == (vn._ob_rms is None) and \
+            (self.rt is None) == (vn._ret_rms is None) and self.ret.numel() == np.size(vn._ret)
+
+    @staticmethod
+    def _pack(rms, eps):
+        mean = np.asarray(rms.mean, np.float64).ravel()
+        var = np.asarray(rms.var, np.float64).ravel()
+        return np.concatenate([mean, var, np.sqrt(var + eps), [np.float64(rms.count)]])
+
+    def upload(self, vn):
+        if self.ob is not None:
+            self.ob.copy_(torch.from_numpy(self._pack(vn._ob_rms, vn.epsilon)))
+        if self.rt is not None:
+            self.rt.copy_(torch.from_numpy(self._pack(vn._ret_rms, vn.epsilon)))
+        self.ret.copy_(torch.from_numpy(np.ascontiguousarray(vn._ret, dtype=np.float64)))
+
+    def download(self, vn):
+        for t, rms in ((self.ob, vn._ob_rms), (self.rt, vn._ret_rms)):
+            if t is None:
+                continue
+            a = t.cpu().numpy()
+            shape = np.shape(rms.mean)
+            n = int(np.prod(shape))
+            rms.mean = a[:n].reshape(shape).copy()
+            rms.var = a[n:2 * n].reshape(shape).copy()
+            rms.count = np.float64(a[3 * n])
+        vn._ret = self.ret.cpu().numpy().copy()
 
 
 class VecMonitor(VecEnvWrapper):

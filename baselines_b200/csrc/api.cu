@@ -89,6 +89,12 @@ int param_perturb_impl(const float*, float*, const void*, int, long long, const 
                        unsigned long long, const unsigned long long*, cudaStream_t);
 int dqn_param_noise_adapt_impl(const float*, const float*, long long, int, int, int, float*, const float*, float*,
                                cudaStream_t);
+int vecnorm_moments_impl(const void*, int, long long, int, double*, cudaStream_t);
+int vecnorm_combine_impl(double*, const double*, int, long long, int, double, cudaStream_t);
+int vecnorm_normalize_impl(const void*, int, long long, int, const double*, double, float*, cudaStream_t);
+int vecnorm_rewards_impl(const void*, int, const uint8_t*, long long, double*, double*, double, double, double, float*,
+                         cudaStream_t);
+int vecnorm_add_latency_impl(int, long long, double*, cudaStream_t);
 
 }  // namespace b200rl
 
@@ -335,6 +341,25 @@ int b200rl_param_perturb(const float* src, float* dst, const void* jobs, int njo
 int b200rl_dqn_param_noise_adapt(const float* q, const float* q_adapt, long long ld, int nA, int dueling, int B,
                                  float* scale_dev, const float* threshold_dev, float* mean_kl_dev, void* stream) {
   return dqn_param_noise_adapt_impl(q, q_adapt, ld, nA, dueling, B, scale_dev, threshold_dev, mean_kl_dev, S(stream));
+}
+
+// common/vec_env/vec_normalize.py:26-47 VecNormalize with running_mean_std.py:22-33 RunningMeanStd
+int b200rl_vecnorm_moments(const void* x, int x_f64, long long N, int D, double* ws, void* stream) {
+  return vecnorm_moments_impl(x, x_f64, N, D, ws, S(stream));
+}
+int b200rl_vecnorm_combine(double* rms, const double* ws, int ws_f32, long long N, int D, double eps, void* stream) {
+  return vecnorm_combine_impl(rms, ws, ws_f32, N, D, eps, S(stream));
+}
+int b200rl_vecnorm_normalize(const void* x, int x_f64, long long N, int D, const double* rms, double clip, float* out,
+                             void* stream) {
+  return vecnorm_normalize_impl(x, x_f64, N, D, rms, clip, out, S(stream));
+}
+int b200rl_vecnorm_rewards(const void* rew, int rew_f64, const uint8_t* news, long long N, double* ret, double* rms,
+                           double gamma, double eps, double cliprew, float* out, void* stream) {
+  return vecnorm_rewards_impl(rew, rew_f64, news, N, ret, rms, gamma, eps, cliprew, out, S(stream));
+}
+int b200rl_vecnorm_add_latency(int f64, long long n, double* out, void* stream) {
+  return vecnorm_add_latency_impl(f64, n, out, S(stream));
 }
 
 }  // extern "C"

@@ -544,3 +544,77 @@ def dqn_param_noise_adapt(q, q_adapt, ld, nA, dueling, B, scale_dev, threshold_d
         _chk(t, torch.float32, nm)
     _lib.call("b200rl_dqn_param_noise_adapt", _ptr(q), _ptr(q_adapt), int(ld), int(nA), int(bool(dueling)), int(B),
               _ptr(scale_dev), _ptr(threshold_dev), _ptr(mean_kl_dev), _stream(), label="dqn_param_noise_adapt")
+
+
+_VN_DTYPES = {torch.float32: 0, torch.float64: 1}
+
+
+def _vn_dtype(t, name):
+    if not t.is_cuda:
+        raise RuntimeError(f"{name}: expected a CUDA tensor (the hot path has no CPU fallback)")
+    if t.dtype not in _VN_DTYPES:
+        raise RuntimeError(f"{name}: expected float32 or float64, got {t.dtype}")
+    if not t.is_contiguous():
+        raise RuntimeError(f"{name}: expected a contiguous tensor")
+    return _VN_DTYPES[t.dtype]
+
+
+def vecnorm_moments(x, ws):
+    """ws float64 [2D] = (np.mean(x, 0), np.var(x, 0)) of x [N, ...] float32 / float64, in numpy's summation order."""
+    f64 = _vn_dtype(x, "x")
+    _chk(ws, torch.float64, "ws")
+    N, D = x.shape[0], x[0].numel()
+    if ws.numel() < 2 * D:
+        raise RuntimeError("vecnorm_moments: ws needs 2 * D elements")
+    _lib.call("b200rl_vecnorm_moments", _ptr(x), f64, int(N), int(D), _ptr(ws), _stream(),
+              label="vecnorm_moments." + ("col" if D > 1 else "pairwise"), flops=4.0 * N * D,
+              nbytes=2.0 * x.numel() * x.element_size())
+
+
+def vecnorm_combine(rms, ws, N, eps, ws_f32):
+    """rms float64 [3D + 1] = (mean, var, std, count) updated with the batch moments ws of N rows (ws_f32: the batch
+    was float32, so bvar * N is a float32 product as in numpy)."""
+    _chk(rms, torch.float64, "rms")
+    _chk(ws, torch.float64, "ws")
+    D = (rms.numel() - 1) // 3
+    if rms.numel() != 3 * D + 1 or ws.numel() < 2 * D:
+        raise RuntimeError("vecnorm_combine: rms must hold 3 * D + 1 and ws 2 * D elements")
+    _lib.call("b200rl_vecnorm_combine", _ptr(rms), _ptr(ws), int(bool(ws_f32)), int(N), int(D), float(eps), _stream(),
+              label="vecnorm_combine", nbytes=56.0 * D)
+
+
+def vecnorm_normalize(x, rms, clip, out):
+    """out float32 [N, D] = clip((x - mean) / std, +-clip) in float64 (rms None: out = float32(x))."""
+    f64 = _vn_dtype(x, "x")
+    _chk(rms, torch.float64, "rms")
+    _chk(out, torch.float32, "out")
+    N, D = x.shape[0], x[0].numel()
+    if out.numel() != N * D or not out.is_contiguous():
+        raise RuntimeError("vecnorm_normalize: out must be contiguous with N * D elements")
+    if rms is not None and rms.numel() != 3 * D + 1:
+        raise RuntimeError("vecnorm_normalize: rms must hold 3 * D + 1 elements")
+    _lib.call("b200rl_vecnorm_normalize", _ptr(x), f64, int(N), int(D), _ptr(rms), float(clip), _ptr(out), _stream(),
+              label="vecnorm_normalize", nbytes=float(x.numel() * (x.element_size() + 4)))
+
+
+def vecnorm_rewards(rew, news, ret, rms, gamma, eps, cliprew, out):
+    """ret = ret * gamma + rew; with rms (float64 [4]): update it with ret's moments and out = clip(rew / std);
+    without: out = float32(rew); then ret = 0 where news (uint8 [N] or None)."""
+    f64 = _vn_dtype(rew, "rew")
+    _chk(news, torch.uint8, "news")
+    _chk(ret, torch.float64, "ret")
+    _chk(rms, torch.float64, "rms")
+    _chk(out, torch.float32, "out")
+    N = rew.numel()
+    if ret.numel() != N or out.numel() != N or (news is not None and news.numel() != N) or \
+            (rms is not None and rms.numel() != 4):
+        raise RuntimeError("vecnorm_rewards: shape mismatch")
+    _lib.call("b200rl_vecnorm_rewards", _ptr(rew), f64, _ptr(news), int(N), _ptr(ret), _ptr(rms), float(gamma),
+              float(eps), float(cliprew), _ptr(out), _stream(), label="vecnorm_rewards",
+              nbytes=float(N * (rew.element_size() + 1 + 24 + 4)))
+
+
+def vecnorm_add_latency(f64, n, out):
+    """out float64 [2]: out[0] = SM cycles per dependent add (float64 if f64), over n adds in one thread."""
+    _chk(out, torch.float64, "out")
+    _lib.call("b200rl_vecnorm_add_latency", int(bool(f64)), int(n), _ptr(out), _stream(), label="vecnorm_add_latency")

@@ -113,11 +113,27 @@ class Runner:
         self._obs_src = None
         # VecFrameStack on the device: only the new frames cross PCIe, the stack lives in the rollout buffer
         # (only when VecFrameStack is the OUTERMOST wrapper: step_frames() would bypass anything wrapped around it)
-        from ..common.vec_env import VecFrameStack
+        from ..common.vec_env import VecFrameStack, VecNormalize
         self.fs = isinstance(env, VecFrameStack) and bool(env.frame_stack_device) and self.u8 and \
             not self.device_env and pin
+        # VecNormalize on the device (likewise only when OUTERMOST): the raw float observations and rewards are
+        # normalised by the b200rl_vecnorm kernels straight into the rollout buffer, the statistics stay in HBM
+        self.vn = isinstance(env, VecNormalize) and bool(env.normalize_device) and not self.u8 and \
+            not getattr(net.tower_pi, "onehot_n", 0) and np_dtype in (np.float32, np.float64) and pin
+        self.vn_dev_env = self.vn and hasattr(env.venv, "step_device") and not isinstance(env.venv, VecEnvWrapper)
         if self.device_env:
             self._dev_obs = env.reset_device()
+        elif self.vn:
+            self._vn_obs = torch.zeros(tuple(self._obs_pin.shape), dtype=self._obs_pin.dtype, device=self.device)
+            self._vn_rew = {}                                # reward dtype -> (pinned staging, device buffer)
+            self._news_pin = torch.zeros(nenv, dtype=torch.uint8).pin_memory()
+            self._news_dev = torch.zeros(nenv, dtype=torch.uint8, device=self.device)
+            with torch.cuda.device(self.device):
+                if self.vn_dev_env:
+                    env.dev_reset(env.reset_raw_device(), self._cur)
+                else:
+                    self._vn_stage(env.reset_raw())
+                    env.dev_reset(self._vn_obs, self._cur)
         elif self.fs:
             c = env.frame_channels
             fshape = (nenv,) + tuple(ob_space.shape[:-1]) + (c,)
@@ -149,11 +165,17 @@ class Runner:
             self._state_dev = torch.from_numpy(np.ascontiguousarray(st, dtype=np.float32)).to(self.device)
             self._mask_dev = torch.zeros(nenv, dtype=torch.uint8, device=self.device)
 
+    @property
+    def _dev_steps(self):
+        """The env is stepped on the device (no per-step host synchronisation): a device env, bare or under the
+        device VecNormalize."""
+        return self.device_env or self.vn_dev_env
+
     def _rnn(self):
         """step_device / value_device keywords of a recurrent policy: the state and this step's mask."""
         if not self.recurrent:
             return {}
-        if self.device_env:
+        if self._dev_steps:
             self._mask_dev.copy_(self._dev_dones)
         else:
             self._mask_dev.copy_(torch.from_numpy(self.dones.astype(np.uint8)))
@@ -170,6 +192,31 @@ class Runner:
             self._obs_src = None
             self.obs = self._obs_pin.numpy()
             self.obs[:] = obs
+
+    def _vn_stage(self, obs, rews=None, news=None):
+        """Raw host step -> device buffers through pinned staging (the obs directly when the env already hands out
+        pinned memory of the right dtype); returns the device rewards (float32, or float64 for any other dtype)."""
+        t = torch.from_numpy(obs) if isinstance(obs, np.ndarray) and obs.flags.c_contiguous else None
+        if t is not None and t.dtype == self._obs_pin.dtype and t.shape == self._obs_pin.shape and t.is_pinned():
+            src = t
+        else:
+            self._obs_pin.numpy()[...] = np.asarray(obs).reshape(self._obs_pin.shape)
+            src = self._obs_pin
+        self._vn_obs.copy_(src, non_blocking=True)
+        if rews is None:
+            return None
+        rews = np.asarray(rews)
+        rdt = np.float32 if rews.dtype == np.float32 else np.float64
+        if rdt not in self._vn_rew:
+            tdt = torch.float32 if rdt == np.float32 else torch.float64
+            self._vn_rew[rdt] = (torch.zeros(self.nenv, dtype=tdt).pin_memory(),
+                                 torch.zeros(self.nenv, dtype=tdt, device=self.device))
+        pin, dev = self._vn_rew[rdt]
+        pin.numpy()[...] = rews.reshape(self.nenv)
+        dev.copy_(pin, non_blocking=True)
+        self._news_pin.numpy()[...] = np.asarray(news, dtype=np.uint8).reshape(self.nenv)
+        self._news_dev.copy_(self._news_pin, non_blocking=True)
+        return dev
 
     def _stack_frames(self, frames, news, prev, out):
         """out = VecFrameStack.step_wait update (vec_frame_stack.py:17-25) of the stacked observation `prev` with
@@ -243,7 +290,7 @@ class Runner:
                 flag = int(self._over_pin[0])
                 self._over_pin.zero_()
                 model.net.check_obs_range(flag)
-            if self.fs:
+            if self.fs or self.vn:
                 ro.obs[0].copy_(self._cur)
             if self.recurrent:
                 ro.states0.copy_(self._state_dev)                              # runner.py:31 mb_states = self.states
@@ -251,12 +298,18 @@ class Runner:
             chunked = self.fs and self.act_chunks > 1 and nz is None and not self.recurrent
             acted = False                      # step t's policy pass already issued (chunk-wise, with the upload)
             for t in range(T):
-                if not self.fs:
+                if not (self.fs or self.vn):
                     self._upload_obs(ro.obs[t])
                 if not acted:
                     model.step_device(ro.obs[t], ro.actions[t], ro.values[t], ro.neglogpacs[t],
                                       noise=None if nz is None else nz[t], persistent=True, **self._rnn())
                 acted = False
+                nxt = ro.obs[t + 1] if t + 1 < T else self._cur
+                if self.vn_dev_env:
+                    ro.dones[t].copy_(self._dev_dones)
+                    obs, rew, self._dev_dones = self.env.step_raw_device(ro.actions[t])
+                    self.env.dev_step(obs, rew, self._dev_dones, nxt, ro.rewards[t])
+                    continue
                 if self.device_env:
                     ro.dones[t].copy_(self._dev_dones)
                     self._dev_obs, rew, self._dev_dones = self.env.step_device(ro.actions[t])
@@ -280,6 +333,11 @@ class Runner:
                         acted = True
                     else:
                         self._stack_frames(frames, self.dones, ro.obs[t], ro.obs[t + 1] if t + 1 < T else self._cur)
+                elif self.vn:
+                    obs, rewards, self.dones, infos = self.env.step_raw(actions)
+                    self.dones = np.asarray(self.dones, dtype=np.bool_)
+                    rew_dev = self._vn_stage(obs, rewards, self.dones)
+                    self.env.dev_step(self._vn_obs, rew_dev, self._news_dev, nxt, ro.rewards[t])
                 else:
                     obs, rewards, self.dones, infos = self.env.step(actions)             # runner.py:38
                     self._take_obs(obs)
@@ -288,18 +346,20 @@ class Runner:
                     maybeepinfo = info.get('episode') if info else None
                     if maybeepinfo:
                         epinfos.append(maybeepinfo)
-                self._rew_host[t] = torch.from_numpy(np.asarray(rewards, dtype=np.float32))
+                if not self.vn:                  # the device VecNormalize has written ro.rewards[t] already
+                    self._rew_host[t] = torch.from_numpy(np.asarray(rewards, dtype=np.float32))
             # bootstrap value of the final observation (runner.py:50)
-            if not self.fs:
+            if not (self.fs or self.vn):
                 self._upload_obs(self._cur)
             model.value_device(self._cur, ro.last_values, persistent=True, **self._rnn())   # runner.py:50
-            if self.device_env:
+            if self._dev_steps:
                 ro.last_dones.copy_(self._dev_dones)
                 if not self.u8:
                     self._over_pin.copy_(model.net.tower_pi.obs_overflow, non_blocking=True)
                     self._over_ev.record()
             else:
-                ro.rewards.copy_(self._rew_host, non_blocking=True)
+                if not self.vn:
+                    ro.rewards.copy_(self._rew_host, non_blocking=True)
                 ro.dones.copy_(self._done_host, non_blocking=True)
                 self._ro_copied.record()
                 ro.last_dones.copy_(torch.from_numpy(self.dones.astype(np.uint8)))

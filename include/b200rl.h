@@ -285,6 +285,29 @@ int b200rl_param_perturb(const float* src, float* dst, const void* jobs, int njo
 int b200rl_dqn_param_noise_adapt(const float* q, const float* q_adapt, long long ld, int nA, int dueling, int B,
                                  float* scale_dev, const float* threshold_dev, float* mean_kl_dev, void* stream);
 
+/* VecNormalize (common/vec_env/vec_normalize.py:26-47) with RunningMeanStd (common/running_mean_std.py:22-33) on the
+ * device, bit for bit with the numpy wrapper.  Running statistics: float64 [mean(D) | var(D) | std(D) | count],
+ * std = sqrt(var + eps) written by every update.  Batch moments: float64 workspace [mean(D) | var(D)].
+ * x: [N, D] rows of float32 (x_f64 = 0) or float64 (x_f64 = 1).
+ * moments: np.mean / np.var of x along axis 0 in x's dtype -- column-sequential sums for D >= 2, numpy's pairwise sum
+ *   for D == 1 (N <= 131072).
+ * combine: the Chan update of rms with ws over a batch of N rows (running_mean_std.py:23-31), in float64 except
+ *   bvar * N, which is a float32 product when the batch was float32 (ws_f32 = 1), as in numpy.
+ * normalize: out f32 [N, D] = float32(clip((x - mean) / std, +-clip)) in float64, NaN kept (vec_normalize.py:43-47);
+ *   rms == NULL: out = float32(x).
+ * rewards: ret = ret * gamma + rew (float64 [N]); with rms (D = 1): update it with the pairwise moments of ret and
+ *   out = float32(clip(rew / std, +-cliprew)), without: out = float32(rew); then ret = 0 where news[e] (news may be
+ *   NULL).  rew: float32 (rew_f64 = 0) or float64 [N]; N <= 131072. */
+int b200rl_vecnorm_moments(const void* x, int x_f64, long long N, int D, double* ws, void* stream);
+int b200rl_vecnorm_combine(double* rms, const double* ws, int ws_f32, long long N, int D, double eps, void* stream);
+int b200rl_vecnorm_normalize(const void* x, int x_f64, long long N, int D, const double* rms, double clip, float* out,
+                             void* stream);
+int b200rl_vecnorm_rewards(const void* rew, int rew_f64, const uint8_t* news, long long N, double* ret, double* rms,
+                           double gamma, double eps, double cliprew, float* out, void* stream);
+/* Latency probe for the moments' chain bound: one thread runs n dependent float32 (f64 = 0) / float64 adds;
+ * out[0] = SM cycles per add.  out[1] seeds the chain (and receives its end). */
+int b200rl_vecnorm_add_latency(int f64, long long n, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
