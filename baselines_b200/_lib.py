@@ -5,67 +5,38 @@ the product path never routes through the CPU oracle or plain PyTorch ops.
 """
 import ctypes as C
 import os
+import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200rl.so")
+HEADER = os.path.join(_HERE, "..", "include", "b200rl.h")
 
-_p, _i, _ll, _f, _d, _ull = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_double, C.c_ulonglong
+# C parameter type -> ctypes type; every pointer passes as c_void_p
+_CTYPES = {"int": C.c_int, "long long": C.c_longlong, "unsigned long long": C.c_ulonglong, "float": C.c_float,
+           "double": C.c_double}
 
-# name -> argtypes (all return int); must mirror include/b200rl.h exactly (checked by tests/test_cabi.py)
-SIGNATURES = {
-    "b200rl_gae_scan": [_p, _p, _p, _p, _p, _p, _p, _i, _i, _d, _d, _i, _p],
-    "b200rl_gemm_f16": [_p, _p, _p, _p, _p, _i, _i, _i, _ll, _ll, _ll, _ll, _i, _i, _i, _f, _i, _i, _i, _i, _i, _p, _p],
-    "b200rl_conv_shift_fwd": [_p, _ll, _i, _i, _i, _p, _ll, _i, _i, _p, _i, _i, _p, _p, _p, _p, _i, _i, _f,
-                              _p, _p, _i, _i, _i, _i, _p, _p, _p],
-    "b200rl_conv_shift_wgrad": [_p, _ll, _i, _p, _i, _i, _p, _p, _ll, _f, _p, _f, _i, _p, _p, _i, _i, _i, _i, _i, _p],
-    "b200rl_conv_gemm": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _p, _ll, _p, _p, _ll, _i, _i, _i,
-                         _i, _f, _i, _i, _i, _i, _i, _p],
-    "b200rl_dgrad_weights": [_p, _p, _i, _i, _i, _i, _i, _ll, _p],
-    "b200rl_im2col": [_p, _i, _p, _p, _ll, _i, _i, _i, _i, _i, _i, _p],
-    "b200rl_s2d_gather": [_p, _p, _p, _ll, _i, _i, _i, _i, _p],
-    "b200rl_frame_stack": [_p, _p, _p, _p, _ll, _ll, _i, _i, _p],
-    "b200rl_col2im": [_p, _p, _p, _ll, _i, _i, _i, _i, _i, _i, _i, _p],
-    "b200rl_colsum": [_p, _p, _ll, _i, _ll, _f, _p],
-    "b200rl_cat_step": [_p, _ll, _i, _p, _i, _p, _ll, _p, _ull, _ull, _p, _p, _p, _p, _ll, _p],
-    "b200rl_bern_step": [_p, _ll, _i, _p, _ll, _p, _ull, _ull, _p, _p, _p, _p, _ll, _p],
-    "b200rl_gauss_step": [_p, _ll, _p, _i, _p, _ll, _p, _ull, _ull, _p, _p, _p, _p, _ll, _p],
-    "b200rl_set_scalars": [_p, _i, _f, _f, _f, _f, _p],
-    "b200rl_shuffle_indices": [_p, _ll, _ull, _ll, _ll, _p],
-    "b200rl_counter_add": [_p, _ull, _p],
-    "b200rl_adv_stats": [_p, _p, _p, _ll, _p, _p],
-    "b200rl_cat_loss": [_p, _ll, _i, _p, _i, _p, _ll, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _ll, _p, _ll, _p, _ll, _p,
-                        _p],
-    "b200rl_bern_loss": [_p, _ll, _i, _p, _ll, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _ll, _p, _ll, _p, _ll, _p, _p],
-    "b200rl_gauss_loss": [_p, _ll, _p, _i, _p, _ll, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _ll, _p, _ll, _p, _f,
-                          _p, _ll, _p, _p],
-    "b200rl_sumsq": [_p, _ll, _p, _p],
-    "b200rl_seg_sumsq": [_p, _p, _i, _p, _p],
-    "b200rl_clip_adam": [_p, _p, _p, _p, _ll, _f, _f, _f, _f, _f, _p, _p, _i, _p, _p],
-    "b200rl_clip_accumulate": [_p, _p, _ll, _f, _f, _p, _p],
-    "b200rl_cast_transpose": [_p, _i, _i, _p, _ll, _p, _ll, _f, _p],
-    "b200rl_cast_transpose_batch": [_p, _i, _i, _i, _p],
-    "b200rl_cast_f32_f16": [_p, _p, _ll, _i, _ll, _ll, _f, _p],
-    "b200rl_obs_encode": [_p, _p, _ll, _i, _i, _i, _p, _p, _f, _f, _i, _p, _i, _p, _p, _p],
-    "b200rl_tree_set": [_p, _p, _ll, _p, _p, _i, _p],
-    "b200rl_tree_range_sum": [_p, _ll, _ll, _ll, _p, _p],
-    "b200rl_per_sample": [_p, _p, _ll, _ll, _p, _i, _d, _p, _p, _p, _p, _p],
-    "b200rl_per_priorities": [_p, _i, _d, _d, _p, _p, _p, _p],
-    "b200rl_per_pow": [_p, _i, _d, _p, _p],
-    "b200rl_dqn_td": [_p, _ll, _p, _ll, _p, _ll, _p, _ll, _p, _ll, _p, _ll, _i, _p, _p, _p, _p, _p, _f, _i, _p, _p,
-                      _ll, _p, _ll, _p, _i, _p],
-    "b200rl_dqn_act": [_p, _ll, _p, _ll, _i, _f, _ull, _ull, _p, _p, _p, _i, _p],
-    "b200rl_lstm_seq_fwd": [_p, _ll, _p, _p, _p, _p, _p, _p, _p, _ll, _p, _p, _p, _i, _i, _i, _p],
-    "b200rl_lstm_seq_bwd": [_p, _ll, _p, _p, _p, _p, _p, _p, _p, _p, _ll, _i, _i, _i, _p],
-    "b200rl_ln_fwd": [_p, _ll, _p, _p, _p, _ll, _ll, _i, _i, _f, _p],
-    "b200rl_ln_bwd": [_p, _ll, _p, _ll, _p, _p, _ll, _p, _p, _ll, _i, _f, _f, _p],
-    "b200rl_param_perturb": [_p, _p, _p, _i, _ll, _p, _p, _ull, _p, _p],
-    "b200rl_dqn_param_noise_adapt": [_p, _p, _ll, _i, _i, _i, _p, _p, _p, _p],
-    "b200rl_vecnorm_moments": [_p, _i, _ll, _i, _p, _p],
-    "b200rl_vecnorm_combine": [_p, _p, _i, _ll, _i, _d, _p],
-    "b200rl_vecnorm_normalize": [_p, _i, _ll, _i, _p, _d, _p, _p],
-    "b200rl_vecnorm_rewards": [_p, _i, _p, _ll, _p, _p, _d, _d, _d, _p, _p],
-    "b200rl_vecnorm_add_latency": [_i, _ll, _p, _p],
-}
+
+def _ctype(param):
+    """ctypes type of one C parameter declaration ("const float* x", "long long ld", ...); raises on a type without
+    a mapping rather than guess one."""
+    if "*" in param:
+        return C.c_void_p
+    typ = " ".join(param.split()[:-1])
+    if typ not in _CTYPES:
+        raise ValueError(f"include/b200rl.h: no ctypes mapping for parameter {param!r}")
+    return _CTYPES[typ]
+
+
+def _signatures():
+    """name -> argtypes of every entry point the header declares, except the two argument-less ones load() binds."""
+    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    decls = re.findall(r"\b(?:int|const char\*)\s+(b200rl_\w+)\s*\(([^;]*?)\)\s*;", src, flags=re.S)
+    return {name: [_ctype(a.strip()) for a in args.split(",")] for name, args in decls
+            if name not in ("b200rl_last_error", "b200rl_version")}
+
+
+# all entry points return int; parsed once per process
+SIGNATURES = _signatures()
 
 _lib = None
 

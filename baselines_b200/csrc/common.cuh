@@ -5,11 +5,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#define B200RL_OK 0
-#define B200RL_ERR_ARG (-1)
-#define B200RL_ERR_CUDA (-2)
-#define B200RL_ERR_UNSUPPORTED (-3)
-#define B200RL_ERR_DRIVER (-4)
+// The entry points are defined extern "C" against these prototypes: a definition whose parameter types differ from
+// the header's is a compile error, not a second overload.
+#include "../../include/b200rl.h"
 
 namespace b200rl {
 

@@ -184,7 +184,7 @@ s2d_gather_kernel(const uint8_t* __restrict__ x, const long long* __restrict__ s
   }
 }
 
-// part[block, c] = alpha * sum over the block's rows of dz[row, c]  (colsum_impl adds the blocks' parts in order)
+// part[block, c] = alpha * sum over the block's rows of dz[row, c]  (b200rl_colsum adds the blocks' parts in order)
 __global__ void __launch_bounds__(256)
 colsum_kernel(const __half* __restrict__ dz, float* __restrict__ part, long long rows, int C, long long ld, float alpha,
               int rows_per_block) {
@@ -270,28 +270,6 @@ static int fill_geom(ConvGeom& g, int H, int W, int C, int rf, int stride, int s
   return (g.OH > 0 && g.OW > 0) ? 0 : -1;
 }
 
-int im2col_impl(const void* x, int src_is_u8, const long long* src_idx, void* cols, long long B, int H, int W, int C,
-                int rf, int stride, int same_pad, cudaStream_t stream) {
-  B200RL_REQUIRE(x && cols && B > 0, "im2col: bad args");
-  ConvGeom g;
-  B200RL_REQUIRE(fill_geom(g, H, W, C, rf, stride, same_pad) == 0, "im2col: empty output");
-  B200RL_REQUIRE((rf * C) % 8 == 0, "im2col: rf*C must be a multiple of 8 (got %d)", rf * C);
-  if (src_is_u8)
-    B200RL_REQUIRE((stride * C) % 8 == 0 && (W * C) % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 7) == 0,
-                   "im2col(u8): stride*C and W*C must be multiples of 8");
-  else
-    B200RL_REQUIRE(C % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0, "im2col(f16): C must be a multiple of 8");
-  const long long total = B * g.OH * g.OW * rf * ((rf * C) / 8);
-  const int grid = grid_for(total, 256);
-  if (src_is_u8)
-    im2col_kernel<uint8_t><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(x), src_idx,
-                                                     reinterpret_cast<__half*>(cols), B, g);
-  else
-    im2col_kernel<__half><<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(x), src_idx,
-                                                    reinterpret_cast<__half*>(cols), B, g);
-  return check_launch("im2col_kernel");
-}
-
 // ------------------------------------------------------------------------------------------------ frame stack
 // Device half of VecFrameStack (reference common/vec_env/vec_frame_stack.py:17-25): out = roll(prev, -1, axis=-1)
 // (ONE channel, the reference's literal shift: a whole frame only when c == 1); out[news] = 0; out[..., -c:] = frame.
@@ -333,8 +311,36 @@ frame_stack_generic_kernel(const uint8_t* __restrict__ prev, const uint8_t* __re
   }
 }
 
-int frame_stack_impl(const void* prev, const void* frame, const void* news, void* out, long long N, long long pixels,
-                     int nstack, int c, cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_im2col(const void* x, int src_is_u8, const long long* src_idx, void* cols, long long B, int H,
+                             int W, int C, int rf, int stride, int same_pad, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200RL_REQUIRE(x && cols && B > 0, "im2col: bad args");
+  ConvGeom g;
+  B200RL_REQUIRE(fill_geom(g, H, W, C, rf, stride, same_pad) == 0, "im2col: empty output");
+  B200RL_REQUIRE((rf * C) % 8 == 0, "im2col: rf*C must be a multiple of 8 (got %d)", rf * C);
+  if (src_is_u8)
+    B200RL_REQUIRE((stride * C) % 8 == 0 && (W * C) % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 7) == 0,
+                   "im2col(u8): stride*C and W*C must be multiples of 8");
+  else
+    B200RL_REQUIRE(C % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0, "im2col(f16): C must be a multiple of 8");
+  const long long total = B * g.OH * g.OW * rf * ((rf * C) / 8);
+  const int grid = grid_for(total, 256);
+  if (src_is_u8)
+    im2col_kernel<uint8_t><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(x), src_idx,
+                                                     reinterpret_cast<__half*>(cols), B, g);
+  else
+    im2col_kernel<__half><<<grid, 256, 0, stream>>>(reinterpret_cast<const __half*>(x), src_idx,
+                                                    reinterpret_cast<__half*>(cols), B, g);
+  return check_launch("im2col_kernel");
+}
+
+extern "C" int b200rl_frame_stack(const void* prev, const void* frame, const void* news, void* out, long long N,
+                                  long long pixels, int nstack, int c, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(prev && frame && news && out && N > 0 && pixels > 0 && nstack >= 1 && c >= 1, "frame_stack: bad args");
   B200RL_REQUIRE(prev != out, "frame_stack: in-place update is not supported (pixels are shifted across threads' words)");
   const long long total = N * pixels;
@@ -367,8 +373,9 @@ int frame_stack_impl(const void* prev, const void* frame, const void* news, void
   return check_launch("frame_stack_kernel");
 }
 
-int s2d_gather_impl(const void* x, const long long* src_idx, void* out, long long B, int H, int W, int C, int s,
-                    cudaStream_t stream) {
+extern "C" int b200rl_s2d_gather(const void* x, const long long* src_idx, void* out, long long B, int H, int W, int C,
+                                 int s, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(x && out && B > 0 && s > 0, "s2d_gather: bad args");
   B200RL_REQUIRE(H % s == 0 && W % s == 0 && (s * C) % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 7) == 0 &&
                      (W * C) % 8 == 0,
@@ -385,8 +392,9 @@ int s2d_gather_impl(const void* x, const long long* src_idx, void* out, long lon
   return check_launch("s2d_gather_kernel");
 }
 
-int col2im_impl(const void* dcols, const void* saved, void* dx, long long B, int H, int W, int C, int rf, int stride,
-                int same_pad, int act, cudaStream_t stream) {
+extern "C" int b200rl_col2im(const void* dcols, const void* saved, void* dx, long long B, int H, int W, int C, int rf,
+                             int stride, int same_pad, int act, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(dcols && dx && B > 0, "col2im: bad args");
   ConvGeom g;
   B200RL_REQUIRE(fill_geom(g, H, W, C, rf, stride, same_pad) == 0, "col2im: empty output");
@@ -398,7 +406,9 @@ int col2im_impl(const void* dcols, const void* saved, void* dx, long long B, int
   return check_launch("col2im_kernel");
 }
 
-int colsum_impl(const void* dz, float* db, long long rows, int C, long long ld, float alpha, cudaStream_t stream) {
+extern "C" int b200rl_colsum(const void* dz, float* db, long long rows, int C, long long ld, float alpha,
+                             void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(dz && db && rows > 0 && C > 0, "colsum: bad args");
   long long rpb = (rows + (long long)device_num_sms() * 8 - 1) / ((long long)device_num_sms() * 8);
   if (rpb < 64) rpb = 64;
@@ -416,5 +426,3 @@ int colsum_impl(const void* dz, float* db, long long rows, int C, long long ld, 
   if (rc == B200RL_OK) rc = sum_partials(part, grid, 1, C, db, C, stream);
   return rc;
 }
-
-}  // namespace b200rl

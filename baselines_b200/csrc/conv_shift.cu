@@ -939,13 +939,18 @@ static bool fill_map(AddrMap& a, const long long* m) {       // {mode, sN, sY, s
   return true;
 }
 
+}  // namespace b200rl
+
+using namespace b200rl;
+
 // X: [B*Hg*Wg, C] fp16 (C = 64 or 128, row pitch C); W: [N, taps*C] fp16 (row pitch ldw), K order (tap, channel);
 // shifts[taps]: absolute row shifts (all >= 0 for forward, all <= 0 for the data gradient).
-int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const void* W, long long ldw, int N,
-                        int taps, const int* shifts, int vy, int vx, void* out, const long long* omap,
-                        const long long* smap, const float* bias, int act, int dact, float alpha,
-                        const void* u8_x, const long long* u8_idx, int u8_H, int u8_W, int u8_C, int u8_s,
-                        void* bits_out, const void* saved_bits, cudaStream_t stream) {
+extern "C" int b200rl_conv_shift_fwd(const void* X, long long B, int Hg, int Wg, int C, const void* W, long long ldw,
+                                     int N, int taps, const int* shifts, int vy, int vx, void* out,
+                                     const long long* omap, const long long* smap, const float* bias, int act, int dact,
+                                     float alpha, const void* u8_x, const long long* u8_idx, int u8_H, int u8_W,
+                                     int u8_C, int u8_s, void* bits_out, const void* saved_bits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE((X || u8_x) && W && out && omap && B > 0, "conv_shift_fwd: null operand");
   B200RL_REQUIRE(!(bits_out && dact) && !(saved_bits && !(dact && smap)), "conv_shift_fwd: bits_out is a forward output, saved_bits a dact input (with smap)");
   if (u8_x) {
@@ -1009,10 +1014,11 @@ int conv_shift_fwd_impl(const void* X, long long B, int Hg, int Wg, int C, const
 }
 
 // G[taps*C, N] (fp32, row pitch ldg) += alpha * sum_m X[m + shift_t, c] * dY[m, n]
-int conv_shift_wgrad_impl(const void* X, long long rows, int C, const void* dY, int N, int taps, const int* shifts,
-                          float* G, long long ldg, float alpha, float* gbias, float alpha_b, int max_ctas,
-                          const void* u8_x, const long long* u8_idx, int u8_H, int u8_W, int u8_C, int u8_s,
-                          int kx, cudaStream_t stream) {
+extern "C" int b200rl_conv_shift_wgrad(const void* X, long long rows, int C, const void* dY, int N, int taps,
+                                       const int* shifts, float* G, long long ldg, float alpha, float* gbias,
+                                       float alpha_b, int max_ctas, const void* u8_x, const long long* u8_idx, int u8_H,
+                                       int u8_W, int u8_C, int u8_s, int kx, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE((X || u8_x) && dY && G && rows > 0, "conv_shift_wgrad: null operand");
   if (kx < 1) kx = 1;
   B200RL_REQUIRE(kx <= 3, "conv_shift_wgrad: kx must be 1..3");
@@ -1061,5 +1067,3 @@ int conv_shift_wgrad_impl(const void* X, long long rows, int C, const void* dY, 
   if (rc == B200RL_OK && gbias) rc = sum_partials(p.ws_b, (int)grid.x, 1, N, gbias, N, stream);
   return rc;
 }
-
-}  // namespace b200rl

@@ -181,9 +181,14 @@ static int make_tmap_tn(CUtensorMap* tm, const void* ptr, int T, int N, int elem
   return B200RL_OK;
 }
 
-int gae_scan_impl(const float* rew, const float* val, const uint8_t* done, const float* last_val,
-                  const uint8_t* last_done, float* adv, float* ret, int T, int N, double gamma, double lam,
-                  int variant, cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_gae_scan(const float* rew, const float* val, const uint8_t* done, const float* last_val,
+                               const uint8_t* last_done, float* adv, float* ret, int T, int N, double gamma, double lam,
+                               int variant, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(rew && val && done && last_val && last_done && adv && ret, "gae: null pointer");
   B200RL_REQUIRE(T > 0 && N > 0, "gae: bad shape T=%d N=%d", T, N);
   const float gamma_f = (float)gamma;
@@ -206,5 +211,3 @@ int gae_scan_impl(const float* rew, const float* val, const uint8_t* done, const
                                                                        T, N, gamma_f, gl);
   return check_launch("gae_direct_kernel");
 }
-
-}  // namespace b200rl

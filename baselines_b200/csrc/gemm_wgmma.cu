@@ -570,11 +570,44 @@ static int gemm_dispatch(int BN, int mn_major, int mode, const CUtensorMap& tmA,
 #undef GEMM_KMAJOR
 }
 
-// C-ABI body (declared in include/b200rl.h)
-int gemm_f16_impl(const void* A, const void* B, void* C, const float* bias, const void* saved, int M, int N, int K,
-                  long long lda, long long ldb, long long ldc, long long ld_saved, int mn_major, int mode, int act,
-                  float alpha, int split_k, int max_ctas, int rm_C, int rm_OW, int rm_Wg, const void* saved_bits,
-                  cudaStream_t stream) {
+template <int CPT, bool MN>
+static int launch_conv(int BN, bool bres, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
+                       cudaStream_t st) {
+  if (MN) {
+    switch (BN) {
+      case 32: return launch<32, CPT, MN, true>(tmA, tmB, p, 0, st);
+      case 64: return launch<64, CPT, MN, true>(tmA, tmB, p, 0, st);
+      case 128: return launch<128, CPT, MN, true>(tmA, tmB, p, 0, st);
+      default: break;
+    }
+  } else if (bres) {
+    switch (BN) {
+      case 32: return launch<32, CPT, false, true, !MN>(tmA, tmB, p, 0, st);
+      case 64: return launch<64, CPT, false, true, !MN>(tmA, tmB, p, 0, st);
+      case 128: return launch<128, CPT, false, true, !MN>(tmA, tmB, p, 0, st);
+      default: break;
+    }
+  } else {
+    switch (BN) {
+      case 32: return launch<32, CPT, false, true>(tmA, tmB, p, 0, st);
+      case 64: return launch<64, CPT, false, true>(tmA, tmB, p, 0, st);
+      case 128: return launch<128, CPT, false, true>(tmA, tmB, p, 0, st);
+      default: break;
+    }
+  }
+  set_last_error("conv_gemm: unsupported tile N=%d", BN);
+  return B200RL_ERR_UNSUPPORTED;
+}
+
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_gemm_f16(const void* A, const void* B, void* C, const float* bias, const void* saved, int M,
+                               int N, int K, long long lda, long long ldb, long long ldc, long long ld_saved,
+                               int mn_major, int mode, int act, float alpha, int split_k, int max_ctas, int rm_C,
+                               int rm_OW, int rm_Wg, const void* saved_bits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(A && B && C, "gemm: null operand");
   B200RL_REQUIRE(rm_C == 0 || (rm_C % 16 == 0 && rm_OW > 0 && rm_Wg >= rm_OW && (mode == MODE_F16_ACT || mode == MODE_F16_DACT)),
                  "gemm: bad column remap");
@@ -626,42 +659,15 @@ int gemm_f16_impl(const void* A, const void* B, void* C, const float* bias, cons
   return rc;
 }
 
-template <int CPT, bool MN>
-static int launch_conv(int BN, bool bres, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
-                       cudaStream_t st) {
-  if (MN) {
-    switch (BN) {
-      case 32: return launch<32, CPT, MN, true>(tmA, tmB, p, 0, st);
-      case 64: return launch<64, CPT, MN, true>(tmA, tmB, p, 0, st);
-      case 128: return launch<128, CPT, MN, true>(tmA, tmB, p, 0, st);
-      default: break;
-    }
-  } else if (bres) {
-    switch (BN) {
-      case 32: return launch<32, CPT, false, true, !MN>(tmA, tmB, p, 0, st);
-      case 64: return launch<64, CPT, false, true, !MN>(tmA, tmB, p, 0, st);
-      case 128: return launch<128, CPT, false, true, !MN>(tmA, tmB, p, 0, st);
-      default: break;
-    }
-  } else {
-    switch (BN) {
-      case 32: return launch<32, CPT, false, true>(tmA, tmB, p, 0, st);
-      case 64: return launch<64, CPT, false, true>(tmA, tmB, p, 0, st);
-      case 128: return launch<128, CPT, false, true>(tmA, tmB, p, 0, st);
-      default: break;
-    }
-  }
-  set_last_error("conv_gemm: unsupported tile N=%d", BN);
-  return B200RL_ERR_UNSUPPORTED;
-}
-
 // Implicit-GEMM convolution on an NHWC fp16 tensor x[B, H, W, C] whose filter window is described by
 // (R x S taps, stride, lower padding).  kind: 0 = forward / dgrad-style (rows = base pixels, K = taps*C,
 // Wt = [N, taps*C] K-major), 1 = wgrad (out[taps*C, N] += x_patches^T * dz, dz = [B*OH*OW, N]).
-int conv_gemm_impl(const void* x, long long B, int H, int W, int C, int R, int S, int stride_h, int stride_w,
-                   int pad_h, int pad_w, int OH, int OW, const void* Wt_or_dz, long long ldb, void* out, long long ldc,
-                   const float* bias, const void* saved, long long ld_saved, int N, int kind, int mode, int act,
-                   float alpha, int split_k, int sh_H, int sh_W, int sh_C, int sh_s, cudaStream_t stream) {
+extern "C" int b200rl_conv_gemm(const void* x, long long B, int H, int W, int C, int R, int S, int stride_h,
+                                int stride_w, int pad_h, int pad_w, int OH, int OW, const void* Wt_or_dz, long long ldb,
+                                void* out, long long ldc, const float* bias, const void* saved, long long ld_saved,
+                                int N, int kind, int mode, int act, float alpha, int split_k, int sh_H, int sh_W,
+                                int sh_C, int sh_s, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(x && Wt_or_dz && out && B > 0, "conv_gemm: null operand");
   B200RL_REQUIRE(C == 16 || C == 32 || C == 64, "conv_gemm: channels per tap must be 16, 32 or 64 (got %d)", C);
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (ldb % 8) == 0, "conv_gemm: alignment");
@@ -727,5 +733,3 @@ int conv_gemm_impl(const void* x, long long B, int H, int W, int C, int R, int S
   if (rc == B200RL_OK && p.ws) rc = sum_partials(p.ws, p.splits, p.M, p.N, reinterpret_cast<float*>(out), ldc, stream);
   return rc;
 }
-
-}  // namespace b200rl

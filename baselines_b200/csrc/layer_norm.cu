@@ -195,8 +195,13 @@ static bool ln_shape_ok(int N, long long ld_a, long long ld_b, long long ld_c, c
     else KERNEL<32, 4><<<(GRID)(32), 32 * LN_WARPS, 0, stream>>>(__VA_ARGS__);                      \
   } while (0)
 
-int ln_fwd_impl(const float* z, long long ld_z, const float* gamma, const float* beta, void* y, long long ld_y,
-                long long rows, int N, int act, float eps, cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_ln_fwd(const float* z, long long ld_z, const float* gamma, const float* beta, void* y,
+                             long long ld_y, long long rows, int N, int act, float eps, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(z && gamma && beta && y && rows > 0 && act >= 0 && act <= 2, "ln_fwd: bad args");
   B200RL_REQUIRE(ln_shape_ok(N, ld_z, ld_y, ld_y, z, y, y),
                  "ln_fwd: N a multiple of 8 in [8, 1024], row pitches multiples of 8 and >= N, 16-byte aligned rows");
@@ -205,9 +210,10 @@ int ln_fwd_impl(const float* z, long long ld_z, const float* gamma, const float*
   return check_launch("ln_fwd_kernel");
 }
 
-int ln_bwd_impl(const void* du, long long ld_du, const float* z, long long ld_z, const float* gamma, void* dz,
-                long long ld_dz, float* dgamma, float* dbeta, long long rows, int N, float alpha, float eps,
-                cudaStream_t stream) {
+extern "C" int b200rl_ln_bwd(const void* du, long long ld_du, const float* z, long long ld_z, const float* gamma,
+                             void* dz, long long ld_dz, float* dgamma, float* dbeta, long long rows, int N, float alpha,
+                             float eps, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(du && z && gamma && dz && dgamma && dbeta && rows > 0, "ln_bwd: bad args");
   B200RL_REQUIRE(ln_shape_ok(N, ld_du, ld_z, ld_dz, du, z, dz),
                  "ln_bwd: N a multiple of 8 in [8, 1024], row pitches multiples of 8 and >= N, 16-byte aligned rows");
@@ -223,5 +229,3 @@ int ln_bwd_impl(const void* du, long long ld_du, const float* z, long long ld_z,
   if (rc == B200RL_OK) rc = sum_partials(pb, parts, 1, N, dbeta, N, stream);
   return rc;
 }
-
-}  // namespace b200rl

@@ -303,9 +303,15 @@ static int lstm_bwd_launch(const LstmBwdParams& p, cudaStream_t stream) {
   return check_launch("lstm_seq_bwd_kernel");
 }
 
-int lstm_seq_fwd_impl(const float* xg, long long ldxg, const void* wh, const uint8_t* masks, const long long* mask_idx,
-                      const float* state_in, const long long* state_idx, float* state_out, void* h_out, long long ldh,
-                      void* hprev_out, float* gates_out, float* c_out, int T, int B, int H, cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_lstm_seq_fwd(const float* xg, long long ldxg, const void* wh, const uint8_t* masks,
+                                   const long long* mask_idx, const float* state_in, const long long* state_idx,
+                                   float* state_out, void* h_out, long long ldh, void* hprev_out, float* gates_out,
+                                   float* c_out, int T, int B, int H, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(xg && wh && masks && state_in && h_out, "lstm_seq_fwd: null operand");
   B200RL_REQUIRE(H == 64 || H == 128, "lstm_seq_fwd: H = %d (instances: 64, 128)", H);
   B200RL_REQUIRE(T >= 1 && B >= 1, "lstm_seq_fwd: T = %d, B = %d", T, B);
@@ -322,9 +328,11 @@ int lstm_seq_fwd_impl(const float* xg, long long ldxg, const void* wh, const uin
   return H == 64 ? lstm_fwd_launch<64>(p, stream) : lstm_fwd_launch<128>(p, stream);
 }
 
-int lstm_seq_bwd_impl(const void* dh, long long lddh, const float* gates, const float* c, const uint8_t* masks,
-                      const long long* mask_idx, const float* state_in, const long long* state_idx, const void* whT,
-                      void* dz, long long lddz, int T, int B, int H, cudaStream_t stream) {
+extern "C" int b200rl_lstm_seq_bwd(const void* dh, long long lddh, const float* gates, const float* c,
+                                   const uint8_t* masks, const long long* mask_idx, const float* state_in,
+                                   const long long* state_idx, const void* whT, void* dz, long long lddz, int T, int B,
+                                   int H, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(dh && gates && c && masks && state_in && whT && dz, "lstm_seq_bwd: null operand");
   B200RL_REQUIRE(H == 64 || H == 128, "lstm_seq_bwd: H = %d (instances: 64, 128)", H);
   B200RL_REQUIRE(T >= 1 && B >= 1, "lstm_seq_bwd: T = %d, B = %d", T, B);
@@ -335,5 +343,3 @@ int lstm_seq_bwd_impl(const void* dh, long long lddh, const float* gates, const 
                   reinterpret_cast<const __half*>(whT), reinterpret_cast<__half*>(dz), lddz, T, B};
   return H == 64 ? lstm_bwd_launch<64>(p, stream) : lstm_bwd_launch<128>(p, stream);
 }
-
-}  // namespace b200rl

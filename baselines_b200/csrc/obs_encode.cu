@@ -91,9 +91,14 @@ __global__ void __launch_bounds__(256) obs_encode_kernel(const ObsEncodeParams p
   }
 }
 
-int obs_encode_impl(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim, int in_pad,
-                    const float* mean, const float* inv_std, float clip_lo, float clip_hi, int onehot_n,
-                    const int* seg_off, int nseg, void* out, int* overflow, cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_obs_encode(const float* x, const long long* src_idx, long long B, int raw_dim, int in_dim,
+                                 int in_pad, const float* mean, const float* inv_std, float clip_lo, float clip_hi,
+                                 int onehot_n, const int* seg_off, int nseg, void* out, int* overflow, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(x && out && B > 0, "obs_encode: null operand");
   B200RL_REQUIRE(in_pad % 8 == 0 && in_pad >= in_dim && in_dim > 0, "obs_encode: in_pad must be a multiple of 8 >= in_dim");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "obs_encode: output must be 16-byte aligned");
@@ -113,5 +118,3 @@ int obs_encode_impl(const float* x, const long long* src_idx, long long B, int r
   obs_encode_kernel<<<(int)blocks, 256, 0, stream>>>(p);
   return check_launch("obs_encode_kernel");
 }
-
-}  // namespace b200rl

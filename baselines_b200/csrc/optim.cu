@@ -234,54 +234,11 @@ static int grid_for(long long n, int threads, int per_sm) {
   return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
 }
 
-int sumsq_impl(const float* g, long long n, double* out, cudaStream_t stream) {
-  B200RL_REQUIRE(g && out && n > 0, "sumsq: bad args");
-  B200RL_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "sumsq: gradient buffer must be 16 B aligned");
-  cudaMemsetAsync(out, 0, sizeof(double), stream);
-  const int grid = grid_for(n / 4 + 1, 256, 4);
-  B200RL_REQUIRE(grid <= SUMSQ_MAX_BLOCKS, "sumsq: %d blocks exceed the partial-sum slots", grid);
-  sumsq_kernel<<<grid, 256, 0, stream>>>(g, n, out);
-  return check_launch("sumsq_kernel");
-}
-
-int seg_sumsq_impl(const float* g, const long long* seg_off, int nseg, double* out, cudaStream_t stream) {
-  B200RL_REQUIRE(g && seg_off && out && nseg > 0, "seg_sumsq: bad args");
-  constexpr int SLICES = 16;
-  double* part = reinterpret_cast<double*>(det_workspace((size_t)nseg * SLICES * 2, stream));
-  if (!part) return B200RL_ERR_CUDA;
-  seg_sumsq_kernel<<<dim3(nseg, SLICES), 256, 0, stream>>>(g, seg_off, part);
-  seg_sumsq_finish_kernel<<<ceil_div(nseg, 128), 128, 0, stream>>>(part, nseg, SLICES, out);
-  return check_launch("seg_sumsq_kernel");
-}
-
-int clip_adam_impl(float* p, const float* g, float* m, float* v, long long n, float lr_t, float beta1, float beta2,
-                   float eps, float clip, const double* sumsq, const long long* seg_off, int nseg,
-                   const float* lr_t_dev, cudaStream_t stream) {
-  B200RL_REQUIRE(p && g && m && v && n > 0, "clip_adam: bad args");
-  B200RL_REQUIRE(clip <= 0.0f || sumsq != nullptr, "clip_adam: clipping needs the device sumsq");
-  AdamArgs a{lr_t, beta1, beta2, eps, clip};
-  clip_adam_kernel<<<grid_for(n, 256, 8), 256, 0, stream>>>(p, g, m, v, n, a, sumsq, seg_off, nseg, lr_t_dev);
-  return check_launch("clip_adam_kernel");
-}
-
 __global__ void set_scalars_kernel(float* dst, float a, float b, float c, float d, int n) {
   const float v[4] = {a, b, c, d};
   if (threadIdx.x < n) dst[threadIdx.x] = v[threadIdx.x];
 }
 __global__ void counter_add_kernel(unsigned long long* ctr, unsigned long long inc) { *ctr += inc; }
-
-// dst[0..n) = {a, b, c, d}[0..n): scalars that change between replays of a captured launch sequence (Adam step size,
-// clip range) travel as kernel arguments of this one-thread kernel, so no host buffer can be overwritten too early
-int set_scalars_impl(float* dst, int n, float a, float b, float c, float d, cudaStream_t stream) {
-  B200RL_REQUIRE(dst && n >= 1 && n <= 4, "set_scalars: 1..4 values");
-  set_scalars_kernel<<<1, 32, 0, stream>>>(dst, a, b, c, d, n);
-  return check_launch("set_scalars_kernel");
-}
-int counter_add_impl(unsigned long long* ctr, unsigned long long inc, cudaStream_t stream) {
-  B200RL_REQUIRE(ctr != nullptr, "counter_add: null counter");
-  counter_add_kernel<<<1, 1, 0, stream>>>(ctr, inc);
-  return check_launch("counter_add_kernel");
-}
 
 // Minibatch shuffle on the device (replaces np.random.shuffle(inds) of ppo2/ppo2.py:160 + the index arithmetic of
 // sf01, ppo2/runner.py:69-74): out[i] = buffer offset of the pi(i)-th sample, pi a keyed pseudo-random BIJECTION of
@@ -320,8 +277,62 @@ shuffle_indices_kernel(long long* __restrict__ out, long long n, unsigned long l
   }
 }
 
-int shuffle_indices_impl(long long* out, long long n, unsigned long long key, long long T, long long N,
-                         cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_sumsq(const float* g, long long n, double* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200RL_REQUIRE(g && out && n > 0, "sumsq: bad args");
+  B200RL_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "sumsq: gradient buffer must be 16 B aligned");
+  cudaMemsetAsync(out, 0, sizeof(double), stream);
+  const int grid = grid_for(n / 4 + 1, 256, 4);
+  B200RL_REQUIRE(grid <= SUMSQ_MAX_BLOCKS, "sumsq: %d blocks exceed the partial-sum slots", grid);
+  sumsq_kernel<<<grid, 256, 0, stream>>>(g, n, out);
+  return check_launch("sumsq_kernel");
+}
+
+extern "C" int b200rl_seg_sumsq(const float* g, const long long* seg_off, int nseg, double* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200RL_REQUIRE(g && seg_off && out && nseg > 0, "seg_sumsq: bad args");
+  constexpr int SLICES = 16;
+  double* part = reinterpret_cast<double*>(det_workspace((size_t)nseg * SLICES * 2, stream));
+  if (!part) return B200RL_ERR_CUDA;
+  seg_sumsq_kernel<<<dim3(nseg, SLICES), 256, 0, stream>>>(g, seg_off, part);
+  seg_sumsq_finish_kernel<<<ceil_div(nseg, 128), 128, 0, stream>>>(part, nseg, SLICES, out);
+  return check_launch("seg_sumsq_kernel");
+}
+
+extern "C" int b200rl_clip_adam(float* p, const float* g, float* m, float* v, long long n, float lr_t, float beta1,
+                                float beta2, float eps, float clip, const double* sumsq, const long long* seg_off,
+                                int nseg, const float* lr_t_dev, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200RL_REQUIRE(p && g && m && v && n > 0, "clip_adam: bad args");
+  B200RL_REQUIRE(clip <= 0.0f || sumsq != nullptr, "clip_adam: clipping needs the device sumsq");
+  AdamArgs a{lr_t, beta1, beta2, eps, clip};
+  clip_adam_kernel<<<grid_for(n, 256, 8), 256, 0, stream>>>(p, g, m, v, n, a, sumsq, seg_off, nseg, lr_t_dev);
+  return check_launch("clip_adam_kernel");
+}
+
+// dst[0..n) = {a, b, c, d}[0..n): scalars that change between replays of a captured launch sequence (Adam step size,
+// clip range) travel as kernel arguments of this one-thread kernel, so no host buffer can be overwritten too early
+extern "C" int b200rl_set_scalars(float* dst, int n, float a, float b, float c, float d, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200RL_REQUIRE(dst && n >= 1 && n <= 4, "set_scalars: 1..4 values");
+  set_scalars_kernel<<<1, 32, 0, stream>>>(dst, a, b, c, d, n);
+  return check_launch("set_scalars_kernel");
+}
+
+extern "C" int b200rl_counter_add(unsigned long long* ctr, unsigned long long inc, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200RL_REQUIRE(ctr != nullptr, "counter_add: null counter");
+  counter_add_kernel<<<1, 1, 0, stream>>>(ctr, inc);
+  return check_launch("counter_add_kernel");
+}
+
+extern "C" int b200rl_shuffle_indices(long long* out, long long n, unsigned long long key, long long T, long long N,
+                                      void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(out && n > 0 && n < (1LL << 40), "shuffle_indices: bad args");
   B200RL_REQUIRE(T == 0 || T * N == n, "shuffle_indices: T*N must equal n");
   int half_bits = 1;
@@ -330,16 +341,18 @@ int shuffle_indices_impl(long long* out, long long n, unsigned long long key, lo
   return check_launch("shuffle_indices_kernel");
 }
 
-int clip_accumulate_impl(const float* g, float* acc, long long n, float clip, float weight, const double* sumsq,
-                         cudaStream_t stream) {
+extern "C" int b200rl_clip_accumulate(const float* g, float* acc, long long n, float clip, float weight,
+                                      const double* sumsq, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(g && acc && n > 0, "clip_accumulate: bad args");
   B200RL_REQUIRE(clip <= 0.0f || sumsq != nullptr, "clip_accumulate: clipping needs the device sumsq");
   clip_accumulate_kernel<<<grid_for(n, 256, 8), 256, 0, stream>>>(g, acc, n, clip, weight, sumsq);
   return check_launch("clip_accumulate_kernel");
 }
 
-int cast_transpose_impl(const float* src, int R, int C, void* dst, long long ld_dst, void* dstT, long long ld_t,
-                        float scale, cudaStream_t stream) {
+extern "C" int b200rl_cast_transpose(const float* src, int R, int C, void* dst, long long ld_dst, void* dstT,
+                                     long long ld_t, float scale, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(src && R > 0 && C > 0 && (dst || dstT), "cast_transpose: bad args");
   dim3 grid(ceil_div(C, 32), ceil_div(R, 32));
   cast_transpose_kernel<<<grid, 256, 0, stream>>>(src, R, C, reinterpret_cast<__half*>(dst), ld_dst,
@@ -347,7 +360,8 @@ int cast_transpose_impl(const float* src, int R, int C, void* dst, long long ld_
   return check_launch("cast_transpose_kernel");
 }
 
-int cast_transpose_batch_impl(const void* jobs, int njobs, int max_rows, int max_cols, cudaStream_t stream) {
+extern "C" int b200rl_cast_transpose_batch(const void* jobs, int njobs, int max_rows, int max_cols, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(jobs && njobs > 0 && njobs <= 65535 && max_rows > 0 && max_cols > 0, "cast_transpose_batch: bad args");
   static_assert(sizeof(CastJob) == 56, "CastJob layout is part of the C ABI (see include/b200rl.h)");
   dim3 grid(ceil_div(max_cols, 32), ceil_div(max_rows, 32), njobs);
@@ -355,8 +369,9 @@ int cast_transpose_batch_impl(const void* jobs, int njobs, int max_rows, int max
   return check_launch("cast_transpose_batch_kernel");
 }
 
-int dgrad_weights_impl(const float* w, void* out, int R, int S, int Cin, int Cout, int s, long long ld,
-                       cudaStream_t stream) {
+extern "C" int b200rl_dgrad_weights(const float* w, void* out, int R, int S, int Cin, int Cout, int s, long long ld,
+                                    void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(w && out && R > 0 && S > 0 && s > 0, "dgrad_weights: bad args");
   const int An = (R + s - 1) / s;
   const long long total = (long long)s * s * Cin * An * An * Cout;
@@ -365,12 +380,11 @@ int dgrad_weights_impl(const float* w, void* out, int R, int S, int Cin, int Cou
   return check_launch("dgrad_weights_kernel");
 }
 
-int cast_f32_f16_impl(const float* src, void* dst, long long rows, int cols, long long ld_src, long long ld_dst,
-                      float scale, cudaStream_t stream) {
+extern "C" int b200rl_cast_f32_f16(const float* src, void* dst, long long rows, int cols, long long ld_src,
+                                   long long ld_dst, float scale, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(src && dst && rows > 0 && cols > 0, "cast: bad args");
   cast_f32_f16_kernel<<<grid_for(rows * cols, 256, 8), 256, 0, stream>>>(src, reinterpret_cast<__half*>(dst), rows,
                                                                          cols, ld_src, ld_dst, scale);
   return check_launch("cast_f32_f16_kernel");
 }
-
-}  // namespace b200rl

@@ -97,9 +97,14 @@ dqn_param_noise_adapt_kernel(const float* __restrict__ q, const float* __restric
   }
 }
 
-int param_perturb_impl(const float* src, float* dst, const void* jobs, int njobs, long long max_len,
-                       const float* scale_dev, const float* normals, unsigned long long seed,
-                       const unsigned long long* offset_dev, cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_param_perturb(const float* src, float* dst, const void* jobs, int njobs, long long max_len,
+                                    const float* scale_dev, const float* normals, unsigned long long seed,
+                                    const unsigned long long* offset_dev, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(src && dst && jobs && njobs > 0 && max_len > 0 && scale_dev && offset_dev, "param_perturb: bad args");
   B200RL_REQUIRE(njobs <= 65535, "param_perturb: at most 65535 variables per launch");
   const dim3 grid((unsigned)std::min<long long>(ceil_div_ll(max_len, 256), 64), (unsigned)njobs);
@@ -108,13 +113,13 @@ int param_perturb_impl(const float* src, float* dst, const void* jobs, int njobs
   return check_launch("param_perturb_kernel");
 }
 
-int dqn_param_noise_adapt_impl(const float* q, const float* q_adapt, long long ld, int nA, int dueling, int B,
-                               float* scale_dev, const float* threshold_dev, float* mean_kl_dev, cudaStream_t stream) {
+extern "C" int b200rl_dqn_param_noise_adapt(const float* q, const float* q_adapt, long long ld, int nA, int dueling,
+                                            int B, float* scale_dev, const float* threshold_dev, float* mean_kl_dev,
+                                            void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(q && q_adapt && nA > 0 && B > 0 && scale_dev && threshold_dev && mean_kl_dev && ld >= nA + (dueling != 0),
                  "dqn_param_noise_adapt: bad args");
   dqn_param_noise_adapt_kernel<<<1, 256, 0, stream>>>(q, q_adapt, ld, nA, dueling, B, scale_dev, threshold_dev,
                                                       mean_kl_dev);
   return check_launch("dqn_param_noise_adapt_kernel");
 }
-
-}  // namespace b200rl

@@ -537,11 +537,16 @@ gauss_loss_kernel(const float* __restrict__ mean, long long ld, const float* __r
   block_accumulate5(st, pc.stats);
 }
 
+}  // namespace b200rl
+
+using namespace b200rl;
+
 // ---------------------------------------------------------------- launchers
-int cat_step_impl(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
-                  long long ldv, const float* uniforms, unsigned long long seed, unsigned long long offset,
-                  const unsigned long long* offset_dev, long long* actions, float* values, float* neglogp, long long B,
-                  cudaStream_t stream) {
+extern "C" int b200rl_cat_step(const float* logits, long long ld, int nA, const int* seg_off, int nseg,
+                               const float* vpred, long long ldv, const float* uniforms, unsigned long long seed,
+                               unsigned long long offset, const unsigned long long* offset_dev, long long* actions,
+                               float* values, float* neglogp, long long B, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(logits && vpred && actions && values && neglogp && B > 0 && nA > 0, "cat_step: bad args");
   B200RL_REQUIRE(seg_off == nullptr || (nseg >= 1 && nseg <= nA), "cat_step: a segment table needs 1 <= nseg <= nA");
   const int grid = (int)ceil_div_ll(B, 256);
@@ -554,38 +559,44 @@ int cat_step_impl(const float* logits, long long ld, int nA, const int* seg_off,
   return check_launch("cat_step_kernel");
 }
 
-int bern_step_impl(const float* logits, long long ld, int n, const float* vpred, long long ldv, const float* uniforms,
-                   unsigned long long seed, unsigned long long offset, const unsigned long long* offset_dev,
-                   float* actions, float* values, float* neglogp, long long B, cudaStream_t stream) {
+extern "C" int b200rl_bern_step(const float* logits, long long ld, int n, const float* vpred, long long ldv,
+                                const float* uniforms, unsigned long long seed, unsigned long long offset,
+                                const unsigned long long* offset_dev, float* actions, float* values, float* neglogp,
+                                long long B, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(logits && vpred && actions && values && neglogp && B > 0 && n > 0, "bern_step: bad args");
   bern_step_kernel<<<(int)ceil_div_ll(B, 256), 256, 0, stream>>>(logits, ld, n, vpred, ldv, uniforms, seed, offset,
                                                                   offset_dev, actions, values, neglogp, B);
   return check_launch("bern_step_kernel");
 }
 
-int gauss_step_impl(const float* mean, long long ld, const float* logstd, int d, const float* vpred, long long ldv,
-                    const float* normals, unsigned long long seed, unsigned long long offset,
-                    const unsigned long long* offset_dev, float* actions, float* values, float* neglogp, long long B,
-                    cudaStream_t stream) {
+extern "C" int b200rl_gauss_step(const float* mean, long long ld, const float* logstd, int d, const float* vpred,
+                                 long long ldv, const float* normals, unsigned long long seed,
+                                 unsigned long long offset, const unsigned long long* offset_dev, float* actions,
+                                 float* values, float* neglogp, long long B, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(mean && logstd && vpred && actions && values && neglogp && B > 0 && d > 0, "gauss_step: bad args");
   gauss_step_kernel<<<(int)ceil_div_ll(B, 256), 256, 0, stream>>>(mean, ld, logstd, d, vpred, ldv, normals, seed,
                                                                    offset, offset_dev, actions, values, neglogp, B);
   return check_launch("gauss_step_kernel");
 }
 
-int adv_stats_impl(const float* returns, const float* values, const long long* src_idx, long long M, double* out,
-                   cudaStream_t stream) {
+extern "C" int b200rl_adv_stats(const float* returns, const float* values, const long long* src_idx, long long M,
+                                double* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(returns && values && out && M > 0, "adv_stats: bad args");
   const int blocks = (int)((M + 4095) / 4096 < ADV_BLOCKS ? (M + 4095) / 4096 : ADV_BLOCKS);
   adv_stats_kernel<<<blocks, 512, 0, stream>>>(returns, values, src_idx, M, out);
   return check_launch("adv_stats_kernel");
 }
 
-int cat_loss_impl(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
-                  long long ldv, const long long* actions, const long long* src_idx, const float* returns,
-                  const float* old_values, const float* old_neglogp, const double* adv_stats, float cliprange,
-                  float ent_coef, float vf_coef, void* dlogits, long long ld_dl, void* dv, long long ld_dv,
-                  double* stats, long long B, const float* cliprange_dev, cudaStream_t stream) {
+extern "C" int b200rl_cat_loss(const float* logits, long long ld, int nA, const int* seg_off, int nseg,
+                               const float* vpred, long long ldv, const long long* actions, const long long* src_idx,
+                               const float* returns, const float* old_values, const float* old_neglogp,
+                               const double* adv_stats, float cliprange, float ent_coef, float vf_coef, void* dlogits,
+                               long long ld_dl, void* dv, long long ld_dv, double* stats, long long B,
+                               const float* cliprange_dev, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(logits && vpred && actions && returns && old_values && old_neglogp && adv_stats && dlogits && dv &&
                      stats && B > 0 && nA > 0,
                  "cat_loss: bad args");
@@ -603,11 +614,13 @@ int cat_loss_impl(const float* logits, long long ld, int nA, const int* seg_off,
   return check_launch("cat_loss_kernel");
 }
 
-int bern_loss_impl(const float* logits, long long ld, int n, const float* vpred, long long ldv, const float* actions,
-                   const long long* src_idx, const float* returns, const float* old_values, const float* old_neglogp,
-                   const double* adv_stats, float cliprange, float ent_coef, float vf_coef, void* dlogits,
-                   long long ld_dl, void* dv, long long ld_dv, double* stats, long long B, const float* cliprange_dev,
-                   cudaStream_t stream) {
+extern "C" int b200rl_bern_loss(const float* logits, long long ld, int n, const float* vpred, long long ldv,
+                                const float* actions, const long long* src_idx, const float* returns,
+                                const float* old_values, const float* old_neglogp, const double* adv_stats,
+                                float cliprange, float ent_coef, float vf_coef, void* dlogits, long long ld_dl,
+                                void* dv, long long ld_dv, double* stats, long long B, const float* cliprange_dev,
+                                void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(logits && vpred && actions && returns && old_values && old_neglogp && adv_stats && dlogits && dv &&
                      stats && B > 0 && n > 0,
                  "bern_loss: bad args");
@@ -618,11 +631,13 @@ int bern_loss_impl(const float* logits, long long ld, int n, const float* vpred,
   return check_launch("bern_loss_kernel");
 }
 
-int gauss_loss_impl(const float* mean, long long ld, const float* logstd, int d, const float* vpred, long long ldv,
-                    const float* actions, const long long* src_idx, const float* returns, const float* old_values,
-                    const float* old_neglogp, const double* adv_stats, float cliprange, float ent_coef, float vf_coef,
-                    void* dmean, long long ld_dm, void* dv, long long ld_dv, float* dlogstd, float inv_M,
-                    double* stats, long long B, const float* cliprange_dev, cudaStream_t stream) {
+extern "C" int b200rl_gauss_loss(const float* mean, long long ld, const float* logstd, int d, const float* vpred,
+                                 long long ldv, const float* actions, const long long* src_idx, const float* returns,
+                                 const float* old_values, const float* old_neglogp, const double* adv_stats,
+                                 float cliprange, float ent_coef, float vf_coef, void* dmean, long long ld_dm, void* dv,
+                                 long long ld_dv, float* dlogstd, float inv_M, double* stats, long long B,
+                                 const float* cliprange_dev, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(mean && logstd && vpred && actions && returns && old_values && old_neglogp && adv_stats && dmean &&
                      dv && dlogstd && stats && B > 0,
                  "gauss_loss: bad args");
@@ -646,5 +661,3 @@ int gauss_loss_impl(const float* mean, long long ld, const float* logstd, int d,
   const int rc = check_launch("gauss_loss_kernel");
   return rc == B200RL_OK ? sum_partials(part, grid, 1, d, dlogstd, d, stream) : rc;
 }
-
-}  // namespace b200rl

@@ -241,9 +241,14 @@ __global__ void dqn_act_kernel(QHead q, int nA, float eps, unsigned long long se
   actions[b] = (u < eps) ? r : arg;
 }
 
+}  // namespace b200rl
+
+using namespace b200rl;
+
 // ------------------------------------------------------------------------------------------ launchers
-int tree_set_impl(double* sum_tree, double* min_tree, long long capacity, const long long* idx, const double* vals,
-                  int n, cudaStream_t stream) {
+extern "C" int b200rl_tree_set(double* sum_tree, double* min_tree, long long capacity, const long long* idx,
+                               const double* vals, int n, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(sum_tree && min_tree && idx && vals && n > 0, "tree_set: bad args");
   B200RL_REQUIRE(capacity > 0 && (capacity & (capacity - 1)) == 0, "tree_set: capacity must be a power of two");
   for (int o = 0; o < n; o += 1024) {
@@ -253,8 +258,9 @@ int tree_set_impl(double* sum_tree, double* min_tree, long long capacity, const 
   return check_launch("tree_set_kernel");
 }
 
-int tree_range_sum_impl(const double* tree, long long capacity, long long start, long long end, double* out,
-                        cudaStream_t stream) {
+extern "C" int b200rl_tree_range_sum(const double* tree, long long capacity, long long start, long long end,
+                                     double* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(tree && out, "tree_range_sum: bad args");
   // reference semantics (segment_tree.py:69-74): end exclusive, negative wraps by +capacity
   if (end < 0) end += capacity;
@@ -264,9 +270,10 @@ int tree_range_sum_impl(const double* tree, long long capacity, long long start,
   return check_launch("tree_range_sum_kernel");
 }
 
-int per_sample_impl(const double* sum_tree, const double* min_tree, long long capacity, long long n_stored,
-                    const double* uniforms, int batch, double beta, long long* idx_out, double* w_out,
-                    float* w_out_f32, int* bad, cudaStream_t stream) {
+extern "C" int b200rl_per_sample(const double* sum_tree, const double* min_tree, long long capacity, long long n_stored,
+                                 const double* uniforms, int batch, double beta, long long* idx_out, double* w_out,
+                                 float* w_out_f32, int* bad, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(sum_tree && min_tree && uniforms && idx_out && w_out && batch > 0, "per_sample: bad args");
   B200RL_REQUIRE(n_stored >= 2 && n_stored <= capacity, "per_sample: need 2 <= n_stored <= capacity");
   B200RL_REQUIRE(beta > 0, "per_sample: beta must be > 0");
@@ -275,25 +282,28 @@ int per_sample_impl(const double* sum_tree, const double* min_tree, long long ca
   return check_launch("per_sample_kernel");
 }
 
-int per_priorities_impl(const float* td, int n, double eps, double alpha, double* powered, double* max_priority,
-                        int* bad, cudaStream_t stream) {
+extern "C" int b200rl_per_priorities(const float* td, int n, double eps, double alpha, double* powered,
+                                     double* max_priority, int* bad, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(td && powered && max_priority && bad && n > 0, "per_priorities: bad args");
   per_priorities_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(td, n, eps, alpha, powered, max_priority, bad);
   return check_launch("per_priorities_kernel");
 }
 
-int per_pow_impl(const double* x, int n, double y, double* out, cudaStream_t stream) {
+extern "C" int b200rl_per_pow(const double* x, int n, double y, double* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(x && out && n > 0, "per_pow: bad args");
   per_pow_kernel<<<ceil_div(n, 256), 256, 0, stream>>>(x, n, y, out);
   return check_launch("per_pow_kernel");
 }
 
-int dqn_td_impl(const float* a_t, long long lda_t, const float* s_t, long long lds_t, const float* a_on,
-                long long lda_on, const float* s_on, long long lds_on, const float* a_tg, long long lda_tg,
-                const float* s_tg, long long lds_tg, int nA, const long long* idx, const long long* actions,
-                const float* rewards, const float* dones, const float* weights, float gamma, int double_q,
-                float* td_out, void* d_a, long long ld_da, void* d_s, long long ld_ds, double* loss_sum, int B,
-                cudaStream_t stream) {
+extern "C" int b200rl_dqn_td(const float* a_t, long long lda_t, const float* s_t, long long lds_t, const float* a_on,
+                             long long lda_on, const float* s_on, long long lds_on, const float* a_tg, long long lda_tg,
+                             const float* s_tg, long long lds_tg, int nA, const long long* idx,
+                             const long long* actions, const float* rewards, const float* dones, const float* weights,
+                             float gamma, int double_q, float* td_out, void* d_a, long long ld_da, void* d_s,
+                             long long ld_ds, double* loss_sum, int B, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(a_t && a_tg && actions && rewards && dones && weights && td_out && d_a && loss_sum && B > 0,
                  "dqn_td: bad args");
   B200RL_REQUIRE(!double_q || a_on, "dqn_td: double_q needs the online q(s')");
@@ -305,13 +315,12 @@ int dqn_td_impl(const float* a_t, long long lda_t, const float* s_t, long long l
   return check_launch("dqn_td_kernel");
 }
 
-int dqn_act_impl(const float* a, long long lda, const float* s, long long lds, int nA, float eps,
-                 unsigned long long seed, unsigned long long step, const float* eps_dev, const unsigned long long* step_dev, long long* actions, int B,
-                 cudaStream_t stream) {
+extern "C" int b200rl_dqn_act(const float* a, long long lda, const float* s, long long lds, int nA, float eps,
+                              unsigned long long seed, unsigned long long step, const float* eps_dev,
+                              const unsigned long long* step_dev, long long* actions, int B, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(a && actions && B > 0 && nA > 0, "dqn_act: bad args");
   QHead q{a, lda, s, lds};
   dqn_act_kernel<<<ceil_div(B, 128), 128, 0, stream>>>(q, nA, eps, seed, step, eps_dev, step_dev, actions, B);
   return check_launch("dqn_act_kernel");
 }
-
-}  // namespace b200rl

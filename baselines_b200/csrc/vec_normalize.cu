@@ -372,7 +372,12 @@ int moments_t(const void* x, long long N, int D, double* ws, cudaStream_t stream
 
 }  // namespace
 
-int vecnorm_moments_impl(const void* x, int x_f64, long long N, int D, double* ws, cudaStream_t stream) {
+}  // namespace b200rl
+
+using namespace b200rl;
+
+extern "C" int b200rl_vecnorm_moments(const void* x, int x_f64, long long N, int D, double* ws, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(x && ws, "vecnorm_moments: null operand");
   B200RL_REQUIRE(N > 0 && D > 0, "vecnorm_moments: empty batch");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(x) & (x_f64 ? 7 : 3)) == 0, "vecnorm_moments: x must be aligned to its dtype");
@@ -382,16 +387,18 @@ int vecnorm_moments_impl(const void* x, int x_f64, long long N, int D, double* w
   return x_f64 ? moments_t<double>(x, N, D, ws, stream) : moments_t<float>(x, N, D, ws, stream);
 }
 
-int vecnorm_combine_impl(double* rms, const double* ws, int ws_f32, long long N, int D, double eps,
-                         cudaStream_t stream) {
+extern "C" int b200rl_vecnorm_combine(double* rms, const double* ws, int ws_f32, long long N, int D, double eps,
+                                      void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(rms && ws && N > 0 && D > 0, "vecnorm_combine: bad operands");
   B200RL_REQUIRE(!ws_f32 || N < (1LL << 24), "vecnorm_combine: float32 batches need N < 2^24");
   vn_combine_kernel<<<1, 256, 0, stream>>>(rms, ws, N, D, eps, ws_f32 != 0);
   return check_launch("vn_combine_kernel");
 }
 
-int vecnorm_normalize_impl(const void* x, int x_f64, long long N, int D, const double* rms, double clip, float* out,
-                           cudaStream_t stream) {
+extern "C" int b200rl_vecnorm_normalize(const void* x, int x_f64, long long N, int D, const double* rms, double clip,
+                                        float* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(x && out && N > 0 && D > 0, "vecnorm_normalize: bad operands");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(x) & (x_f64 ? 7 : 3)) == 0, "vecnorm_normalize: x must be aligned to its dtype");
   const long long total = N * D;
@@ -404,8 +411,10 @@ int vecnorm_normalize_impl(const void* x, int x_f64, long long N, int D, const d
   return check_launch("vn_normalize_kernel");
 }
 
-int vecnorm_rewards_impl(const void* rew, int rew_f64, const uint8_t* news, long long N, double* ret, double* rms,
-                         double gamma, double eps, double cliprew, float* out, cudaStream_t stream) {
+extern "C" int b200rl_vecnorm_rewards(const void* rew, int rew_f64, const uint8_t* news, long long N, double* ret,
+                                      double* rms, double gamma, double eps, double cliprew, float* out,
+                                      void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(rew && ret && out && N > 0, "vecnorm_rewards: bad operands");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(rew) & (rew_f64 ? 7 : 3)) == 0, "vecnorm_rewards: rew must be aligned to its dtype");
   B200RL_REQUIRE(N <= PW_MAX_N, "vecnorm_rewards: needs N <= %lld", PW_MAX_N);
@@ -418,7 +427,8 @@ int vecnorm_rewards_impl(const void* rew, int rew_f64, const uint8_t* news, long
   return check_launch("vn_rewards_kernel");
 }
 
-int vecnorm_add_latency_impl(int f64, long long n, double* out, cudaStream_t stream) {
+extern "C" int b200rl_vecnorm_add_latency(int f64, long long n, double* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(out && n > 0, "vecnorm_add_latency: bad operands");
   if (f64)
     vn_add_chain_kernel<double><<<1, 1, 0, stream>>>(n, out);
@@ -426,5 +436,3 @@ int vecnorm_add_latency_impl(int f64, long long n, double* out, cudaStream_t str
     vn_add_chain_kernel<float><<<1, 1, 0, stream>>>(n, out);
   return check_launch("vn_add_chain_kernel");
 }
-
-}  // namespace b200rl

@@ -183,7 +183,7 @@ class Linear:
 
     def wgrad(self, x, ldx, dz, lddz, M, alpha):
         """gW += alpha * x^T dz (fp32 atomics, split-K over the batch rows); gb += alpha * colsum(dz)."""
-        bn = 256 if (self.N > 128 and self.N % 256 == 0) else (128 if self.N > 64 else 64)   # gemm_f16_impl's N tile
+        bn = 256 if (self.N > 128 and self.N % 256 == 0) else (128 if self.N > 64 else 64)   # b200rl_gemm_f16's N tile
         tiles = -(-self.K // 128) * -(-self.N // bn)
         kb = -(-M // 64)
         split = max(1, min(kb // 2 if kb >= 2 else 1, -(-2 * ops.num_sms() // tiles)))
@@ -424,14 +424,14 @@ def _shift_stack_ok(ob_shape, convs):
             return False
         k, Hg, Wg, Cg = rf // st, H // st, W // st, C * st * st
         span = (k - 1) * Wg + (k - 1)                    # rows between the first and the last tap
-        # conv_shift_fwd_impl: C = 64 or 128, 1..16 taps, grid >= 2 x 2; conv_shift_wgrad_impl: N = 32 or 64
+        # b200rl_conv_shift_fwd: C = 64 or 128, 1..16 taps, grid >= 2 x 2; b200rl_conv_shift_wgrad: N = 32 or 64
         if Cg not in (64, 128) or k * k > 16 or Hg < 2 or Wg < 2 or nf not in (32, 64):
             return False
-        # conv_shift_fwd_impl: span <= 32 rows for C = 64, <= 16 for C = 128 (sh_arows); resident weights
+        # b200rl_conv_shift_fwd: span <= 32 rows for C = 64, <= 16 for C = 128 (sh_arows); resident weights
         # taps * C/64 * N * 128 B <= 80 KB for C = 64, <= 64 KB for C = 128 (sh_wres_bytes)
         if span > (32 if Cg == 64 else 16) or k * k * (Cg // 64) * nf * 128 > (80 if Cg == 64 else 64) * 1024:
             return False
-        # the data gradient of layer i > 0 is conv_shift_fwd_impl with C = nf: 64
+        # the data gradient of layer i > 0 is b200rl_conv_shift_fwd with C = nf: 64
         if i > 0 and nf != 64:
             return False
         OH, OW = ops._conv_out(H, W, rf, st, False)
@@ -439,7 +439,7 @@ def _shift_stack_ok(ob_shape, convs):
             nrf, nst = convs[i + 1][2], convs[i + 1][3]
             if OH % nst or OW % nst:                     # layer i writes its output space-to-depth'ed for layer i+1
                 return False
-            # the data gradient of layer i+1 writes N = s^2 * nf outputs (conv_shift_fwd_impl: N = 64 or 128 here, C =
+            # the data gradient of layer i+1 writes N = s^2 * nf outputs (b200rl_conv_shift_fwd: N = 64 or 128 here, C =
             # 64, resident weights taps * N * 128 B <= 80 KB)
             kn = nrf // nst
             if nf * nst * nst not in (64, 128) or kn * kn * nf * nst * nst * 128 > 80 * 1024:
@@ -449,7 +449,7 @@ def _shift_stack_ok(ob_shape, convs):
 
 
 def _implicit_geom(H, W, C, rf, st, same_pad, s2d):
-    """The input as TMA im2col sees it, or None.  conv_gemm_impl: 16, 32 or 64 channels per tap; a layer with few
+    """The input as TMA im2col sees it, or None.  b200rl_conv_gemm: 16, 32 or 64 channels per tap; a layer with few
     channels is viewed through "super-pixels" of 16 consecutive (x, c) elements when the stride allows it."""
     if s2d:
         return (H // st, W // st, C * st * st, rf // st, rf // st, 1, 1, 0, 0)
@@ -487,19 +487,19 @@ def plan_conv_stack(ob_shape, convs, same_pad, has_fc):
             layers.append(ConvLayerPlan("shift", st > 1, None, False, k if (k, nf, Cg) in _XFOLD_WGRAD else 1))
             H, W, C = OH, OW, nf
         _nm, nf0, rf0, st0 = convs[0]
-        # conv_shift_fwd_impl / conv_shift_wgrad_impl, uint8 source: s = 4, s*C = 16, N = 32, resident weights
+        # b200rl_conv_shift_fwd / b200rl_conv_shift_wgrad, uint8 source: s = 4, s*C = 16, N = 32, resident weights
         # taps * N * 128 B <= 16 KB (SH_U8_WRES_BYTES)
         fused_u8 = st0 == 4 and ob_shape[2] == 4 and nf0 == 32 and (rf0 // st0) ** 2 * nf0 * 128 <= 16 * 1024
         return ConvStackPlan(True, fused_u8, layers)
     H, W, C = ob_shape
     layers = []
     for i, (_nm, nf, rf, st) in enumerate(convs):
-        # first layer: space-to-depth'ed by s2d_gather_impl (H, W multiples of s; s*C, W*C multiples of 8) into the
-        # 16 / 32 / 64 channels per tap of conv_gemm_impl
+        # first layer: space-to-depth'ed by b200rl_s2d_gather (H, W multiples of s; s*C, W*C multiples of 8) into the
+        # 16 / 32 / 64 channels per tap of b200rl_conv_gemm
         s2d = (i == 0 and st > 1 and not same_pad and rf % st == 0 and H % st == 0 and W % st == 0 and
                C * st * st in (16, 32, 64) and (st * C) % 8 == 0 and (W * C) % 8 == 0)
         geom = _implicit_geom(H, W, C, rf, st, same_pad, s2d)
-        # pixel-shuffle data gradient (conv_gemm_impl over dz: 16 / 32 / 64 channels per tap; shuffle epilogue:
+        # pixel-shuffle data gradient (b200rl_conv_gemm over dz: 16 / 32 / 64 channels per tap; shuffle epilogue:
         # C % 16 == 0; VALID padding only)
         implicit_dgrad = i > 0 and geom is not None and not same_pad and nf in (16, 32, 64) and C % 16 == 0
         layers.append(ConvLayerPlan("explicit" if geom is None else "implicit", s2d, geom, implicit_dgrad, 1))

@@ -155,8 +155,9 @@ int b200rl_adv_stats(const float* returns, const float* values, const long long*
 
 /* PPO2 loss + gradient w.r.t. head outputs: ppo2/model.py:57-91.  stats[5] += per-sample sums of
  * {pg_loss, vf_loss, entropy, approxkl, clipfrac} (model.py:115); gradients in "sum" scaling.
- * cat_loss: Categorical (seg_off == NULL, actions [*]) or MultiCategorical (distributions.py:76-94; seg_off / nseg as
- * for cat_step, actions [*, nseg]); bern_loss: Bernoulli (distributions.py:115-128, actions float32 [*, n]). */
+ * cat_loss: Categorical (distributions.py:164-198; seg_off == NULL, actions [*]) or MultiCategorical
+ * (distributions.py:76-94,206-225; seg_off / nseg as for cat_step, actions [*, nseg]); bern_loss: Bernoulli
+ * (distributions.py:115-128,254-276, actions float32 [*, n]). */
 int b200rl_cat_loss(const float* logits, long long ld, int nA, const int* seg_off, int nseg, const float* vpred,
                     long long ldv, const long long* actions, const long long* src_idx, const float* returns,
                     const float* old_values, const float* old_neglogp, const double* adv_stats, float cliprange,
@@ -194,8 +195,9 @@ int b200rl_cast_transpose_batch(const void* jobs, int njobs, int max_rows, int m
 int b200rl_cast_f32_f16(const float* src, void* dst, long long rows, int cols, long long ld_src, long long ld_dst,
                         float scale, void* stream);
 
-/* Vector-observation encoding: common/input.py:43-63 (Box -> to_float, Discrete -> one_hot), the optional
- * clip((x - mean) / std, lo, hi) of common/policies.py:182-185, and the minibatch row gather of ppo2/ppo2.py:165.
+/* Vector-observation encoding: common/input.py:43-63 encode_observation (Box -> to_float, Discrete -> one_hot
+ * :54-55), the optional clip((x - mean) / std, lo, hi) of common/policies.py:182-185, and the minibatch row gather of
+ * ppo2/ppo2.py:165.
  * x: float32 [*, raw_dim]; out: fp16 [B, 2*in_pad] = [hi | lo] with hi = fp16(v), lo = fp16(v - hi), so the first
  * GEMM (K = 2*in_pad against [W ; W]) sees the float32 observation to 2^-22 relative (2^-25 absolute once lo is
  * fp16-subnormal, |v| < ~2^-3) instead of an fp16-rounded copy.  overflow (optional device int): set to 1 when an
@@ -272,7 +274,8 @@ int b200rl_ln_bwd(const void* du, long long ld_du, const float* z, long long ld_
                   long long ld_dz, float* dgamma, float* dbeta, long long rows, int N, float alpha, float eps,
                   void* stream);
 
-/* DQN parameter-space noise (deepq/build_graph.py:202-314), csrc/param_noise.cu.
+/* DQN parameter-space noise (deepq/build_graph.py:202-314; perturb_vars, mean_kl and the scale adaptation :258-287),
+ * csrc/param_noise.cu.
  * param_perturb: for each of njobs device records {src_off, dst_off, len, perturb} (4 x int64; max_len = the largest
  * len): dst[dst_off + i] = src[src_off + i] + (perturb ? scale_dev[0] * n : 0), float32, n ~ N(0, 1) by Box-Muller over
  * the Philox4x32-10 stream (seed, position *offset_dev), or normals[dst_off + i] when normals is given.

@@ -30,15 +30,31 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in include/b200rl.h but not exported"
 
 
-def test_binding_table_matches_header_arity():
+def test_binding_table_covers_every_header_parameter():
+    """_lib.SIGNATURES is derived from the header: one row per int-returning declaration, one ctypes type per
+    parameter, and every parameter type of the header has a mapping."""
     from baselines_b200 import _lib
     decl = _declared()
+    assert set(_lib.SIGNATURES) == set(decl) - {"b200rl_last_error", "b200rl_version"}
+    known = {ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_ulonglong, ctypes.c_float, ctypes.c_double}
     for name, argtypes in _lib.SIGNATURES.items():
-        assert name in decl, name
         nargs = len([a for a in decl[name].split(",") if a.strip() and a.strip() != "void"])
         assert nargs == len(argtypes), f"{name}: header has {nargs} args, binding has {len(argtypes)}"
-    for name in decl:
-        assert name in _lib.SIGNATURES or name in ("b200rl_last_error", "b200rl_version")
+        assert all(t in known for t in argtypes), name
+        assert decl[name].split(",")[-1].strip() == "void* stream", f"{name}: the stream is the last parameter"
+
+
+def test_binding_rows_match_hand_written_ones():
+    """Two derived rows against hand-written ones (gae_scan is the ctypes stub of INTEGRATION.md section 3), and a
+    parameter type without a mapping is refused rather than guessed."""
+    from baselines_b200 import _lib
+    p, i, ll, f, d = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_double
+    assert _lib.SIGNATURES["b200rl_gae_scan"] == [p] * 7 + [i, i, d, d, i, p]
+    assert _lib.SIGNATURES["b200rl_gemm_f16"] == [p] * 5 + [i] * 3 + [ll] * 4 + [i] * 3 + [f] + [i] * 5 + [p, p]
+    assert _lib._ctype("unsigned long long seed") is ctypes.c_ulonglong
+    for bad in ("size_t n", "const int n", "long n", "unsigned n"):
+        with pytest.raises(ValueError):
+            _lib._ctype(bad)
 
 
 def test_version_and_error_string():

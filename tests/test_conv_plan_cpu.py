@@ -26,8 +26,8 @@ def test_shift_unfused_first_layer():
 
 def test_shift_span_limit_of_128_channel_inputs():
     # c1 over 8 channels of 84x84: space-to-depth gives C = 128 and a 22-row shift span, past the 16 rows
-    # conv_shift_fwd_impl takes for C = 128; nor can c1 run space-to-depth'ed as an implicit GEMM (conv_gemm_impl takes
-    # at most 64 channels per tap), so it reads 16-channel super-pixels
+    # b200rl_conv_shift_fwd takes for C = 128; nor can c1 run space-to-depth'ed as an implicit GEMM
+    # (b200rl_conv_gemm takes at most 64 channels per tap), so it reads 16-channel super-pixels
     p = _plan((84, 84, 8))
     assert not p.shift
     c1, c2, c3 = p.layers

@@ -37,7 +37,7 @@ def _sms():
 
 
 def _plan(C, N, nchunks):
-    """Chunk groups and the per-warpgroup chunk counts conv_shift_wgrad_impl and the kernel choose."""
+    """Chunk groups and the per-warpgroup chunk counts b200rl_conv_shift_wgrad and the kernel choose."""
     qw = 4 if N == 32 else (3 if C == 64 else 2)
     groups = _cdiv(nchunks, 2 * qw)
     nwg = 2 * groups

@@ -50,7 +50,7 @@ def _sms():
 
 
 def _groups(C, N, shifts, kx):
-    """Chunk groups (grid.y) and CTAs per cluster that conv_shift_wgrad_impl chooses."""
+    """Chunk groups (grid.y) and CTAs per cluster that b200rl_conv_shift_wgrad chooses."""
     qw = 2 if N == 64 else 4
     groups = _cdiv(len(shifts) * kx * (C // 64), 2 * qw)
     g = min(groups, 8)

@@ -62,7 +62,7 @@ def _density(K, target=150.0):
 
 # ------------------------------------------------------------------------------ python model of the host launch logic
 def gemm_bn(N, mn_major):
-    """N tile gemm_f16_impl picks (csrc/gemm_wgmma.cu)."""
+    """N tile b200rl_gemm_f16 picks (csrc/gemm_wgmma.cu)."""
     if mn_major:
         return 256 if (N > 128 and N % 256 == 0) else 128 if N > 64 else 64
     return 256 if (N > 128 and N % 256 == 0) else 128 if N > 64 else 64 if N > 32 else 32
