@@ -149,6 +149,10 @@ class PolicyNet:
             self.rms_names = {k: f"{scope}/{k}:0" for k in self.obs_rms}
         store.finalize()
         self._materialize()
+        # read from the final operand tensors (fuse0 re-points the first layers' w_fwd); built here, never in refresh(),
+        # which runs inside captured graphs
+        self._operand_launches = [f for t in (self.tower_pi, self.tower_vf) if t for f in t.operand_launches()]
+        self.cast_plan = ops.CastPlan(self.cast_jobs(), device)
         self.set_obs_rms()
         self.refresh()
 
@@ -258,35 +262,22 @@ class PolicyNet:
             self.head_pi.gw.zero_()
             self.head_pi.gb.zero_()
 
+    def cast_jobs(self):
+        """The casts of every fp16 operand: the towers', then the heads'.  With fuse0 the first layers' w_fwd are the
+        halves of w0cat."""
+        heads = [self.head_pi, self.head_vf] if self.tower_vf else [self.head]
+        return [j for m in [self.tower_pi, self.tower_vf] + heads if m for j in m.cast_jobs()]
+
     def refresh(self):
-        """Re-derive the fp16 operand copies from the fp32 master weights (after init / Adam / load): one batched
-        launch (ops.CastPlan) for every cast / transpose, plus the few operand kernels that are not plain casts."""
-        if getattr(self, "_cast_plan", None) is None:
-            self._cast_plan = ops.CastPlan(self._refresh_layers, self.device)
-        else:
-            self._refresh_other()
-        self._cast_plan.run()
+        """Re-derive the fp16 operand copies from the fp32 master weights (after init / Adam / load): the few operand
+        kernels that are not plain casts, then one batched launch (ops.CastPlan) for every cast / transpose."""
+        for f in self._operand_launches:
+            f()
+        self.cast_plan.run()
         if self.fuse0:                                     # the fused first layer's bias operand [b_pi | b_vf]
             N = self.tower_pi.fcs[0].N
             self.b0cat[:N].copy_(self.tower_pi.fcs[0].b)
             self.b0cat[N:].copy_(self.tower_vf.fcs[0].b)
-
-    def _refresh_other(self):
-        """Operand refreshes that are not cast_transpose jobs (they ran eagerly while the plan was recorded)."""
-        for t in (self.tower_pi, self.tower_vf):
-            if t is not None:
-                for c in t.convs:
-                    if c.wdg is not None:
-                        ops.dgrad_weights(c.w, c.wdg, c.rf, c.rf, c.C, c.nf, c.stride, c.ld_wdg)
-
-    def _refresh_layers(self):
-        self.tower_pi.refresh()
-        if self.tower_vf:
-            self.tower_vf.refresh()
-            self.head_pi.refresh()
-            self.head_vf.refresh()
-        else:
-            self.head.refresh()
 
     # ------------------------------------------------------------------------------------------
     def encode_obs(self, obs_host_or_dev):

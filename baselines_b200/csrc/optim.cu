@@ -134,12 +134,13 @@ clip_accumulate_kernel(const float* __restrict__ g, float* __restrict__ acc, lon
     acc[i] += g[i] * sc;
 }
 
-// dst16[r, c] = src[r, c]*scale (row pitch ld_dst), and optionally dstT16[c, r] = src[r, c]*scale (pitch ld_t)
-__global__ void __launch_bounds__(256)
-cast_transpose_kernel(const float* __restrict__ src, int R, int C, __half* __restrict__ dst, long long ld_dst,
-                      __half* __restrict__ dstT, long long ld_t, float scale) {
+// The 32 x 32 tile at (r0, c0) of dst16[r, c] = src[r, c]*scale (row pitch ld_dst), and optionally of
+// dstT16[c, r] = src[r, c]*scale (pitch ld_t), by a block of 256 threads
+__device__ __forceinline__ void cast_transpose_tile(const float* __restrict__ src, int R, int C,
+                                                    __half* __restrict__ dst, long long ld_dst,
+                                                    __half* __restrict__ dstT, long long ld_t, float scale, int r0,
+                                                    int c0) {
   __shared__ float tile[32][33];
-  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;   // 32 x 8
   for (int i = ty; i < 32; i += 8) {
     const int r = r0 + i, c = c0 + tx;
@@ -157,6 +158,13 @@ cast_transpose_kernel(const float* __restrict__ src, int R, int C, __half* __res
       if (r < R && c < C) dstT[(long long)c * ld_t + r] = __float2half_rn(tile[tx][i]);
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+cast_transpose_kernel(const float* __restrict__ src, int R, int C, __half* __restrict__ dst, long long ld_dst,
+                      __half* __restrict__ dstT, long long ld_t, float scale) {
+  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+  cast_transpose_tile(src, R, C, dst, ld_dst, dstT, ld_t, scale, r0, c0);
 }
 
 __global__ void __launch_bounds__(256)
@@ -187,24 +195,7 @@ cast_transpose_batch_kernel(const CastJob* __restrict__ jobs) {
   const CastJob j = jobs[blockIdx.z];
   const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
   if (c0 >= j.C || r0 >= j.R) return;
-  __shared__ float tile[32][33];
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  for (int i = ty; i < 32; i += 8) {
-    const int r = r0 + i, c = c0 + tx;
-    float x = 0.0f;
-    if (r < j.R && c < j.C) {
-      x = j.src[(long long)r * j.C + c] * j.scale;
-      if (j.dst) j.dst[(long long)r * j.ld_dst + c] = __float2half_rn(x);
-    }
-    tile[i][tx] = x;
-  }
-  __syncthreads();
-  if (j.dstT) {
-    for (int i = ty; i < 32; i += 8) {
-      const int c = c0 + i, r = r0 + tx;
-      if (r < j.R && c < j.C) j.dstT[(long long)c * j.ld_t + r] = __float2half_rn(tile[tx][i]);
-    }
-  }
+  cast_transpose_tile(j.src, j.R, j.C, j.dst, j.ld_dst, j.dstT, j.ld_t, j.scale, r0, c0);
 }
 
 // Weight operand of the implicit-GEMM data gradient of a strided convolution ("pixel shuffle" form):

@@ -63,6 +63,9 @@ class QNet:
             self.stream_lns.append(lns)
         store.finalize()
         self._materialize()
+        # built once: refresh() runs inside captured graphs
+        self._operand_launches = self.trunk.operand_launches()
+        self.cast_plan = ops.CastPlan(self.cast_jobs(), device)
         self.refresh()
 
     def _materialize(self):
@@ -89,23 +92,21 @@ class QNet:
         self.ld_dout = 64 * ((self.s_col + 1 + 63) // 64)
         self.dout = torch.zeros(cap, self.ld_dout, **f16)
 
-    def refresh(self):
-        """fp16 operand copies of every layer in one batched launch (ops.CastPlan)."""
-        if getattr(self, "_cast_plan", None) is None:
-            self._cast_plan = ops.CastPlan(self._refresh_layers, self.device)
-        else:
-            for c in self.trunk.convs:
-                if c.wdg is not None:
-                    ops.dgrad_weights(c.w, c.wdg, c.rf, c.rf, c.C, c.nf, c.stride, c.ld_wdg)
-        self._cast_plan.run()
-
-    def _refresh_layers(self):
-        self.trunk.refresh()
+    def cast_jobs(self):
+        """The casts of every fp16 operand: the trunk's, then per stream its layers' and its block of w_cat_bwd."""
+        jobs = self.trunk.cast_jobs()
         for si, layers in enumerate(self.streams):
-            for l in layers:
-                l.refresh()
+            jobs += [j for l in layers for j in l.cast_jobs()]
             l0 = layers[0]
-            ops.cast_transpose(l0.w, l0.K, l0.N, self.w_cat_bwd[:, self.cat_off[si]:], self.cat_w, None, 0)
+            jobs.append(ops.CastJob(l0.w, l0.K, l0.N, self.w_cat_bwd[:, self.cat_off[si]:], self.cat_w, None, 0, 1.0))
+        return jobs
+
+    def refresh(self):
+        """fp16 operand copies of every layer: the trunk's operand kernels that are not plain casts, then one batched
+        launch (ops.CastPlan) for every cast."""
+        for f in self._operand_launches:
+            f()
+        self.cast_plan.run()
 
     def encode(self, obs, idx=None):
         """-> (x, src_idx) in the trunk's input format."""
@@ -215,12 +216,11 @@ class StreamCopy:
                 mine.append(c)
             self.streams.append(mine)
         self.out = torch.zeros_like(q.out)
-        self.cast = ops.CastPlan(self._cast_layers, dev)
+        self.cast = ops.CastPlan(self.cast_jobs(), dev)
 
-    def _cast_layers(self):
-        for layers in self.streams:
-            for c in layers:
-                ops.cast_transpose(c.w, c.K, c.N, None, 0, c.w_fwd, c.Kf)
+    def cast_jobs(self):
+        """The casts of the copy's fp16 operands: the forward operands w_fwd (the copy has no backward)."""
+        return [ops.CastJob(c.w, c.K, c.N, None, 0, c.w_fwd, c.Kf, 1.0) for layers in self.streams for c in layers]
 
     def export_tf(self):
         host = self.params.cpu().numpy()

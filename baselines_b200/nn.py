@@ -6,6 +6,7 @@ Mirrors (by behaviour, not by code) the layer primitives of the reference:
   nature_cnn / mlp / conv_only      baselines/common/models.py:15-26, 74-103, 221-249
 All math runs in hand-written CUDA (ops.*); torch here only allocates memory and provides streams.
 """
+import functools
 import math
 from collections import OrderedDict, namedtuple
 
@@ -171,10 +172,12 @@ class Linear:
         self.w_fwd = torch.zeros(self.N, self.Kf, dtype=torch.float16, device=dev)
         self.w_bwd = torch.zeros(self.K, self.Np, dtype=torch.float16, device=dev)
 
-    def refresh(self):
-        ops.cast_transpose(self.w, self.K, self.N, self.w_bwd, self.Np, self.w_fwd, self.Kf, scale=self.in_scale)
+    def cast_jobs(self):
+        """The casts that derive w_bwd and w_fwd (both halves of a split_in one) from the fp32 master weight."""
+        jobs = [ops.CastJob(self.w, self.K, self.N, self.w_bwd, self.Np, self.w_fwd, self.Kf, self.in_scale)]
         if self.split_in:
-            ops.cast_transpose(self.w, self.K, self.N, None, 0, self.w_fwd[:, self.Kp:], self.Kf, scale=self.in_scale)
+            jobs.append(ops.CastJob(self.w, self.K, self.N, None, 0, self.w_fwd[:, self.Kp:], self.Kf, self.in_scale))
+        return jobs
 
     def forward(self, x, ldx, M, out, ldo, mode=ops.MODE_F16_ACT, act=None):
         K = self.Kp + self.K if self.split_in else self.K
@@ -300,10 +303,13 @@ class Conv(Linear):
             self.wdg = torch.zeros(self.stride * self.stride * self.C, self.ld_wdg, dtype=torch.float16,
                                    device=self.store.device)
 
-    def refresh(self):
-        super().refresh()
-        if self.wdg is not None:
-            ops.dgrad_weights(self.w, self.wdg, self.rf, self.rf, self.C, self.nf, self.stride, self.ld_wdg)
+    def operand_launches(self):
+        """The operand kernels that are not casts, as calls without arguments: the pixel-shuffle data-gradient weights
+        wdg."""
+        if self.wdg is None:
+            return []
+        return [functools.partial(ops.dgrad_weights, self.w, self.wdg, self.rf, self.rf, self.C, self.nf, self.stride,
+                                  self.ld_wdg)]
 
     def fwd_implicit(self, x, B, out):
         H, W, C, R, S, sh, sw, pt, pl = self.geom
@@ -369,9 +375,15 @@ class LSTM:
         self.dh = torch.zeros(cap, H, **f16)              # d loss / d h_t, written by the heads' data gradient
         self.dz = torch.zeros(cap, 4 * H, **f16)
 
+    def cast_jobs(self):
+        """wx's casts, then wh16 = fp16(wh) and whT16 = fp16(wh^T)."""
+        return self.wx.cast_jobs() + [ops.CastJob(self.wh, self.H, 4 * self.H, self.wh16, 4 * self.H, self.whT16, self.H,
+                                                  1.0)]
+
     def refresh(self):
-        self.wx.refresh()
-        ops.cast_transpose(self.wh, self.H, 4 * self.H, self.wh16, 4 * self.H, self.whT16, self.H)
+        """Eager operand refresh, one launch per cast."""
+        for j in self.cast_jobs():
+            ops.cast_transpose(*j)
 
     def forward(self, x, ldx, seq, train=True):
         """x: [T*B, *] fp16 input rows (time-major).  train=False: only h and the state (acting / value passes)."""
@@ -658,12 +670,6 @@ class Tower:
         self.wd = [None] + [torch.zeros(g["Cg"], g["k"] * g["k"] * c.nf, **f16) for c, g in zip(cv[1:], self.sg[1:])]
         self.flat = cv[-1].OH * cv[-1].OW * cv[-1].nf
 
-    def _refresh_shift(self):
-        for c, g, wd in zip(self.convs[1:], self.sg[1:], self.wd[1:]):
-            taps, Cg, nf = g["k"] * g["k"], g["Cg"], c.nf
-            for t in range(taps):                      # wd[:, t*nf:(t+1)*nf] = fp16(W[t*Cg:(t+1)*Cg, :])
-                ops.cast_transpose(c.w[t * Cg:(t + 1) * Cg], Cg, nf, wd[:, t * nf:], taps * nf, None, 0)
-
     def _forward_shift(self, x, B, src_idx, masks=True):
         cv, sg = self.convs, self.sg
         c0 = cv[0]
@@ -710,13 +716,30 @@ class Tower:
                                smap=smap, act=ops.ACT_RELU, dact=True, tag="dgrad." + c.name,
                                saved_bits=self.hbits[i - 1], useful_rows=B * c.OH * c.OW)
 
-    def refresh(self):
-        for l in self.layers:
-            l.refresh()
+    def cast_jobs(self):
+        """The casts of the tower's fp16 operands: its layers', the shift-GEMM data-gradient tap blocks wd, the LSTM's.
+        They read the operand tensors as they are when called."""
+        jobs = [j for l in self.layers for j in l.cast_jobs()]
         if self.convs and self.shift_mode:
-            self._refresh_shift()
+            for c, g, wd in zip(self.convs[1:], self.sg[1:], self.wd[1:]):
+                taps, Cg, nf = g["k"] * g["k"], g["Cg"], c.nf
+                # wd[:, t*nf:(t+1)*nf] = fp16(W[t*Cg:(t+1)*Cg, :])
+                jobs += [ops.CastJob(c.w[t * Cg:(t + 1) * Cg], Cg, nf, wd[:, t * nf:], taps * nf, None, 0, 1.0)
+                         for t in range(taps)]
         if self.lstm is not None:
-            self.lstm.refresh()
+            jobs += self.lstm.cast_jobs()
+        return jobs
+
+    def operand_launches(self):
+        """The convs' operand kernels that are not casts (Conv.operand_launches)."""
+        return [f for c in self.convs for f in c.operand_launches()]
+
+    def refresh(self):
+        """Eager operand refresh: the launches a network's refresh makes for this tower, with one launch per cast."""
+        for f in self.operand_launches():
+            f()
+        for j in self.cast_jobs():
+            ops.cast_transpose(*j)
 
     # x: uint8 [*,H,W,C] images (cnn) or fp16 [*, in_pad] rows (mlp); src_idx gathers samples from it
     def encode(self, x, B, src_idx=None):

@@ -3,6 +3,8 @@
 Every function launches hand-written sm_90a kernels from libb200rl.so; nothing here computes with
 torch ops (torch is plumbing: allocation, streams, torch.distributed).
 """
+from collections import namedtuple
+
 import torch
 
 from . import _lib
@@ -345,31 +347,25 @@ def clip_accumulate(g, acc, clip, weight, sumsq_buf):
               _ptr(sumsq_buf), _stream(), label="clip_accumulate", nbytes=12.0 * g.numel())
 
 
-_cast_recording = None      # list of jobs while a CastPlan is being recorded
+CastJob = namedtuple("CastJob", "src R C dst ld_dst dstT ld_t scale")
+CastJob.__doc__ = """One fp32 -> fp16 operand cast (struct CastJob of csrc/optim.cu): dst[r, c] = fp16(src[r, c] * scale)
+(row pitch ld_dst) and dstT[c, r] likewise (row pitch ld_t) for the contiguous float32 [R, C] src; dst or dstT may be
+None.  The fields are cast_transpose's arguments, in its order."""
 
 
 def cast_transpose(src, R, C, dst, ld_dst, dstT, ld_t, scale=1.0):
     _chk(src, torch.float32, "src")
-    if _cast_recording is not None:
-        _cast_recording.append((src, int(R), int(C), dst, int(ld_dst), dstT, int(ld_t), float(scale)))
-        return
     _lib.call("b200rl_cast_transpose", _ptr(src), int(R), int(C), _ptr(dst), int(ld_dst), _ptr(dstT), int(ld_t),
               float(scale), _stream())
 
 
 class CastPlan:
-    """The fp16 operand refresh of a whole network (every cast_transpose its layers issue) as ONE launch: the calls are
-    recorded once into a device table of jobs (pointers are fixed for the life of the network)."""
+    """A list of CastJobs (the fp16 operand casts of a whole network) as ONE launch: a device table of the jobs, built
+    once.  Building it copies to the device, so it cannot happen inside a graph capture; running it can."""
 
-    def __init__(self, fn, device):
-        global _cast_recording
+    def __init__(self, jobs, device):
         import numpy as np
-        _cast_recording = []
-        try:
-            fn()
-            jobs = _cast_recording
-        finally:
-            _cast_recording = None
+        jobs = list(jobs)
         self.n = len(jobs)
         self.keep = jobs                                   # keeps the tensors (and their storage) alive
         rec = np.zeros(max(self.n, 1), dtype=np.dtype([("src", "<u8"), ("dst", "<u8"), ("dstT", "<u8"), ("ld_dst", "<i8"),
@@ -377,11 +373,12 @@ class CastPlan:
                                                         ("pad", "<i4")]))
         assert rec.dtype.itemsize == 56
         for i, (src, Rr, Cc, dst, ld_dst, dstT, ld_t, scale) in enumerate(jobs):
+            _chk(src, torch.float32, "src")
             rec[i] = (src.data_ptr(), 0 if dst is None else dst.data_ptr(), 0 if dstT is None else dstT.data_ptr(),
                       ld_dst, ld_t, Rr, Cc, scale, 0)
         self.table = torch.from_numpy(rec.view(np.uint8).copy()).to(device)
-        self.max_r = max([j[1] for j in jobs], default=1)
-        self.max_c = max([j[2] for j in jobs], default=1)
+        self.max_r = max([j.R for j in jobs], default=1)
+        self.max_c = max([j.C for j in jobs], default=1)
 
     def run(self):
         if self.n:
