@@ -182,6 +182,17 @@ def with_q_norms(params, n_hidden=1, scope="deepq/q_func"):
     return out
 
 
+def randomise_norms(params, rng):
+    """gamma = 1, beta = 0 would leave a network blind to both (and to a norm credited to its neighbour): gamma drawn
+    from U(0.5, 1.5), beta from N(0, 0.3^2), in place and in key order, as float32."""
+    for k in params:
+        if k.endswith("gamma:0"):
+            params[k] = rng.uniform(0.5, 1.5, np.shape(params[k])).astype(np.float32)
+        elif k.endswith("beta:0") and "LayerNorm" in k:
+            params[k] = (rng.randn(*np.shape(params[k])) * 0.3).astype(np.float32)
+    return params
+
+
 # ---------------------------------------------------------------------------------------------- parameter-space noise
 class ParamNoiseState:
     """The act-call state machine of deepq/build_graph.py:290-313 in float32: sticky eps and threshold, and the scale

@@ -6,6 +6,8 @@ primitives (nature_cnn, encode_observation, the distributions, the global-norm c
   lstm_cell_seq           a2c/utils.py:84-97 lstm() over [nsteps] steps of [nenv] rows (batch_to_seq env-major)
   recurrent_forward       policies.py:41-64 on the recurrent latent, rows env-major (row e * nsteps + t)
   RecurrentPPO2Oracle     ppo2/model.py:133-158 train() with states and masks (ppo2.py:167-180 minibatches)
+  lstm_steps              the cell over time-major rows from the input projection, keeping gates, c and masked h_{t-1}
+  lstm_steps_backward     its BPTT (d loss / d pre-activation gates), as the sequence kernels of csrc/lstm.cu compute it
 
 Gradients come from torch.autograd (the oracle only); float64 by default."""
 import math
@@ -144,3 +146,52 @@ def lstm_numpy_loop(xs, ms, s, wx, wh, b):
                 h[e, j] = sig(z[2]) * math.tanh(c[e, j])
                 out[e, t, j] = h[e, j]
     return out, np.concatenate([c, h], 1)
+
+
+def _sig(x):
+    return 1.0 / (1.0 + np.exp(-x))
+
+
+def lstm_steps(xg, wh, masks, s0, T, B, H, mistake=None):
+    """a2c/utils.py lstm() over time-major rows (row t*B + b), numpy float64, with what a backward needs: returns
+    (h, c, gates [i | f | o | u], masked h_{t-1}, final state [c | h]).  mistake: 'mask_after' (reset after the
+    step), 'swap_fi'."""
+    xg = xg.reshape(T, B, 4 * H)
+    c, h = s0[:, :H].copy(), s0[:, H:].copy()
+    hs, cs, gs, hps = [], [], [], []
+    for t in range(T):
+        keep = (1.0 - masks[t])[:, None]
+        if mistake != "mask_after":
+            c, h = c * keep, h * keep
+        hps.append(h)
+        z = xg[t] + h @ wh
+        i, f, o, u = _sig(z[:, :H]), _sig(z[:, H:2 * H]), _sig(z[:, 2 * H:3 * H]), np.tanh(z[:, 3 * H:])
+        if mistake == "swap_fi":
+            i, f = f, i
+        c = f * c + i * u
+        h = o * np.tanh(c)
+        if mistake == "mask_after":
+            c, h = c * keep, h * keep
+        hs.append(h), cs.append(c), gs.append(np.concatenate([i, f, o, u], 1))
+    return (np.concatenate(hs), np.concatenate(cs), np.concatenate(gs), np.concatenate(hps),
+            np.concatenate([c, h], 1))
+
+
+def lstm_steps_backward(dh, gates, cs, masks, s0, wh, T, B, H, mistake=None):
+    """BPTT of lstm_steps: dz [T*B, 4H].  mistake: 'no_carry' (drops the recurrent dh)."""
+    dh, gates, cs = dh.reshape(T, B, H), gates.reshape(T, B, 4 * H), cs.reshape(T, B, H)
+    dz = np.zeros((T, B, 4 * H))
+    dc = np.zeros((B, H))
+    carry = np.zeros((B, H))
+    for t in reversed(range(T)):
+        keep = (1.0 - masks[t])[:, None]
+        i, f, o, u = (gates[t][:, k * H:(k + 1) * H] for k in range(4))
+        cp = (cs[t - 1] if t > 0 else s0[:, :H]) * keep
+        d = dh[t] + (0 if mistake == "no_carry" else carry)
+        tc = np.tanh(cs[t])
+        dc = dc + d * o * (1 - tc * tc)
+        dz[t] = np.concatenate([dc * u * i * (1 - i), dc * cp * f * (1 - f), d * tc * o * (1 - o),
+                                dc * i * (1 - u * u)], 1)
+        carry = (dz[t] @ wh.T) * keep
+        dc = dc * f * keep
+    return dz.reshape(T * B, 4 * H)

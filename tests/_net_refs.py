@@ -16,11 +16,22 @@ rnd=True evaluates what the kernels evaluate:
   * ReLU decisions taken from `masks` (name -> 0/1 tensor shaped like the pre-activation) where the caller supplies
     them, e.g. from the kernels' own stored activations; for a tanh layer `masks[name]` is the stored activation itself,
     which replaces the mirror's in the forward (the backward keeps the mirror's 1 - s^2);
-  * mlp observations kept in float32: the encoder's fp16 hi/lo split loses at most max(2^-22 |v|, 2^-25).
+  * a ReLU layer's stored activation taken from `stored` (name -> the kernels' fp16 values) where the caller supplies
+    it, as the forward value only (straight-through): the kernels round an fp32 sum and the mirror a float64 one, so
+    the two can differ by one fp16 rounding, and under a recurrence (cnn_lstm's latent into the cell) such a flip
+    carries into every later step.  The caller checks that both agree within that rounding first;
+  * mlp observations kept in float32: the encoder's fp16 hi/lo split loses at most max(2^-22 |v|, 2^-25);
+  * LayerNorm: z stays fp32 (exact here), the output activation y is stored fp16, d loss / d z is stored fp16;
+  * LSTM: Wx and Wh fp16; xg, c and the gates fp32 (exact here); h and the masked h_{t-1} stored fp16; dz rounded to
+    fp16 where the weight-gradient / data-gradient GEMMs read it, unrounded in the recurrent carry.
 
 absolute=True evaluates the same network on |x|, |W|, |b| and |seed| with the ReLU masks and stored tanh activations of
-a signed run (`ref_acts`): a tanh layer outputs |s| and passes the gradient through |1 - s^2|.  Its outputs and
-gradients are the scale S of the error bound (tests/_refs.py), the network analogue of |A| @ |B|.
+a signed run (`ref_acts`): a tanh layer outputs |s| and passes the gradient through |1 - s^2|; a LayerNorm outputs
+|gamma| (|xhat| + |J| z) + |beta| (its size plus the error z carries into it) and passes the gradient through |J|^T, the
+magnitudes of its Jacobian's terms.  The LSTM cell's forward outputs |h| of the signed run only: it does not carry the
+size of |x| |Wx| + |h_{t-1}| |Wh| into h, so the cell's forward rounding error is not in S and the fitted per-tensor
+factor g of the GPU tests absorbs it; its backward takes every factor of the BPTT by magnitude.  Outputs and gradients
+are the scale S of the error bound (tests/_refs.py), the network analogue of |A| @ |B|.
 """
 import collections
 import types
@@ -28,6 +39,8 @@ import types
 import numpy as np
 import torch
 
+import _layer_norm_refs as LN
+import _lstm_oracle as LO
 import _refs as R
 
 NATURE_CONVS = (("c1", 32, 8, 4), ("c2", 64, 4, 2), ("c3", 64, 3, 1))   # common/models.py:21-24
@@ -119,11 +132,77 @@ class _GradRound(torch.autograd.Function):
         return g.half().double()
 
 
+class _AbsLayerNorm(torch.autograd.Function):
+    """Absolute mode of a LayerNorm at the signed run's xhat and rstd, with |J| the magnitudes of the terms of
+    J = rstd (I - 1/N - xhat xhat^T / N): u = |gamma| (|xhat| + |J| z) + |beta| for the absolute run's z (the size of
+    xhat plus the error z carries into it); the backward passes |J|^T (|gamma| g) to z, and g (|xhat| + |J| z), g to
+    gamma and beta."""
+
+    @staticmethod
+    def forward(ctx, z, gamma, beta, xhat, rstd):
+        ax = xhat.abs()
+        scale = ax + rstd * (z + z.mean(1, keepdim=True) + ax * (ax * z).mean(1, keepdim=True))
+        ctx.save_for_backward(gamma, ax, rstd, scale)
+        return gamma * scale + beta
+
+    @staticmethod
+    def backward(ctx, g):
+        gamma, ax, rstd, scale = ctx.saved_tensors
+        gg = gamma * g
+        dz = rstd * (gg + gg.mean(1, keepdim=True) + ax * (gg * ax).mean(1, keepdim=True))
+        return dz, (g * scale).sum(0), g.sum(0), None, None
+
+
+class _LSTMSeq(torch.autograd.Function):
+    """h rows [T*E, H] of the cell (tests/_lstm_oracle.py lstm_steps) from the input projection xg [T*E, 4H], Wh, masks
+    [T, E] and start states [E, 2H]; the backward is lstm_steps_backward.  The recurrent carry keeps dz unrounded (the
+    kernel holds it in fp32); with rnd the gradients of xg (-> Wx, b, x) and Wh take dz rounded to fp16 and Wh's takes
+    the stored fp16 masked h_{t-1}, as the weight-gradient GEMMs read them.  With ref (the signed run's gates, c,
+    masked h_{t-1}) the absolute network: |h| of the signed run forward (see the module docstring), every factor of
+    the BPTT taken by magnitude.  unmasked_dwh
+    (mutant): dWh from h_{t-1} before the mask."""
+
+    @staticmethod
+    def forward(ctx, xg, wh, masks, s0, rnd, ref, unmasked_dwh):
+        T, E = masks.shape
+        H = wh.shape[0]
+        np_ = lambda t: t.detach().cpu().numpy()
+        if ref is None:
+            h, cs, gates, hps, _ = LO.lstm_steps(np_(xg), np_(wh), masks, s0, T, E, H)
+            prev = np.concatenate([s0[None, :, H:], h.reshape(T, E, H)[:-1]]).reshape(T * E, H)
+        else:
+            h, cs, gates, hps, prev = ref
+            h, cs, gates = np.abs(h), np.abs(cs), gates.copy()
+            gates[:, 3 * H:] = np.abs(gates[:, 3 * H:])
+            s0 = np.abs(s0)
+        ctx.saved = (gates, cs, hps, prev, masks, s0, np_(wh), rnd, ref is not None, unmasked_dwh)
+        ctx.dev = xg.device
+        ctx.record = (h, cs, gates, hps, prev)
+        return torch.as_tensor(h, device=xg.device)
+
+    @staticmethod
+    def backward(ctx, dh):
+        gates, cs, hps, prev, masks, s0, wh, rnd, absolute, unmasked_dwh = ctx.saved
+        T, E = masks.shape
+        H = wh.shape[0]
+        dhn = dh.detach().cpu().numpy()
+        dz = LO.lstm_steps_backward(np.abs(dhn) if absolute else dhn, gates, cs, masks, s0, wh, T, E, H)
+        a = np.abs(prev if unmasked_dwh else hps) if absolute else (prev if unmasked_dwh else hps)
+        if rnd:
+            dz, a = _f16(dz), _f16(a)
+        t = lambda v: torch.as_tensor(v, device=ctx.dev)
+        return t(dz), t(a.T @ dz), None, None, None, None, None
+
+
+def _f16(a):
+    return np.asarray(a).astype(np.float16).astype(np.float64)
+
+
 class _Net:
     """Evaluation state of one mirror run: rounding, masks, the signed run's activations (absolute mode), records."""
 
-    def __init__(self, rnd, masks, absolute, ref_acts, no_dact):
-        self.rnd, self.masks, self.absolute = rnd, masks or {}, absolute
+    def __init__(self, rnd, masks, absolute, ref_acts, no_dact, stored=None):
+        self.rnd, self.masks, self.absolute, self.stored = rnd, masks or {}, absolute, stored or {}
         self.ref_acts, self.no_dact = ref_acts or {}, set(no_dact or ())
         self.pres, self.acts = collections.OrderedDict(), collections.OrderedDict()
 
@@ -146,13 +225,42 @@ class _Net:
             a = pre * m
             if name in self.no_dact:                    # mutant: the mask's derivative left out of the backward
                 a = pre + (a - pre).detach()
-            return a + (a.half().double() - a).detach() if self.rnd else a
+            a = a + (a.half().double() - a).detach() if self.rnd else a
+            st = self.stored.get(name)
+            return a if st is None else a + (st.double() - a).detach()
         s = _StoredTanh.apply(pre, self.rnd, name in self.no_dact)
         m = self.masks.get(name)
         if m is not None:                               # the kernels' stored activation (forward value only)
             s = s + (m.double() - s).detach()
         self.acts[name] = s.detach()
         return s
+
+    def ln(self, scope, z, gamma, beta):
+        """LayerNorm `scope` over a fully connected layer's fp32 pre-activation z: u = gamma * xhat + beta
+        (_layer_norm_refs.ln_torch).  With rnd the kernels' stored d loss / d z is fp16; z itself stays fp32 (exact
+        here).  The caller passes u to act(), which rounds the stored activation and d loss / d u."""
+        if self.rnd:
+            z = _GradRound.apply(z)
+        if self.absolute:
+            return _AbsLayerNorm.apply(z, gamma, beta, *self.ref_acts[scope])
+        zd = z.detach()
+        mean = zd.mean(1, keepdim=True)
+        rstd = 1.0 / torch.sqrt(((zd - mean) ** 2).mean(1, keepdim=True) + LN.EPS)
+        self.acts[scope] = ((zd - mean) * rstd, rstd)
+        return LN.ln_torch(z, gamma, beta)
+
+    def lstm(self, name, xg, wh, seq, unmasked_dwh=False):
+        """The LSTM cell over the time-major rows of xg = x.wx + b (seq = (masks [T, E], start states [E, 2H]), numpy
+        float64).  With rnd h is stored fp16 and the heads' d loss / d h arrives in fp16."""
+        masks, s0 = seq
+        h = _LSTMSeq.apply(xg, wh, masks, s0, self.rnd, self.ref_acts.get(name) if self.absolute else None,
+                           unmasked_dwh)
+        if not self.absolute:
+            self.acts[name] = h.grad_fn.record if h.grad_fn is not None else None
+        if self.rnd:
+            h = _GradRound.apply(h)
+            h = h + (h.half().double() - h).detach()
+        return h
 
 
 def _leaves(params, first_convs, rnd, absolute, dev):
@@ -161,7 +269,7 @@ def _leaves(params, first_convs, rnd, absolute, dev):
     scale1 = torch.tensor(1.0 / 255.0, dtype=torch.float32)
     for k, v in params.items():
         t = torch.as_tensor(np.asarray(v))
-        is_w = k.endswith("/w:0") or k.endswith("/weights:0")
+        is_w = k.endswith(("/w:0", "/weights:0", "/lstm/wx:0", "/lstm/wh:0"))
         if k in first_convs:
             t = (t.float() * scale1).half().double() if rnd else t.double() / 255.0
         elif is_w and rnd:
@@ -173,10 +281,17 @@ def _leaves(params, first_convs, rnd, absolute, dev):
     return out
 
 
-def _tower(P, net, prefix, kind, x, convs=NATURE_CONVS, same=False, num_layers=2, contrib=False, ob_shape=None):
-    """Latent of one nn.Tower: cnn / conv_only convs over uint8 images [B, H, W, C] (as float64), or the tanh mlp over
-    encoded observation rows [B, in_dim]."""
+def _tower(P, net, prefix, kind, x, convs=NATURE_CONVS, same=False, num_layers=2, contrib=False, ob_shape=None,
+           seq=None, unmasked_dwh=False):
+    """Latent of one nn.Tower: cnn / conv_only convs over uint8 images [B, H, W, C] (as float64), the tanh mlp over
+    encoded observation rows [B, in_dim] (layer-normalised where P holds the norms), or the LSTM cell of lstm /
+    cnn_lstm over time-major rows (seq: see policy_ref)."""
     B = x.shape[0]
+    if kind in ("lstm", "cnn_lstm"):
+        # models.py lstm: the encoded observation straight into the cell; cnn_lstm: the NatureCNN latent
+        lat = x if kind == "lstm" else _tower(P, net, prefix, "cnn", x, ob_shape=ob_shape)
+        xg = lat @ P[f"{prefix}/lstm/wx:0"] + P[f"{prefix}/lstm/b:0"]
+        return net.lstm(f"{prefix}/lstm", xg, P[f"{prefix}/lstm/wh:0"], seq, unmasked_dwh=unmasked_dwh)
     if kind in ("cnn", "conv_only"):
         if contrib:
             names = [f"{prefix}/convnet/{'Conv' if i == 0 else f'Conv_{i}'}" for i in range(len(convs))]
@@ -192,13 +307,17 @@ def _tower(P, net, prefix, kind, x, convs=NATURE_CONVS, same=False, num_layers=2
         return net.act(f"{prefix}/fc1", flat @ P[f"{prefix}/fc1/w:0"] + P[f"{prefix}/fc1/b:0"], "relu")
     h = x
     for i in range(num_layers):
-        h = net.act(f"{prefix}/mlp_fc{i}", h @ P[f"{prefix}/mlp_fc{i}/w:0"] + P[f"{prefix}/mlp_fc{i}/b:0"], "tanh")
+        z = h @ P[f"{prefix}/mlp_fc{i}/w:0"] + P[f"{prefix}/mlp_fc{i}/b:0"]
+        ln = f"{prefix}/{LN.ln_scope(i)}"
+        if f"{ln}/gamma:0" in P:                                        # mlp(layer_norm=True), models.py:97-98
+            z = net.ln(ln, z, P[f"{ln}/gamma:0"], P[f"{ln}/beta:0"])
+        h = net.act(f"{prefix}/mlp_fc{i}", z, "tanh")
     return h
 
 
 def _first_convs(kind, prefixes, contrib=False):
     """TF names of the first conv weights (the ones that carry models.py:19's 1/255)."""
-    if kind not in ("cnn", "conv_only"):
+    if kind not in ("cnn", "conv_only", "cnn_lstm"):
         return set()
     return {f"{p}/convnet/Conv/weights:0" if contrib else f"{p}/c1/w:0" for p in prefixes}
 
@@ -218,11 +337,15 @@ def _t(a, dev):
 
 # ------------------------------------------------------------------------------------------------ PPO2 policy
 def policy_ref(params, cfg, obs, seed_pi, seed_v, rnd=False, masks=None, absolute=False, ref_acts=None, no_dact=(),
-               identity=False, dev="cpu"):
+               identity=False, seq=None, unmasked_dwh=False, stored=None, dev="cpu"):
     """PolicyNet's forward (towers, [pi | vf] heads) and d(sum(pi * seed_pi) + sum(v * seed_v)) / d(param).
 
-    cfg: dict(kind='mlp' | 'cnn', copy=value_network == 'copy', num_layers, ob_shape, scope).  obs: uint8 images (cnn)
-    or encoded observation rows (mlp, see `encode_obs`).  identity: the frozen identity head (no 'pi/w', 'pi/b').
+    cfg: dict(kind='mlp' | 'cnn' | 'lstm' | 'cnn_lstm', copy=value_network == 'copy', num_layers, ob_shape, scope).
+    obs: uint8 images (cnn, cnn_lstm) or encoded observation rows (mlp, lstm, see `encode_obs`); the recurrent networks
+    take T*E time-major rows (row t*E + e) with seq = (masks [T, E] "done before step t", start states [E, 2H]), numpy
+    float64.  identity: the frozen identity head (no 'pi/w', 'pi/b').  The norms of mlp(layer_norm=True) are used
+    wherever params holds them.  unmasked_dwh (mutant): the LSTM's dWh from h_{t-1} before the mask.  stored: ReLU
+    layers' stored activations to use as forward values (module docstring).
     Returns a namespace: pi [B, nout], v [B], pres (name -> pre-activation), acts (ReLU masks / stored tanh
     activations, for an absolute run), grads (TF name -> gradient; 'head_pi/w', 'head_pi/b' for the identity head)."""
     scope = cfg.get("scope", "ppo2_model")
@@ -230,12 +353,12 @@ def policy_ref(params, cfg, obs, seed_pi, seed_v, rnd=False, masks=None, absolut
     P = dict(params)
     P.pop(f"{scope}/pi/logstd:0", None)                          # the loss kernel's own gradient (not the network's)
     first = _first_convs(kind, [f"{scope}/pi"] + ([f"{scope}/vf"] if copy else []))
-    net = _Net(rnd, masks, absolute, ref_acts, no_dact)
+    net = _Net(rnd, masks, absolute, ref_acts, no_dact, stored)
     leaves = _leaves(P, first, rnd, absolute, dev)
     x = _t(obs, dev)
     if absolute:
         x = x.abs()
-    tw = dict(num_layers=cfg.get("num_layers", 2), ob_shape=cfg.get("ob_shape"))
+    tw = dict(num_layers=cfg.get("num_layers", 2), ob_shape=cfg.get("ob_shape"), seq=seq, unmasked_dwh=unmasked_dwh)
     lat = _tower(leaves, net, f"{scope}/pi", kind, x, **tw)
     vlat = _tower(leaves, net, f"{scope}/vf", kind, x, **tw) if copy else lat
     if identity:
@@ -301,6 +424,9 @@ def q_ref(params, cfg, obs, seed_a, seed_s=None, rnd=False, masks=None, absolute
         for j in range(len(hiddens) + 1):
             pfx = f"{scope}/{sname}/{_fc_name(j)}"
             z = h @ leaves[pfx + "/weights:0"] + leaves[pfx + "/biases:0"]
+            ln = f"{scope}/{sname}/{LN.ln_scope(j)}"
+            if j < len(hiddens) and f"{ln}/gamma:0" in leaves:        # layer_norm=True, deepq/models.py:24-25,34-35
+                z = net.ln(ln, z, leaves[f"{ln}/gamma:0"], leaves[f"{ln}/beta:0"])
             h = net.act(pfx, z, "relu" if j < len(hiddens) else None)
         outs.append(h)
     A = outs[0]
@@ -344,6 +470,26 @@ DQN_CONFIGS = {
     "mlp_disc7_dueling_h64": dict(kind="mlp", ob=("discrete", 7), hiddens=(64,), dueling=True, double_q=True),
 }
 
+# The layer-normalised and recurrent networks of tests/test_update_composition_rnn_ln_gpu.py.  Recurrent minibatches
+# are E whole environments of T steps (nlstm: the cell width).
+PPO_RNN_LN_CONFIGS = {
+    "mlp376_gauss17_copy_ln": dict(kind="mlp", ob=("box", (376,)), ac=("gauss", 17), copy=True, layer_norm=True),
+    "mlp11_cat4_shared_ln": dict(kind="mlp", ob=("box", (11,)), ac=("cat", 4), layer_norm=True),
+    "lstm_box7_gauss3_h128": dict(kind="lstm", ob=("box", (7,)), ac=("gauss", 3), nlstm=128),
+    "lstm_disc5_cat3_h64": dict(kind="lstm", ob=("discrete", 5), ac=("cat", 3), nlstm=64),
+    "cnn_lstm_cat6_h64": dict(kind="cnn_lstm", ob=("box", (84, 84, 4)), ac=("cat", 6), nlstm=64),
+    "cnn_lstm_cat6_h128": dict(kind="cnn_lstm", ob=("box", (84, 84, 4)), ac=("cat", 6), nlstm=128),
+}
+
+DQN_LN_CONFIGS = {
+    "mlp_dueling_h64_32_double_ln": dict(kind="mlp", ob=("box", (8,)), hiddens=(64, 32), dueling=True, double_q=True,
+                                         layer_norm=True),
+    "mlp_plain_h32_32_ln": dict(kind="mlp", ob=("box", (8,)), hiddens=(32, 32), dueling=False, double_q=False,
+                                layer_norm=True),
+    "conv_only_dueling_h256_ln": dict(kind="conv_only", ob=("box", (84, 84, 4)), hiddens=(256,), dueling=True,
+                                      double_q=True, layer_norm=True),
+}
+
 
 def in_dim(ob):
     """Width of the encoded observation rows (mlp) or the image shape (cnn)."""
@@ -362,6 +508,8 @@ def ppo_mirror_cfg(cfg):
 
 
 def ppo_identity(cfg):
+    if cfg["kind"] in ("lstm", "cnn_lstm"):
+        return cfg["nlstm"] == ppo_nout(cfg["ac"])
     return cfg["kind"] == "mlp" and cfg.get("num_hidden", 64) == ppo_nout(cfg["ac"])
 
 

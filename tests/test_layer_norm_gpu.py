@@ -65,7 +65,12 @@ def _fwd_bound(ref, u):
     return R16 * np.abs(ref) + 1e-5 * (1.0 + np.abs(u)) + 1e-7
 
 
-@pytest.mark.parametrize("N", [8, 64, 72, 256, 1024])
+# every (lanes per row, chunks per lane) instance of csrc/layer_norm.cu LN_DISPATCH, each with full and partial last chunks:
+# <8,1> N <= 64, <32,1> N <= 256, <32,2> N <= 512, <32,4> beyond
+LN_WIDTHS = [8, 64, 72, 256, 264, 384, 512, 520, 1000, 1024]
+
+
+@pytest.mark.parametrize("N", LN_WIDTHS)
 @pytest.mark.parametrize("rows", [1, 31, 32, 33, 1000])
 def test_ln_fwd_matches_float64(N, rows):
     z, gamma, beta, _ = _data(rows, N, seed=N + rows)
@@ -118,7 +123,7 @@ def test_large_mean_small_spread_keeps_its_variance():
     assert np.mean(np.abs(bad - ref) > bound) > 0.5
 
 
-@pytest.mark.parametrize("N", [8, 64, 72, 256, 1024])
+@pytest.mark.parametrize("N", LN_WIDTHS)
 @pytest.mark.parametrize("rows", [1, 33, 127, 128, 129, 1000])
 def test_ln_bwd_matches_float64(N, rows):
     z, gamma, _, du = _data(rows, N, seed=3 * N + rows)
@@ -141,7 +146,7 @@ def test_ln_bwd_matches_float64(N, rows):
     assert np.array_equal(dz2, dz) and np.array_equal(dg2, dg) and np.array_equal(db2, db)
 
 
-@pytest.mark.parametrize("N,lanes", [(64, 8), (256, 32)])
+@pytest.mark.parametrize("N,lanes", [(64, 8), (256, 32), (384, 32), (1000, 32)])
 def test_norm_gradients_repeat_and_follow_the_documented_order(N, lanes):
     """dgamma / dbeta are the same bits on every run, and dbeta is the float32 sum in the order csrc/layer_norm.cu
     documents (fixed 128-row slices, whatever the grid): an order that only depends on the data."""
@@ -185,12 +190,7 @@ def _mk_ppo(case, M, seed=0):
 
 def _randomise_norms(model, oparams, seed):
     """gamma = 1, beta = 0 would leave the forward blind to both: give them values, in the model and the reference."""
-    rng = np.random.RandomState(seed)
-    for k in oparams:
-        if k.endswith("gamma:0"):
-            oparams[k] = rng.uniform(0.5, 1.5, oparams[k].shape).astype(np.float32)
-        elif k.endswith("beta:0") and "LayerNorm" in k:
-            oparams[k] = (rng.randn(*oparams[k].shape) * 0.3).astype(np.float32)
+    L.randomise_norms(oparams, np.random.RandomState(seed))
     model.set_params(oparams)
 
 
@@ -319,11 +319,7 @@ def test_dqn_layer_norm_train_step_matches_float64(network, ob_shape, dtype, due
     for k in qp:
         assert np.array_equal(mp[k], qp[k]), k
     rng = np.random.RandomState(0)
-    for k in qp:                                                      # see _randomise_norms
-        if k.endswith("gamma:0"):
-            qp[k] = rng.uniform(0.5, 1.5, qp[k].shape).astype(np.float32)
-        elif k.endswith("beta:0"):
-            qp[k] = (rng.randn(*qp[k].shape) * 0.3).astype(np.float32)
+    L.randomise_norms(qp, rng)
     obs = (lambda: rng.randint(0, 256, (B,) + ob_shape).astype(np.uint8)) if dtype == np.uint8 else \
           (lambda: (rng.randn(B, *ob_shape) * 2.0).astype(np.float32))
     dev = model.device

@@ -1,14 +1,18 @@
 """CPU: the float64 network mirror (tests/_net_refs.py), rounding off, equals the CPU oracle (oracle/nets.py) run in
-float64 on every network of tests/test_update_composition_gpu.py: the same head outputs, and the same gradient of
-every TF variable when it is seeded with the oracle's own d(loss)/d(head) -- from ppo_loss / the DQN Huber loss where
-the oracle has that network, from a random seed on the head outputs otherwise.  This ties the mirror the GPU test
-trusts to the restated reference."""
+float64 on every network of tests/test_update_composition_gpu.py and tests/test_update_composition_rnn_ln_gpu.py: the
+same head outputs, and the same gradient of every TF variable when it is seeded with the oracle's own d(loss)/d(head)
+-- from ppo_loss / the DQN Huber loss where the oracle has that network, from a random seed on the head outputs
+otherwise.  The layer-normalised networks run the oracle with tests/_layer_norm_refs.py's norms, the recurrent ones
+against tests/_lstm_oracle.py (env-major rows there, time-major in the mirror).  This ties the mirror the GPU tests
+trust to the restated reference."""
 import math
 
 import numpy as np
 import pytest
 import torch
 
+import _layer_norm_refs as L
+import _lstm_oracle as LO
 import _net_refs as N
 from oracle import nets
 
@@ -24,7 +28,7 @@ def _close(got, want, what):
 
 
 def _ppo_case(name, B=7, seed=0):
-    cfg = N.PPO_CONFIGS[name]
+    cfg = N.PPO_CONFIGS[name] if name in N.PPO_CONFIGS else N.PPO_RNN_LN_CONFIGS[name]
     rng = np.random.RandomState(seed)
     okind = cfg["ob"][0]
     if cfg["kind"] == "cnn":
@@ -43,9 +47,12 @@ def _ppo_case(name, B=7, seed=0):
     params = nets.init_policy_params(cfg["kind"], N.in_dim(cfg["ob"]), "box" if cfg["ac"][0] == "gauss" else "discrete",
                                      nout, value_network="copy" if cfg.get("copy") else None, seed=seed, **net_kw)
     # non-zero biases, so that a missing bias term shows
+    if cfg.get("layer_norm"):
+        params = L.randomise_norms(L.with_policy_norms(params, num_layers=cfg.get("num_layers", 2)), rng)
     params = {k: (v + 0.1 * rng.randn(*v.shape).astype(np.float32)) if k.endswith("/b:0") else v
               for k, v in params.items()}
     return cfg, params, x, nout, rng
+
 
 
 def _oracle_policy(tp, cfg, x):
@@ -125,7 +132,7 @@ def test_policy_mirror_seeded_by_ppo_loss_matches_oracle_autograd(name, monkeypa
 
 
 def _dqn_case(name, B=7, seed=0):
-    cfg = N.DQN_CONFIGS[name]
+    cfg = N.DQN_CONFIGS[name] if name in N.DQN_CONFIGS else N.DQN_LN_CONFIGS[name]
     rng = np.random.RandomState(seed)
     nA = 6
     if cfg["kind"] != "mlp":
@@ -136,16 +143,21 @@ def _dqn_case(name, B=7, seed=0):
         x = (rng.randn(B, *cfg["ob"][1]) * 2).astype(np.float32).astype(np.float64)
     params = nets.init_q_params(cfg["kind"], N.in_dim(cfg["ob"]), nA, hiddens=cfg["hiddens"], dueling=cfg["dueling"],
                                 seed=seed)
+    if cfg.get("layer_norm"):
+        params = L.randomise_norms(L.with_q_norms(params, len(cfg["hiddens"])), rng)
     params = {k: (v + 0.1 * rng.randn(*v.shape).astype(np.float32)) if ("/b:0" in k or "biases" in k) else v
               for k, v in params.items()}
     return cfg, params, x, nA, rng
 
 
-@pytest.mark.parametrize("name", list(N.DQN_CONFIGS))
+@pytest.mark.parametrize("name", list(N.DQN_CONFIGS) + list(N.DQN_LN_CONFIGS))
 def test_q_mirror_seeded_by_td_loss_matches_oracle_autograd(name, monkeypatch):
     """q(s) and d(Huber TD loss)/d(param) of the oracle's DQN step == the mirror's A, S and its gradient seeded with
-    d loss / dA = dq - mean(dq), d loss / dS = sum(dq) (dueling) or dq."""
+    d loss / dA = dq - mean(dq), d loss / dS = sum(dq) (dueling) or dq.  The layer-normalised streams run the oracle
+    with _layer_norm_refs.q_forward."""
     cfg, params, x, nA, rng = _dqn_case(name)
+    if cfg.get("layer_norm"):
+        monkeypatch.setattr(nets, "q_forward", L.q_forward)
     B = x.shape[0]
     oracle = nets.DQNOracle(params, cfg["kind"], 0.99, n_hidden=len(cfg["hiddens"]), dueling=cfg["dueling"],
                             double_q=cfg["double_q"], dtype=torch.float64)
@@ -172,6 +184,7 @@ def test_q_mirror_seeded_by_td_loss_matches_oracle_autograd(name, monkeypatch):
     else:
         da, ds = dq, None
     ref = N.q_ref(params, N.dqn_mirror_cfg(cfg), x, da, ds)
+    assert list(ref.grads) == list(params)                       # TF names, in creation order
     qm = ref.A if not cfg["dueling"] else ref.S[:, None] + ref.A - ref.A.mean(1, keepdim=True)
     _close(qm, q.detach(), f"{name} q")
     for k, t in oracle.tp.items():
@@ -206,3 +219,94 @@ def test_policy_mirror_takes_stored_tanh_activations(name):
     moved = dict(tanh_acts, **{last: tanh_acts[last] * 0.5})
     other = N.policy_ref(params, mcfg, x, z, zv, rnd=True, masks=moved, identity=ident)
     assert not torch.equal(other.pi, ref.pi)
+
+
+LN_PPO = [n for n, c in N.PPO_RNN_LN_CONFIGS.items() if c.get("layer_norm")]
+RNN_PPO = [n for n, c in N.PPO_RNN_LN_CONFIGS.items() if "nlstm" in c]
+
+
+@pytest.mark.parametrize("name", LN_PPO)
+def test_layer_norm_policy_mirror_matches_oracle(name, monkeypatch):
+    """mlp(layer_norm=True): the mirror against oracle/nets.py with _layer_norm_refs.mlp, every norm's gamma and beta
+    included, under the reference's names and in its creation order."""
+    cfg, params, x, nout, rng = _ppo_case(name)
+    assert sum("LayerNorm" in k for k in params) == 4 * (2 if cfg.get("copy") else 1)
+    monkeypatch.setattr(nets, "mlp", L.mlp)
+    tp = nets.to_torch(params, torch.float64, requires_grad=True)
+    pi, v = _oracle_policy(tp, cfg, torch.as_tensor(x))
+    dpi, dv = rng.randn(*pi.shape), rng.randn(*v.shape)
+    ((pi * torch.as_tensor(dpi)).sum() + (v * torch.as_tensor(dv)).sum()).backward()
+    _check_policy(name, cfg, params, x, tp, pi, v, dpi, dv)
+    ref = N.policy_ref(params, N.ppo_mirror_cfg(cfg), x, dpi, dv)
+    assert list(ref.grads) == [k for k in params if not k.endswith("logstd:0")]
+
+
+def _recurrent_case(name, T, E, seed=0):
+    """Parameters, env-major raw observations / masks (the oracle's rows e*T + t), start states, and the time-major
+    order of the mirror's rows."""
+    cfg = N.PPO_RNN_LN_CONFIGS[name]
+    rng = np.random.RandomState(seed)
+    (ok, oa), nout, H = cfg["ob"], N.ppo_nout(cfg["ac"]), cfg["nlstm"]
+    onehot = oa if ok == "discrete" else 0
+    params = LO.init_recurrent_params(cfg["kind"], oa if ok == "box" else (), "box" if cfg["ac"][0] == "gauss" else
+                                      "discrete", nout, nlstm=H, seed=seed, onehot_n=onehot)
+    params = {k: (v + 0.1 * rng.randn(*v.shape).astype(np.float32)) if k.endswith("/b:0") else v
+              for k, v in params.items()}
+    n = T * E
+    if cfg["kind"] == "cnn_lstm":
+        obs = rng.randint(0, 256, (n,) + oa).astype(np.uint8)
+    elif onehot:
+        obs = rng.randint(0, onehot, n)
+    else:
+        obs = (rng.randn(n, *oa) * 2).astype(np.float32)
+    masks = (rng.rand(n) < 0.3).astype(np.float64)
+    states = rng.randn(E, 2 * H) * 0.5
+    tm = np.array([e * T + t for t in range(T) for e in range(E)])
+    return cfg, params, obs, masks, states, tm, onehot, rng
+
+
+def _mirror_rows(cfg, obs, onehot):
+    if cfg["kind"] == "cnn_lstm":
+        return obs
+    return N.encode_obs(obs.astype(np.float32), onehot_n=onehot)
+
+
+@pytest.mark.parametrize("name", RNN_PPO)
+def test_recurrent_policy_mirror_matches_lstm_oracle(name):
+    """lstm / cnn_lstm: the mirror over time-major rows with per-row masks and per-environment start states against
+    _lstm_oracle.recurrent_forward (a2c/utils.py lstm() through autograd), forward and every TF variable's gradient."""
+    T, E = 4, 3
+    cfg, params, obs, masks, states, tm, onehot, rng = _recurrent_case(name, T, E)
+    tp = nets.to_torch(params, torch.float64, requires_grad=True)
+    pi, _, v, _ = LO.recurrent_forward(tp, cfg["kind"], torch.as_tensor(obs), masks, states, E, onehot_n=onehot)
+    dpi, dv = rng.randn(*pi.shape), rng.randn(*v.shape)
+    ((pi * torch.as_tensor(dpi)).sum() + (v * torch.as_tensor(dv)).sum()).backward()
+    seq = (masks.reshape(E, T).T.copy(), states)
+    ref = N.policy_ref(params, N.ppo_mirror_cfg(cfg), _mirror_rows(cfg, obs[tm], onehot), dpi[tm], dv[tm], seq=seq)
+    _close(ref.pi, pi.detach()[tm], f"{name} pi")
+    _close(ref.v, v.detach()[tm], f"{name} v")
+    assert list(ref.grads) == [k for k in params if not k.endswith("logstd:0")]
+    for k, t in tp.items():
+        if not k.endswith("logstd:0"):
+            _close(ref.grads[k], t.grad, f"{name} d/d {k}")
+
+
+@pytest.mark.parametrize("name", ["lstm_box7_gauss3_h128", "mlp11_cat4_shared_ln"])
+def test_absolute_mirror_bounds_the_signed_one(name):
+    """The absolute network (the error scale S) through a LayerNorm or the LSTM cell: every output and gradient is at
+    least as large as the signed run's, element by element."""
+    if name in RNN_PPO:
+        T, E = 5, 3
+        cfg, params, obs, masks, states, tm, onehot, rng = _recurrent_case(name, T, E, seed=3)
+        x, kw = _mirror_rows(cfg, obs[tm], onehot), dict(seq=(masks.reshape(E, T).T.copy(), states))
+    else:
+        cfg, params, x, nout, rng = _ppo_case(name, B=9, seed=3)
+        kw = {}
+    mcfg = N.ppo_mirror_cfg(cfg)
+    n, nout = len(x), N.ppo_nout(cfg["ac"])
+    dpi, dv = rng.randn(n, nout), rng.randn(n)
+    ref = N.policy_ref(params, mcfg, x, dpi, dv, rnd=True, **kw)
+    S = N.policy_ref(params, mcfg, x, dpi, dv, absolute=True, ref_acts=ref.acts, **kw)
+    assert (S.pi >= ref.pi.abs() * (1 - 1e-12)).all() and (S.v >= ref.v.abs() * (1 - 1e-12)).all()
+    for k, g in ref.grads.items():
+        assert (S.grads[k] >= g.abs() * (1 - 1e-9) - 1e-300).all(), k

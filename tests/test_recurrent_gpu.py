@@ -12,56 +12,11 @@ import numpy as np
 import pytest
 import torch
 
+from _lstm_oracle import lstm_steps as ref_forward, lstm_steps_backward as ref_backward
+
 pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
-
-
-def _sig(x):
-    return 1.0 / (1.0 + np.exp(-x))
-
-
-def ref_forward(xg, wh, masks, s0, T, B, H, mistake=None):
-    """a2c/utils.py lstm() in float64 over time-major rows.  mistake: 'mask_after' (reset after the step), 'swap_fi'."""
-    xg = xg.reshape(T, B, 4 * H)
-    c, h = s0[:, :H].copy(), s0[:, H:].copy()
-    hs, cs, gs, hps = [], [], [], []
-    for t in range(T):
-        keep = (1.0 - masks[t])[:, None]
-        if mistake != "mask_after":
-            c, h = c * keep, h * keep
-        hps.append(h)
-        z = xg[t] + h @ wh
-        i, f, o, u = _sig(z[:, :H]), _sig(z[:, H:2 * H]), _sig(z[:, 2 * H:3 * H]), np.tanh(z[:, 3 * H:])
-        if mistake == "swap_fi":
-            i, f = f, i
-        c = f * c + i * u
-        h = o * np.tanh(c)
-        if mistake == "mask_after":
-            c, h = c * keep, h * keep
-        hs.append(h), cs.append(c), gs.append(np.concatenate([i, f, o, u], 1))
-    return (np.concatenate(hs), np.concatenate(cs), np.concatenate(gs), np.concatenate(hps),
-            np.concatenate([c, h], 1))
-
-
-def ref_backward(dh, gates, cs, masks, s0, wh, T, B, H, mistake=None):
-    """BPTT of ref_forward: dz [T*B, 4H].  mistake: 'no_carry' (drops the recurrent dh)."""
-    dh, gates, cs = dh.reshape(T, B, H), gates.reshape(T, B, 4 * H), cs.reshape(T, B, H)
-    dz = np.zeros((T, B, 4 * H))
-    dc = np.zeros((B, H))
-    carry = np.zeros((B, H))
-    for t in reversed(range(T)):
-        keep = (1.0 - masks[t])[:, None]
-        i, f, o, u = (gates[t][:, k * H:(k + 1) * H] for k in range(4))
-        cp = (cs[t - 1] if t > 0 else s0[:, :H]) * keep
-        d = dh[t] + (0 if mistake == "no_carry" else carry)
-        tc = np.tanh(cs[t])
-        dc = dc + d * o * (1 - tc * tc)
-        dz[t] = np.concatenate([dc * u * i * (1 - i), dc * cp * f * (1 - f), d * tc * o * (1 - o),
-                                dc * i * (1 - u * u)], 1)
-        carry = (dz[t] @ wh.T) * keep
-        dc = dc * f * keep
-    return dz.reshape(T * B, 4 * H)
 
 
 def _masks(kind, T, B, rng):
@@ -127,6 +82,76 @@ def test_sequence_kernels_against_float64(H, B, T, mkind):
         wrong_dz = ref_backward(dh.astype(np.float64), rg, rc, masks, s0.astype(np.float64), wh, T, B, H,
                                 mistake="no_carry")
         assert np.abs(dz - wrong_dz).max() > 10 * bound
+
+
+def _assert_float64_bounds(H, B, T, wh, xg, s0, masks, dh, h, hp, c, gates, s_out, dz):
+    """The bounds of test_sequence_kernels_against_float64 (s_out None: not written)."""
+    rh, rc, rg, rhp, rs = ref_forward(xg.astype(np.float64), wh, masks, s0.astype(np.float64), T, B, H)
+    assert (np.abs(h - rh) <= 2e-4 + 2.0 ** -11 * np.abs(rh)).all()
+    assert (np.abs(hp - rhp) <= 2e-4 + 2.0 ** -11 * np.abs(rhp)).all()
+    assert np.abs(c - rc).max() <= 2e-4 * max(1.0, np.abs(rc).max())
+    assert np.abs(gates - rg).max() <= 2e-4
+    if s_out is not None:
+        assert np.abs(s_out - rs).max() <= 2e-4 * max(1.0, np.abs(rc).max())
+    rdz = ref_backward(dh.astype(np.float64), rg, rc, masks, s0.astype(np.float64), wh, T, B, H)
+    assert np.abs(dz - rdz).max() <= 1e-3 * max(1.0, np.abs(rdz).max()) + 2.0 ** -11 * np.abs(rdz).max()
+
+
+@pytest.mark.parametrize("H", [64, 128])
+@pytest.mark.parametrize("B,T", [(37, 5), (9, 1)])
+def test_sequence_kernels_in_the_operand_forms_training_uses(H, B, T):
+    """The forms nn.LSTM.forward / backward call the kernels in: gates_out is xg (ldxg = 4H), masks gathered through
+    mask_idx and start states through state_idx from a larger permuted rollout, and row pitches ldh, lddh > H and
+    lddz > 4H.  Every output is bit-identical to the contiguous call on the equivalent dense operands, meets the float64
+    bounds, and leaves the padding columns as they were."""
+    from baselines_b200 import ops
+    wh, xg, _, _, dh = _case(H, B, T, "random", seed=11)
+    rng = np.random.default_rng(H + B)
+    n_roll, n_env = 3 * T * B + 5, 2 * B + 3                 # the rollout the minibatch's rows and states come from
+    masks_roll = (rng.random(n_roll) < 0.25).astype(np.uint8)
+    states_roll = (rng.standard_normal((n_env, 2 * H)) * 0.5).astype(np.float32)
+    mask_idx = rng.permutation(n_roll)[:T * B]
+    state_idx = rng.permutation(n_env)[:B]
+    masks = masks_roll[mask_idx].reshape(T, B).astype(np.float64)
+    s0 = states_roll[state_idx]
+    dense = _run_kernels(H, B, T, wh, xg, s0, masks, dh)
+
+    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(DEV, dt)
+    ldh, lddh, lddz = H + 8, H + 16, 4 * H + 8
+    xg_d = t(xg, torch.float32)                              # receives the gates in place
+    h = torch.full((T * B, ldh), -7.0, dtype=torch.float16, device=DEV)
+    hp = torch.zeros(T * B, H, dtype=torch.float16, device=DEV)
+    c = torch.zeros(T * B, H, dtype=torch.float32, device=DEV)
+    s_out = torch.zeros(B, 2 * H, dtype=torch.float32, device=DEV)
+    m_d, mi_d = t(masks_roll, torch.uint8), t(mask_idx, torch.int64)
+    s_d, si_d = t(states_roll, torch.float32), t(state_idx, torch.int64)
+    ops.lstm_seq_fwd(xg_d, 4 * H, t(wh, torch.float16), m_d, s_d, h, ldh, T, B, H, mask_idx=mi_d, state_idx=si_d,
+                     state_out=s_out, hprev_out=hp, gates_out=xg_d, c_out=c)
+    dh_d = torch.full((T * B, lddh), 3.0, dtype=torch.float16, device=DEV)
+    dh_d[:, :H] = t(dh, torch.float16)
+    dz = torch.full((T * B, lddz), 5.0, dtype=torch.float16, device=DEV)
+    ops.lstm_seq_bwd(dh_d, lddh, xg_d, c, m_d, s_d, t(wh.T, torch.float16), dz, lddz, T, B, H, mask_idx=mi_d,
+                     state_idx=si_d)
+    torch.cuda.synchronize()
+    assert torch.all(h[:, H:] == -7.0) and torch.all(dh_d[:, H:] == 3.0) and torch.all(dz[:, 4 * H:] == 5.0)
+    assert torch.equal(s_d, t(states_roll, torch.float32))   # the rollout's states are only read
+    g = lambda a: a.double().cpu().numpy()
+    got = (g(h[:, :H]), g(hp), g(c), g(xg_d), g(s_out), g(dz[:, :4 * H]))
+    for name, a, b in zip(("h", "hprev", "c", "gates", "state_out", "dz"), got, dense):
+        assert np.array_equal(a, b), name
+    _assert_float64_bounds(H, B, T, wh, xg, s0, masks, dh, *got)
+    # the gather matters: the rollout's first rows and states are another input
+    plain = _run_kernels(H, B, T, wh, xg, states_roll[:B], masks_roll[:T * B].reshape(T, B).astype(np.float64), dh)
+    assert not np.array_equal(plain[0], got[0])
+
+    if T == 1:
+        # acting: the state advances in place (state_out is state_in, no state_idx)
+        st = t(s0, torch.float32)
+        h1 = torch.zeros(B, H, dtype=torch.float16, device=DEV)
+        mk = t(masks.reshape(-1), torch.uint8)
+        ops.lstm_seq_fwd(t(xg, torch.float32), 4 * H, t(wh, torch.float16), mk, st, h1, H, 1, B, H, state_out=st)
+        torch.cuda.synchronize()
+        assert torch.equal(h1.double().cpu(), torch.from_numpy(dense[0])) and np.array_equal(g(st), dense[4])
 
 
 @pytest.mark.parametrize("H", [64, 128])
