@@ -73,14 +73,15 @@ def conv_stack(x, Ws, bs, geometry, act):
     return a, pres
 
 
-def kernel_act(tower, i, B):
-    """NHWC [B, OH, OW, nf] view of the kernels' stored activation of conv i of an nn.Tower."""
+def kernel_act(tower, i, B, start=0):
+    """NHWC [B, OH, OW, nf] view of the kernels' stored activation of conv i of an nn.Tower, samples start .. start+B.
+    Every layout stores a sample's activations as one run of OH * OW * nf elements."""
     c = tower.convs[i]
     h = tower.hconv[i]
     if tower.shift_mode and i + 1 < len(tower.convs) and tower.convs[i + 1].stride > 1:
         s = tower.convs[i + 1].stride
-        return R.depth_to_space(h[:B].view(B, c.OH // s, c.OW // s, s * s * c.nf), s)
-    return h.reshape(-1)[:B * c.P * c.nf].view(B, c.OH, c.OW, c.nf)
+        return R.depth_to_space(h[start:start + B].view(B, c.OH // s, c.OW // s, s * s * c.nf), s)
+    return h.reshape(-1)[start * c.P * c.nf:(start + B) * c.P * c.nf].view(B, c.OH, c.OW, c.nf)
 
 
 def reference(tower, imgs, Ws, bs, masks, dlat, B, rnd=True):
@@ -375,6 +376,37 @@ def policy_ref(params, cfg, obs, seed_pi, seed_v, rnd=False, masks=None, absolut
         sp, sv = sp.abs(), sv.abs()
     g = _grads((pi * sp).sum() + (v * sv).sum(), leaves, first)
     return types.SimpleNamespace(pi=pi.detach(), v=v.detach(), pres=net.pres, acts=net.acts, grads=g)
+
+
+def policy_ref_sliced(params, cfg, obs, seed_pi, seed_v, rows, masks=None, each=None, identity=False, dev="cpu"):
+    """policy_ref (rnd=True) and its absolute network, the error scale S, over consecutive slices of `rows` samples:
+    the float64 activations of a whole benchmark minibatch do not fit in memory at once.  Every term of a gradient
+    belongs to one row (fixed ReLU decisions, per-element roundings), so the slices' gradients add up to the unsliced
+    ones to float64 rounding.
+    obs, seed_pi, seed_v: as policy_ref, sliced here (obs may stay uint8: each slice is widened on its own).  masks:
+    None (the mirror's own ReLU decisions) or masks(s, e) -> the decisions of rows s .. e-1, built per slice.  each:
+    each(s, e, ref, S) with both runs of every slice, for per-row checks.
+    Returns a namespace: pi, v (every row), grads and S (TF name -> float64 sums over the slices)."""
+    n = obs.shape[0]
+    pis, vs, grads, S = [], [], None, None
+    for s in range(0, n, rows):
+        e = min(s + rows, n)
+        m = None if masks is None else masks(s, e)
+        ref = policy_ref(params, cfg, obs[s:e], seed_pi[s:e], seed_v[s:e], rnd=True, masks=m, identity=identity,
+                         dev=dev)
+        ab = policy_ref(params, cfg, obs[s:e], seed_pi[s:e], seed_v[s:e], absolute=True, ref_acts=ref.acts,
+                        identity=identity, dev=dev)
+        if each is not None:
+            each(s, e, ref, ab)
+        pis.append(ref.pi)
+        vs.append(ref.v)
+        if grads is None:
+            grads, S = ref.grads, ab.grads
+        else:
+            for k in grads:
+                grads[k] += ref.grads[k]
+                S[k] += ab.grads[k]
+    return types.SimpleNamespace(pi=torch.cat(pis), v=torch.cat(vs), grads=grads, S=S)
 
 
 def encode_obs(obs, onehot_n=0, nvec=None, mean=None, inv_std=None, clip=(-5.0, 5.0)):

@@ -291,6 +291,29 @@ def test_recurrent_policy_mirror_matches_lstm_oracle(name):
             _close(ref.grads[k], t.grad, f"{name} d/d {k}")
 
 
+@pytest.mark.parametrize("name", ["cnn84_cat6_shared", "mlp376_gauss17_copy_h64"])
+def test_sliced_mirror_equals_unsliced(name):
+    """policy_ref_sliced over uneven slices (3, 3, 1 rows, ReLU decisions handed in per slice) against one policy_ref
+    pass over all rows: the same head outputs, gradients and absolute network S, to float64 rounding; every slice is
+    handed to `each` once, in order."""
+    cfg, params, x, nout, rng = _ppo_case(name)
+    mcfg, ident = N.ppo_mirror_cfg(cfg), N.ppo_identity(cfg)
+    dpi, dv = rng.randn(len(x), nout), rng.randn(len(x))
+    ref = N.policy_ref(params, mcfg, x, dpi, dv, rnd=True, identity=ident)
+    S = N.policy_ref(params, mcfg, x, dpi, dv, absolute=True, ref_acts=ref.acts, identity=ident)
+    masks = {k: a for k, a in ref.acts.items() if cfg["kind"] == "cnn"}
+    seen = []
+    sl = N.policy_ref_sliced(params, mcfg, x, dpi, dv, 3, masks=lambda s, e: {k: m[s:e] for k, m in masks.items()},
+                             each=lambda s, e, r, a: seen.append((s, e, len(r.pi), len(a.pi))), identity=ident)
+    assert seen == [(0, 3, 3, 3), (3, 6, 3, 3), (6, 7, 1, 1)]
+    _close(sl.pi, ref.pi, f"{name} sliced pi")
+    _close(sl.v, ref.v, f"{name} sliced v")
+    assert list(sl.grads) == list(ref.grads) and list(sl.S) == list(S.grads)
+    for k in ref.grads:
+        _close(sl.grads[k], ref.grads[k], f"{name} sliced d/d {k}")
+        _close(sl.S[k], S.grads[k], f"{name} sliced S of {k}")
+
+
 @pytest.mark.parametrize("name", ["lstm_box7_gauss3_h128", "mlp11_cat4_shared_ln"])
 def test_absolute_mirror_bounds_the_signed_one(name):
     """The absolute network (the error scale S) through a LayerNorm or the LSTM cell: every output and gradient is at

@@ -38,7 +38,7 @@ import _loss_refs as lr
 import _net_refs as N
 import _refs as R
 from baselines_b200 import _lib
-from test_update_path_gpu import G_DLOGSTD, _gauss_nscale, _within_f16
+from test_update_path_gpu import G_DLOGSTD, G_STATS, _gauss_nscale, _stats_check, _within_f16
 
 pytestmark = pytest.mark.gpu
 
@@ -195,7 +195,20 @@ def _ppo_model(name, M, chunk=None, seed=0):
     model = Model(policy=pol, ob_space=ob, ac_space=ac, nbatch_act=8, nbatch_train=M, nsteps=1, ent_coef=ENT,
                   vf_coef=VFC, max_grad_norm=PPO_CLIP.get(name, 1e3), comm=False, train_chunk=chunk or M)
     net = model.net
-    # biases away from zero, so that a missing bias term or a stale bias operand shows
+    rng = _move_off_zero(model, seed)
+    if cfg.get("normalize"):
+        # statistics with |(x - mean) / std| beyond 5 for a good share of the observations: the clip is active
+        d = N.in_dim(cfg["ob"])[0]
+        net.set_obs_rms(dict(runningsum=rng.randn(d) * 5.0, runningsumsq=rng.rand(d) * 20.0 + 30.0, count=10.0))
+        assert net.obs_rms is not None
+    assert net.pi_identity == N.ppo_identity(cfg)
+    return model
+
+
+def _move_off_zero(model, seed):
+    """Biases away from zero, so that a missing bias term or a stale bias operand shows, and a non-zero Gaussian
+    logstd.  Returns the random stream, for further settings."""
+    net = model.net
     rng = np.random.RandomState(seed + 100)
     p = net.store.export_tf("params")
     for k in p:
@@ -204,13 +217,7 @@ def _ppo_model(name, M, chunk=None, seed=0):
     if net.pd == "gauss":
         p["ppo2_model/pi/logstd:0"] = (0.2 * rng.randn(1, net.nout)).astype(np.float32)
     model.set_params(p)
-    if cfg.get("normalize"):
-        # statistics with |(x - mean) / std| beyond 5 for a good share of the observations: the clip is active
-        d = N.in_dim(cfg["ob"])[0]
-        net.set_obs_rms(dict(runningsum=rng.randn(d) * 5.0, runningsumsq=rng.rand(d) * 20.0 + 30.0, count=10.0))
-        assert net.obs_rms is not None
-    assert net.pi_identity == N.ppo_identity(cfg)
-    return model
+    return rng
 
 
 def _norm_arrays(net):
@@ -279,18 +286,18 @@ def _flat_state(store):
     return {k: getattr(store, k).detach().double().cpu().numpy().copy() for k in ("params", "m", "v")}
 
 
-def _ppo_step(model, roll, rows, graph):
+def _ppo_step(model, roll, rows, graph, lr_=PPO_LR, cliprange=CLIPRANGE):
     """One train_rollout on rows `rows` of the rollout: gathered through src_idx (graph-captured) or as contiguous
     M-row buffers (eager).  Returns the pre-step flat state and exported parameters."""
     before = _flat_state(model.net.store)
     params = model.net.store.export_tf("params")
     if graph:
-        model.train_rollout(PPO_LR, CLIPRANGE, roll["obs"], roll["acts"], roll["ret"], roll["oldv"], roll["oldnlp"],
+        model.train_rollout(lr_, cliprange, roll["obs"], roll["acts"], roll["ret"], roll["oldv"], roll["oldnlp"],
                             torch.as_tensor(rows).to(DEV))
     else:
         r = torch.as_tensor(rows).to(DEV)
         sel = lambda t: t.index_select(0, r).contiguous()
-        model.train_rollout(PPO_LR, CLIPRANGE, sel(roll["obs"]), sel(roll["acts"]), sel(roll["ret"]),
+        model.train_rollout(lr_, cliprange, sel(roll["obs"]), sel(roll["acts"]), sel(roll["ret"]),
                             sel(roll["oldv"]), sel(roll["oldnlp"]), None)
     torch.cuda.synchronize()
     return before, params
@@ -303,8 +310,11 @@ def _ppo_heads(net, B):
             net.dpi[:B, :nout].double().cpu(), net.dv[:B, 0].double().cpu())
 
 
-def _check_ppo_heads(name, cfg, net, roll, rows, M, params):
-    """(a) head-gradient rows against _loss_refs.ppo_ref at the kernels' own head outputs."""
+def _check_ppo_heads(name, cfg, net, roll, rows, M, params, clip=CLIPRANGE, ent=ENT, vfc=VFC, stats=None,
+                     g_dlogstd=G_DLOGSTD, dlogstd_drop=1):
+    """(a) head-gradient rows against _loss_refs.ppo_ref at the kernels' own head outputs; with `stats` (the kernels'
+    five loss-statistic sums) those too, against the same reference's per-row terms.  A Gaussian's dL/dlogstd is
+    within g_dlogstd of its absolute row sum, a bound that rejects the first dlogstd_drop rows dropped."""
     pd = cfg["ac"][0]
     pi, v, dpi, dv = _ppo_heads(net, M)
     nvec = list(cfg["ac"][1]) if pd == "mcat" else None
@@ -314,11 +324,11 @@ def _check_ppo_heads(name, cfg, net, roll, rows, M, params):
     acts = roll["acts_np"][rows]
     ls = params["ppo2_model/pi/logstd:0"].reshape(-1) if pd == "gauss" else None      # the pre-step logstd
     pi32, v32 = pi.numpy().astype(np.float32), v.numpy().astype(np.float32)
-    args = (pd, pi32, v32, acts, R_, oldv, oldnlp, adv, CLIPRANGE, ENT, VFC)
+    args = (pd, pi32, v32, acts, R_, oldv, oldnlp, adv, clip, ent, vfc)
     ref = lr.ppo_ref(*args, nvec=nvec, logstd=ls)
     ok = ~ref.near
     assert ok.mean() > 0.95
-    nb = lr.ppo_ref(pd, pi32, v32, np.roll(acts, 1, 0), R_, oldv, oldnlp, adv, CLIPRANGE, ENT, VFC, nvec=nvec, logstd=ls)
+    nb = lr.ppo_ref(pd, pi32, v32, np.roll(acts, 1, 0), *args[4:], nvec=nvec, logstd=ls)
     nscale = _gauss_nscale(acts, pi32, ls, oldnlp)[ok] if pd == "gauss" else None
     _within_f16(dpi.numpy()[ok], ref.dhead[ok], {"actions of the neighbouring row": nb.dhead[ok]},
                 f"{name} dpi", nscale)
@@ -330,25 +340,31 @@ def _check_ppo_heads(name, cfg, net, roll, rows, M, params):
         got = net.store.export_tf("grads")["ppo2_model/pi/logstd:0"].reshape(-1).astype(np.float64)
         S = np.abs(rws).sum(0) + np.abs(want)
         t = lambda a: torch.as_tensor(np.asarray(a, np.float64))
-        seen = R.assert_within(t(got), t(want), t(S), G_DLOGSTD, 0.0,
-                               {"row 0 dropped": t(want - rws[0]),
-                                "-ent_coef term dropped": t(lr.ppo_ref(*args, nvec=nvec, logstd=ls,
-                                                                       mutant="no_entropy").dlogstd_rows.sum(0) / M)},
-                               f"{name} pi/logstd")
-        _report(f"{name} pi/logstd", seen, G_DLOGSTD)
+        muts = {"row 0 dropped" if dlogstd_drop == 1 else f"rows 0..{dlogstd_drop - 1} dropped":
+                t(want - rws[:dlogstd_drop].sum(0))}
+        if ent:                                   # without an entropy bonus the mutant is the reference itself
+            muts["-ent_coef term dropped"] = t(lr.ppo_ref(*args, nvec=nvec, logstd=ls,
+                                                          mutant="no_entropy").dlogstd_rows.sum(0) / M)
+        for mn, mv in muts.items():
+            print(f"[mutant] {name} pi/logstd {mn}: g = {R.excess(mv, t(want), t(S), 0.0):.3e}")
+        seen = R.assert_within(t(got), t(want), t(S), g_dlogstd, 0.0, muts, f"{name} pi/logstd")
+        _report(f"{name} pi/logstd", seen, g_dlogstd)
+    if stats is not None:
+        seen = _stats_check(stats, ref, pd, pi32, acts, oldnlp, adv, ls, M, name)
+        _report(f"{name} loss statistics", seen, G_STATS)
     return dpi, dv
 
 
-def _ppo_masks(net, M):
-    """ReLU decisions of the kernels' stored activations, keyed like the mirror's layers."""
+def _ppo_masks(net, M, start=0):
+    """ReLU decisions of the kernels' stored activations of rows start .. start+M, keyed like the mirror's layers."""
     masks = {}
     towers = [("pi", net.tower_pi)] + ([("vf", net.tower_vf)] if net.tower_vf is not None else [])
     for nm, t in towers:
         if t.kind != "cnn":
             continue
         for i, c in enumerate(t.convs):
-            masks[f"ppo2_model/{nm}/{c.name.split('/')[-1]}"] = (N.kernel_act(t, i, M) > 0).double()
-        masks[f"ppo2_model/{nm}/fc1"] = (t.hfc[0][:M, :t.fcs[0].N] > 0).double()
+            masks[f"ppo2_model/{nm}/{c.name.split('/')[-1]}"] = (N.kernel_act(t, i, M, start) > 0).double()
+        masks[f"ppo2_model/{nm}/fc1"] = (t.hfc[0][start:start + M, :t.fcs[0].N] > 0).double()
     return masks
 
 
@@ -356,21 +372,28 @@ def _short(k):
     return k.replace("ppo2_model/", "").replace("deepq/q_func/", "").replace(":0", "")
 
 
-def _check_masks(what, ref, S, masks):
+def _check_masks(what, ref, S, masks, report=True, g_mask=G_MASK):
+    """Every kernel ReLU decision that differs from the mirror's lies within g_mask * S of zero.  Returns name ->
+    (worst |pre| / S, decisions that differ)."""
+    out = {}
     for k, m in masks.items():
         p, pa = ref.pres[k], S.pres[k]
         off = m != (p > 0).double()
         worst = float((p.abs()[off] / pa[off]).max()) if bool(off.any()) else 0.0
-        _report(f"{what} {_short(k)} ReLU decisions ({int(off.sum())} differ) |pre|/S", worst, G_MASK)
-        assert worst <= G_MASK, (what, k, worst)
+        out[k] = (worst, int(off.sum()))
+        if report:
+            _report(f"{what} {_short(k)} ReLU decisions ({int(off.sum())} differ) |pre|/S", worst, g_mask)
+        assert worst <= g_mask, (what, k, worst)
+    return out
 
 
-def _assert_grads(what, table_key, got, ref_g, S_g, mutants, names, alpha):
+def _assert_grads(what, table_key, got, ref_g, S_g, mutants, names, alpha, g_table=None):
     """(b): every TF variable in `names` within its bound, each bound rejecting its mutants.  mutants: name ->
-    (grads dict, target tensors or None for all)."""
+    (grads dict, target tensors or None for all).  g_table: (table_key, short name) -> g, G by default."""
+    g_table = G if g_table is None else g_table
     for k in names:
         gt = torch.as_tensor(got[k]).to(DEV).double().reshape(ref_g[k].shape)
-        ref, S, g = ref_g[k] * alpha, S_g[k] * alpha, G[(table_key, _short(k))]
+        ref, S, g = ref_g[k] * alpha, S_g[k] * alpha, g_table[(table_key, _short(k))]
         muts = {mn: mg[k] * alpha for mn, (mg, targets) in mutants.items() if targets is None or k in targets}
         for mn, mg in muts.items():
             print(f"[mutant] {what} {_short(k)} {mn}: g = {R.excess(mg, ref, S, R.R_F32):.3e}")
@@ -453,13 +476,16 @@ def _lr_t(lr_):
     return lambda t: _f32(lr_ * math.sqrt(1.0 - 0.999 ** t) / (1.0 - 0.9 ** t))
 
 
-def _ppo_adam(what, name, model, before, M):
+def _ppo_adam(what, name, model, before, M, lr_=PPO_LR, clipped=None):
+    """(c) for a PPO2 step with learning rate lr_; clipped: whether the global clip scales this step (by default
+    whether the configuration is in PPO_CLIP)."""
     store, net = model.net.store, model.net
     g_flat = store.grads.detach().double().cpu().numpy()
     clip = model.max_grad_norm
     sc = lr.clip_scale(math.fsum(g_flat * g_flat), clip)
-    assert (sc < 1.0) == (name in PPO_CLIP), (name, sc)          # which case this run is in
-    _check_adam(what, store, before, g_flat, _lr_t(PPO_LR), model.opt.t, 1e-5, sc, sc < 1.0)
+    clipped = name in PPO_CLIP if clipped is None else clipped
+    assert (sc < 1.0) == clipped, (name, sc)                     # which case this run is in
+    _check_adam(what, store, before, g_flat, _lr_t(lr_), model.opt.t, 1e-5, sc, sc < 1.0)
     if net.pi_identity:                                          # the frozen identity block: bit-for-bit unchanged
         h = net.head_pi if net.head is None else net.head
         hw, gw = (h.w, h.gw) if net.head is None else (h.w[:, :net.nout], h.gw[:, :net.nout])
@@ -549,7 +575,9 @@ DQN_CLIP_CASE = {"mlp_dueling_h64_32_double": "none", "mlp_plain_h20_max": "off"
                  "cnn_dueling_h256": "mixed", "conv_only_dueling_h256": "mixed", "mlp_disc7_dueling_h64": "off"}
 
 
-def _dqn_model(name, seed=3):
+def _dqn_model(name, seed=3, B=DQN_B, lr_=DQN_LR, clip=None):
+    """The DQNModel of configuration `name` (learning rate lr_, batch B, grad_norm_clipping clip), biases away from
+    zero and a target network that differs from the online one."""
     from baselines_b200.common import spaces
     from baselines_b200.deepq.build_graph import DQNModel
     cfg = N.DQN_CONFIGS[name]
@@ -558,8 +586,8 @@ def _dqn_model(name, seed=3):
         ob = spaces.Discrete(oa)
     else:
         ob = spaces.Box(0, 255, oa, np.uint8) if cfg["kind"] != "mlp" else spaces.Box(-5, 5, oa, np.float32)
-    model = DQNModel(ob, DQN_NA, cfg["kind"], lr=DQN_LR, gamma=GAMMA, grad_norm_clipping=DQN_CLIP[name],
-                     double_q=cfg["double_q"], batch_cap=DQN_B, seed=seed, hiddens=cfg["hiddens"],
+    model = DQNModel(ob, DQN_NA, cfg["kind"], lr=lr_, gamma=GAMMA, grad_norm_clipping=clip,
+                     double_q=cfg["double_q"], batch_cap=B, seed=seed, hiddens=cfg["hiddens"],
                      dueling=cfg["dueling"])
     rng = np.random.RandomState(seed + 100)
     p = model.q.store.export_tf("params")
@@ -630,17 +658,26 @@ def _check_dqn_heads(what, model, cfg, b, rows, w, B):
     return da, ds
 
 
-def _dqn_mutants(cfg, params, x, da, ds, masks, mcfg, names):
+def _dqn_mutants(cfg, params, x, da, ds, masks, mcfg, names, block=None):
+    """block: (k, short names): for those tensors, whose bound cannot see one sample, k consecutive rows dropped from
+    the row with the largest TD gradient on."""
     run = lambda a, s, xx=x, **kw: N.q_ref(params, mcfg, xx, a, s, rnd=True, masks=masks, dev=DEV, **kw).grads
     # the row with the largest TD gradient: both streams' seeds of a row come from the same d loss / dq
     i = int(da.abs().sum(1).argmax() if ds is None else ds.abs().argmax())
-    a0 = da.clone()
-    a0[i] = 0.0
-    s0 = None
-    if ds is not None:
-        s0 = ds.clone()
-        s0[i] = 0.0
-    out = {"one sample dropped": (run(a0, s0), None)}
+
+    def drop(k):
+        r = slice(min(i, len(da) - k), min(i, len(da) - k) + k)
+        a0 = da.clone()
+        a0[r] = 0.0
+        s0 = None
+        if ds is not None:
+            s0 = ds.clone()
+            s0[r] = 0.0
+        return run(a0, s0)
+    weak = set() if block is None else {k for k in names if _short(k) in block[1]}
+    out = {"one sample dropped": (drop(1), None if block is None else set(names) - weak)}
+    if block is not None:
+        out[f"{block[0]} consecutive rows dropped"] = (drop(block[0]), weak)
     sc = "deepq/q_func"
     trunk = {k for k in names if "_value/" not in k}
     if cfg["dueling"]:
@@ -661,9 +698,17 @@ def _dqn_mutants(cfg, params, x, da, ds, masks, mcfg, names):
 @pytest.mark.parametrize("replay", [False, True], ids=["gathered", "replay_idx"])
 @pytest.mark.parametrize("name", list(N.DQN_CONFIGS))
 def test_dqn_update_composition_vs_float64(name, replay):
+    _dqn_update_run(name, replay, clip=DQN_CLIP[name], w_scale=DQN_W_SCALE.get(name, 1.0), case=DQN_CLIP_CASE[name])
+
+
+def _dqn_update_run(name, replay, B=DQN_B, lr_=DQN_LR, clip=None, w_scale=1.0, case="off", g_table=None,
+                    table_key=None, block=None):
+    """Three DQN updates of configuration `name` at batch B, learning rate lr_ and grad_norm_clipping clip, checked
+    (a) to (d).  w_scale: the scale of the importance weights; case: which variables the clip scales in the first
+    update ("mixed", "none" or "off"); g_table / table_key: the gradient bounds (G and name by default); block: see
+    _dqn_mutants."""
     cfg = N.DQN_CONFIGS[name]
-    B = DQN_B
-    model = _dqn_model(name)
+    model = _dqn_model(name, B=B, lr_=lr_, clip=clip)
     q = model.q
     if cfg["dueling"] and q.first_widths[0] % 8:                 # the state stream starts past padding columns
         assert q.cat_off[1] == -(-q.first_widths[0] // 8) * 8 > q.first_widths[0], q.cat_off
@@ -678,7 +723,7 @@ def test_dqn_update_composition_vs_float64(name, replay):
         rows = perm[step * B:(step + 1) * B]
         what = f"{name} {'replay' if replay else 'gathered'} step {step + 1}"
         replays = _lib.REPLAYS
-        w = ((rng.rand(B) * 0.9 + 0.1) * DQN_W_SCALE.get(name, 1.0)).astype(np.float32)
+        w = ((rng.rand(B) * 0.9 + 0.1) * w_scale).astype(np.float32)
         before = _flat_state(q.store)
         params = q.store.export_tf("params")
         if replay:
@@ -700,12 +745,11 @@ def test_dqn_update_composition_vs_float64(name, replay):
         _check_masks(what, ref, S, masks)
         got = q.store.export_tf("grads")
         names = list(got)
-        muts = _dqn_mutants(cfg, params, x, da.to(DEV), None if ds is None else ds.to(DEV), masks, mcfg, names)
-        _assert_grads(what, name, got, ref.grads, S.grads, muts, names, 1.0 / B)
+        muts = _dqn_mutants(cfg, params, x, da.to(DEV), None if ds is None else ds.to(DEV), masks, mcfg, names, block)
+        _assert_grads(what, table_key or name, got, ref.grads, S.grads, muts, names, 1.0 / B, g_table)
         # (c) per-variable clip_by_norm, then Adam
         g_flat = q.store.grads.detach().double().cpu().numpy()
         off = q.store.segment_offsets()
-        clip = DQN_CLIP[name]
         scale = np.ones_like(g_flat)
         facs = []
         for s0, s1 in zip(off[:-1], off[1:]):
@@ -714,9 +758,9 @@ def test_dqn_update_composition_vs_float64(name, replay):
             scale[s0:s1] = f
             facs.append(f)
         print(f"[observed] {what} per-variable clip factors: {np.round(facs, 3).tolist()}")
-        case = DQN_CLIP_CASE[name] if step == 0 else ("off" if clip is None else "any")   # which case this run is in
-        if case == "mixed":
+        now = case if step == 0 else ("off" if clip is None else "any")           # which case this run is in
+        if now == "mixed":
             assert min(facs) < 1.0 and max(facs) == 1.0, (name, facs)
-        elif case != "any":
-            assert all(f == 1.0 for f in facs) and (clip is None) == (case == "off"), (name, facs)
-        _check_adam(what, q.store, before, g_flat, _lr_t(DQN_LR), model.opt.t, 1e-8, scale, min(facs) < 1.0)
+        elif now != "any":
+            assert all(f == 1.0 for f in facs) and (clip is None) == (now == "off"), (name, facs)
+        _check_adam(what, q.store, before, g_flat, _lr_t(lr_), model.opt.t, 1e-8, scale, min(facs) < 1.0)
