@@ -309,7 +309,6 @@ class DQNModel:
             self._w_buf = torch.zeros(batch_cap, dtype=torch.float32, device=dev)
             self._eps_dev = torch.zeros(1, dtype=torch.float32, device=dev)
             self._step_dev = torch.zeros(1, dtype=torch.int64, device=dev)
-            self._act_obs = None
         self.graphs = graphs.GraphCache()
         self.batch_cap = batch_cap
         self.eps = 0.0
@@ -323,18 +322,20 @@ class DQNModel:
         self.qt.store.params.copy_(self.q.store.params)
         self.qt.refresh()
 
+    def _stage_act(self, obs_dev, B, eps):
+        """The inputs of an acting pass over B observations: the observations go to a fixed buffer (graphs.home) and
+        eps to the device, so the pass is a replayable launch sequence.  Returns the staged observations."""
+        if B > self.batch_cap:
+            raise ValueError(f"act batch {B} exceeds batch_cap {self.batch_cap}")
+        x = self.graphs.home("act_obs", self.batch_cap, obs_dev.shape[1:], obs_dev.dtype, self.device)[:B]
+        x.copy_(obs_dev)
+        ops.set_scalars(self._eps_dev, eps)
+        return x
+
     def act_device(self, obs_dev, B, eps):
         """build_graph.py:184-192 on B observations.  The observations are staged in a fixed buffer, eps and the
         random-stream position live on the device, so the pass is captured once per B and replayed."""
-        if B > self.batch_cap:
-            raise ValueError(f"act batch {B} exceeds batch_cap {self.batch_cap}")
-        if self._act_obs is None or self._act_obs.shape[1:] != obs_dev.shape[1:] or self._act_obs.dtype != obs_dev.dtype:
-            self._act_obs = torch.zeros((self.batch_cap,) + tuple(obs_dev.shape[1:]), dtype=obs_dev.dtype,
-                                        device=self.device)
-            self.graphs.clear()
-        self._act_obs[:B].copy_(obs_dev)
-        ops.set_scalars(self._eps_dev, eps)
-        x = self._act_obs[:B]
+        x = self._stage_act(obs_dev, B, eps)
 
         def body():
             out = self.q.forward(x, B)
@@ -353,15 +354,7 @@ class DQNModel:
         (3) to the TF runtime.)  One trunk forward serves all three networks; the sequence is captured per
         (B, reset, update_scale)."""
         pn, q = self.pn, self.q
-        if B > self.batch_cap:
-            raise ValueError(f"act batch {B} exceeds batch_cap {self.batch_cap}")
-        if self._act_obs is None or self._act_obs.shape[1:] != obs_dev.shape[1:] or self._act_obs.dtype != obs_dev.dtype:
-            self._act_obs = torch.zeros((self.batch_cap,) + tuple(obs_dev.shape[1:]), dtype=obs_dev.dtype,
-                                        device=self.device)
-            self.graphs.clear()
-        self._act_obs[:B].copy_(obs_dev)
-        ops.set_scalars(self._eps_dev, eps)
-        x = self._act_obs[:B]
+        x = self._stage_act(obs_dev, B, eps)
 
         def body():
             q.trunk_forward(x, B)

@@ -29,6 +29,19 @@ class GraphCache:
         self.graphs = {}          # key -> (graph, number of library kernels launches captured in it)
         self.seen = set()
         self.max_graphs = max_graphs
+        self.homes = {}
+
+    def home(self, name, rows, trailing, dtype, device):
+        """The fixed buffer `name` with at least `rows` rows of shape `trailing`: captured graphs read it, each call
+        refills it.  Its leading dimension may grow; its trailing shape and dtype are fixed.  A request that does not
+        fit allocates it anew at exactly that size; replacing an earlier buffer drops every graph and the seen set,
+        since a graph captured over the old buffer would otherwise replay reading freed memory."""
+        buf = self.homes.get(name)
+        if buf is None or buf.shape[0] < rows or buf.shape[1:] != tuple(trailing) or buf.dtype != dtype:
+            if buf is not None:
+                self.clear()
+            buf = self.homes[name] = torch.zeros((rows,) + tuple(trailing), dtype=dtype, device=device)
+        return buf
 
     def run(self, key, fn, allow_fallback=False):
         if not enabled() or _lib._prof is not None:            # per-call profiling needs the eager sequence

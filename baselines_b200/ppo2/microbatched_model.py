@@ -45,15 +45,9 @@ class MicrobatchedModel(Model):
             self._acc.zero_()
             net.stats.zero_()
             ops.adv_stats(returns, values, src_idx, M, net.adv_st)        # microbatched_model.py:43: FULL minibatch
-            for s in range(0, M, mb):
+            for *args, _ in self._chunks(M, mb, src_idx, obs, actions, returns, values, neglogpacs):
                 store.grads.zero_()
-                if src_idx is not None:
-                    net.loss_backward(obs, mb, src_idx[s:s + mb], actions, returns, values, neglogpacs, cliprange,
-                                      self.ent_coef, self.vf_coef, 1.0 / mb)
-                else:
-                    sl = slice(s, s + mb)
-                    net.loss_backward(obs[sl], mb, None, actions[sl], returns[sl], values[sl], neglogpacs[sl],
-                                      cliprange, self.ent_coef, self.vf_coef, 1.0 / mb)
+                net.loss_backward(*args, cliprange, self.ent_coef, self.vf_coef, 1.0 / mb)
                 net.freeze_identity()
                 self.dist.average_gradients(store)                        # inside compute_gradients, before the clip
                 clip = opt.clip if opt.clip is not None else 0.0

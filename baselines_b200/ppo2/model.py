@@ -50,11 +50,9 @@ class Model(object):
             with torch.cuda.device(self.device):
                 self._act_state = torch.zeros(nbatch_act, 2 * self.net.nlstm, dtype=torch.float32, device=self.device)
                 self._act_mask = torch.zeros(nbatch_act, dtype=torch.uint8, device=self.device)
-            self._seq_idx = self._seq_env = None      # fixed homes of a recurrent minibatch's row / environment indices
         self.act_model = self.train_model = self
         self._rng_seed = int(np.random.randint(0, 2 ** 31 - 1))
         self.graphs = graphs.GraphCache()
-        self._mb_idx = None                       # fixed home of the current minibatch's indices (graph replays)
         self._stats_out = torch.zeros(5, dtype=torch.float64, device=self.device)
         self.comm = comm
         self.dist = dist_util.DataParallel(comm, mpi_rank_weight)
@@ -166,60 +164,16 @@ class Model(object):
         obs/actions/returns/values/neglogpacs: flat device buffers in buffer order; src_idx: int64 device
         tensor of the M buffer offsets forming this minibatch (the shuffled `mbinds` of ppo2.py:164 mapped to
         buffer order), or None for "all rows in order".  Returns a device float64[5] of the loss statistics."""
-        net, store = self.net, self.net.store
+        arrays = (obs, actions, returns, values, neglogpacs)
         M = int(src_idx.numel()) if src_idx is not None else int(returns.numel())
+        idx = key = None                                         # rows in order: caller-owned temporaries, run eagerly
         with torch.cuda.device(self.device):
-            # scalars that change from call to call go to device memory first; everything after that is a fixed launch
-            # sequence for a given (rollout buffers, M), captured once and replayed (graphs.py)
-            ops.set_scalars(net.clip_dev, cliprange)
-            self.opt.begin_step(lr)
-            idx_all = None
             if src_idx is not None:
-                if self._mb_idx is None or self._mb_idx.numel() < M:
-                    self._mb_idx = torch.empty(max(M, self.nbatch_train), dtype=torch.int64, device=self.device)
-                self._mb_idx[:M].copy_(src_idx)
-                idx_all = self._mb_idx
-            inv_M = 1.0 / M
-
-            def grads():
-                store.grads.zero_()
-                net.stats.zero_()
-                ops.adv_stats(returns, values, None if idx_all is None else idx_all[:M], M, net.adv_st)  # model.py:139
-                for s in range(0, M, self.chunk):
-                    B = min(self.chunk, M - s)
-                    if idx_all is not None:
-                        net.loss_backward(obs, B, idx_all[s:s + B], actions, returns, values, neglogpacs, None,
-                                          self.ent_coef, self.vf_coef, inv_M)
-                    else:
-                        sl = slice(s, s + B)
-                        net.loss_backward(obs[sl], B, None, actions[sl], returns[sl], values[sl], neglogpacs[sl],
-                                          None, self.ent_coef, self.vf_coef, inv_M)
-                net.freeze_identity()
-
-            def update():
-                self.opt.apply()                                         # model.py:107 clip -> :114 Adam
-                net.refresh()
-                self._stats_out.copy_(net.stats)
-
-            if idx_all is None:                                          # caller-owned temporaries: run eagerly
-                grads()
-                self.dist.average_gradients(store)
-                update()
-            else:
-                key = ("train", M, obs.data_ptr(), actions.data_ptr(), returns.data_ptr(), values.data_ptr(),
-                       neglogpacs.data_ptr())
-                if self.dist.active and os.environ.get("B200RL_GRAPH_NCCL", "0") != "1":
-                    self.graphs.run(key + ("grads",), grads)
-                    self.dist.average_gradients(store)                   # mpi_adam_optimizer.py:39-40, BEFORE the clip
-                    self.graphs.run(key + ("update",), update)
-                else:
-                    # single process: one graph per minibatch.  (B200RL_GRAPH_NCCL=1 also captures the NCCL all-reduce;
-                    # measured on 2 GPUs it is no faster than the split form -- 236.7 vs 236.6 ms -- and the process
-                    # group then hangs at teardown, so the split form is the default.)
-                    self.graphs.run(key, lambda: (grads(), self.dist.average_gradients(store), update()),
-                                    allow_fallback=self.dist.active)
-            self._after_train_call()
-            return self._stats_out / M
+                idx = self.graphs.home("mb_idx", max(M, self.nbatch_train), (), torch.int64, self.device)[:M]
+                idx.copy_(src_idx)
+                key = ("train", M) + tuple(a.data_ptr() for a in arrays)
+            return self._train_step(lr, cliprange, M, returns, values, idx, self._chunks(M, self.chunk, idx, *arrays),
+                                    key)
 
     def train_rollout_seq(self, lr, cliprange, obs, actions, returns, values, neglogpacs, dones, states0, rows, envs,
                           eager=False):
@@ -229,60 +183,81 @@ class Model(object):
         states0.  The sequence kernels take time-major rows (t*E + e), so the launch order is built here; the loss is a
         mean, so the order does not change it.  Chunks are whole environments (chunk // T of them).  Returns a device
         float64[5] of the loss statistics.  eager: the buffers are the caller's temporaries (no graph capture)."""
-        net, store = self.net, self.net.store
         rows = np.asarray(rows, dtype=np.int64)
         envs = np.asarray(envs, dtype=np.int64).reshape(-1)
         E, T = rows.shape
         M = E * T
         per = max(1, self.chunk // T)
-        chunks = [(e0, min(E, e0 + per)) for e0 in range(0, E, per)]
+        spans = [(e0, min(E, e0 + per)) for e0 in range(0, E, per)]
         # per chunk, the time-major row offsets of its environments, chunk after chunk
-        order = np.concatenate([rows[e0:e1].T.reshape(-1) for e0, e1 in chunks])
+        order = np.concatenate([rows[e0:e1].T.reshape(-1) for e0, e1 in spans])
         with torch.cuda.device(self.device):
-            dev = self.device
-            if self._seq_idx is None or self._seq_idx.numel() < M or self._seq_env.numel() < E:
-                self._seq_idx = torch.empty(max(M, self.nbatch_train), dtype=torch.int64, device=dev)
-                self._seq_env = torch.empty(max(E, self.nbatch_train // max(T, 1), 1), dtype=torch.int64, device=dev)
-            self._seq_idx[:M].copy_(torch.from_numpy(order))
-            self._seq_env[:E].copy_(torch.from_numpy(envs))
-            ops.set_scalars(net.clip_dev, cliprange)
-            self.opt.begin_step(lr)
-            idx, env = self._seq_idx, self._seq_env
-            inv_M = 1.0 / M
+            idx = self.graphs.home("seq_idx", max(M, self.nbatch_train), (), torch.int64, self.device)[:M]
+            env = self.graphs.home("seq_env", max(E, self.nbatch_train // max(T, 1), 1), (), torch.int64,
+                                   self.device)[:E]
+            idx.copy_(torch.from_numpy(order))
+            env.copy_(torch.from_numpy(envs))
+            chunks = [(obs, (e1 - e0) * T, idx[e0 * T:e1 * T], actions, returns, values, neglogpacs,
+                       Seq(T, e1 - e0, dones, idx[e0 * T:e1 * T], states0, env[e0:e1], None)) for e0, e1 in spans]
+            key = None if eager else ("train_seq", E, T) + tuple(
+                a.data_ptr() for a in (obs, actions, returns, values, neglogpacs, dones, states0))
+            return self._train_step(lr, cliprange, M, returns, values, idx, chunks, key)
 
-            def grads():
-                store.grads.zero_()
-                net.stats.zero_()
-                ops.adv_stats(returns, values, idx[:M], M, net.adv_st)                        # model.py:139
-                for e0, e1 in chunks:
-                    B, s = (e1 - e0) * T, e0 * T
-                    seq = Seq(T, e1 - e0, dones, idx[s:s + B], states0, env[e0:e1], None)
-                    net.loss_backward(obs, B, idx[s:s + B], actions, returns, values, neglogpacs, None,
-                                      self.ent_coef, self.vf_coef, inv_M, seq=seq)
-                net.freeze_identity()
-
-            def update():
-                self.opt.apply()
-                net.refresh()
-                self._stats_out.copy_(net.stats)
-
-            if eager:
-                grads()
-                self.dist.average_gradients(store)
-                update()
-                self._after_train_call()
-                return self._stats_out / M
-            key = ("train_seq", E, T, obs.data_ptr(), actions.data_ptr(), returns.data_ptr(), values.data_ptr(),
-                   neglogpacs.data_ptr(), dones.data_ptr(), states0.data_ptr(), idx.data_ptr(), env.data_ptr())
-            if self.dist.active and os.environ.get("B200RL_GRAPH_NCCL", "0") != "1":
-                self.graphs.run(key + ("grads",), grads)
-                self.dist.average_gradients(store)
-                self.graphs.run(key + ("update",), update)
+    @staticmethod
+    def _chunks(M, size, idx, obs, actions, returns, values, neglogpacs):
+        """M samples in chunks of at most `size`, each as loss_backward's leading arguments (x, B, src_idx, actions,
+        returns, values, neglogpacs) and seq (None): gathered through idx, or (idx None) the rows in order, sliced."""
+        out = []
+        for s in range(0, M, size):
+            B = min(size, M - s)
+            if idx is not None:
+                out.append((obs, B, idx[s:s + B], actions, returns, values, neglogpacs, None))
             else:
-                self.graphs.run(key, lambda: (grads(), self.dist.average_gradients(store), update()),
-                                allow_fallback=self.dist.active)
-            self._after_train_call()
-            return self._stats_out / M
+                sl = slice(s, s + B)
+                out.append((obs[sl], B, None, actions[sl], returns[sl], values[sl], neglogpacs[sl], None))
+        return out
+
+    def _train_step(self, lr, cliprange, M, returns, values, idx, chunks, key):
+        """The update of one minibatch of M samples from its chunks (see _chunks); idx: the minibatch's buffer offsets
+        into returns / values, or None for their rows in order.  key: the graph the step is captured as and
+        replayed from, or None to run it eagerly.  Runs on the current device.  Returns a device float64[5] of the loss
+        statistics."""
+        net, store = self.net, self.net.store
+        # scalars that change from call to call go to device memory first; everything after that is a fixed launch
+        # sequence for a given key, captured once and replayed (graphs.py)
+        ops.set_scalars(net.clip_dev, cliprange)
+        self.opt.begin_step(lr)
+        inv_M = 1.0 / M
+
+        def grads():
+            store.grads.zero_()
+            net.stats.zero_()
+            ops.adv_stats(returns, values, idx, M, net.adv_st)                             # model.py:139
+            for *args, seq in chunks:
+                net.loss_backward(*args, None, self.ent_coef, self.vf_coef, inv_M, seq=seq)
+            net.freeze_identity()
+
+        def update():
+            self.opt.apply()                                             # model.py:107 clip -> :114 Adam
+            net.refresh()
+            self._stats_out.copy_(net.stats)
+
+        if key is None:
+            grads()
+            self.dist.average_gradients(store)
+            update()
+        elif self.dist.active and os.environ.get("B200RL_GRAPH_NCCL", "0") != "1":
+            self.graphs.run(key + ("grads",), grads)
+            self.dist.average_gradients(store)                           # mpi_adam_optimizer.py:39-40, BEFORE the clip
+            self.graphs.run(key + ("update",), update)
+        else:
+            # single process: one graph per minibatch.  (B200RL_GRAPH_NCCL=1 also captures the NCCL all-reduce;
+            # measured on 2 GPUs it is no faster than the split form -- 236.7 vs 236.6 ms -- and the process
+            # group then hangs at teardown, so the split form is the default.)
+            self.graphs.run(key, lambda: (grads(), self.dist.average_gradients(store), update()),
+                            allow_fallback=self.dist.active)
+        self._after_train_call()
+        return self._stats_out / M
 
     def _after_train_call(self):
         """mpi_adam_optimizer.py:41-42: every 100th compute_gradients call checks that the ranks still hold identical
@@ -306,6 +281,7 @@ class Model(object):
             x = self.net.encode_obs(np.asarray(obs))
             a = torch.as_tensor(np.ascontiguousarray(actions), dtype=self.net.action_dtype).to(dev).contiguous()
             f = lambda z: torch.as_tensor(np.ascontiguousarray(z), dtype=torch.float32).to(dev)
+            # the buffers are this call's temporaries: both kinds run eagerly (eager=True; src_idx None)
             if self.recurrent:
                 T = self.nsteps
                 E = int(np.shape(states)[0])
