@@ -615,3 +615,105 @@ def vecnorm_add_latency(f64, n, out):
     """out float64 [2]: out[0] = SM cycles per dependent add (float64 if f64), over n adds in one thread."""
     _chk(out, torch.float64, "out")
     _lib.call("b200rl_vecnorm_add_latency", int(bool(f64)), int(n), _ptr(out), _stream(), label="vecnorm_add_latency")
+
+
+# ---- DDPG (csrc/ddpg.cu) ---------------------------------------------------------------------------------------------
+def ddpg_encode(obs, out, B, obs_dim, in_pad, sel=None, limit=0, mean=None, std=None, clip=5.0, act=None, act_sel=False,
+                nA=0, overflow=None):
+    """[clip(normalize(obs), +-clip) | action] -> fp16 [hi | lo] operand rows out [B, 2 * in_pad]; rows at the ring
+    selection sel ([start, idx...], int64) or row b; act: float32 [*, nA] rows (ring rows when act_sel) or None."""
+    for t, dt, nm in ((obs, torch.float32, "obs"), (out, torch.float16, "out"), (sel, torch.int64, "sel"),
+                      (mean, torch.float32, "mean"), (std, torch.float32, "std"), (act, torch.float32, "act"),
+                      (overflow, torch.int32, "overflow")):
+        _chk(t, dt, nm)
+    _lib.call("b200rl_ddpg_encode", _ptr(obs), _ptr(sel), int(limit), int(B), int(obs_dim), _ptr(mean), _ptr(std),
+              float(clip), _ptr(act), int(bool(act_sel)), int(nA), int(in_pad), _ptr(out), _ptr(overflow), _stream(),
+              label="ddpg_encode", nbytes=float(B) * (4.0 * (obs_dim + nA) + 4.0 * in_pad))
+
+
+def ddpg_tanh(z, ldz, mu, B, nA):
+    _chk(z, torch.float32, "z")
+    _chk(mu, torch.float32, "mu")
+    _lib.call("b200rl_ddpg_tanh", _ptr(z), int(ldz), _ptr(mu), int(B), int(nA), _stream(), label="ddpg_tanh")
+
+
+def ddpg_denorm(q, ldq, mean, std, out, B):
+    for t, nm in ((q, "q"), (mean, "mean"), (std, "std"), (out, "out")):
+        _chk(t, torch.float32, nm)
+    _lib.call("b200rl_ddpg_denorm", _ptr(q), int(ldq), _ptr(mean), _ptr(std), _ptr(out), int(B), _stream(),
+              label="ddpg_denorm")
+
+
+def ddpg_target(q1, ldq, sel, limit, rewards, terminals, mean, std, gamma, y, B):
+    for t, nm in ((q1, "q1"), (rewards, "rewards"), (terminals, "terminals"), (mean, "mean"), (std, "std"), (y, "y")):
+        _chk(t, torch.float32, nm)
+    _chk(sel, torch.int64, "sel")
+    _lib.call("b200rl_ddpg_target", _ptr(q1), int(ldq), _ptr(sel), int(limit), _ptr(rewards), _ptr(terminals),
+              _ptr(mean), _ptr(std), float(gamma), _ptr(y), int(B), _stream(), label="ddpg_target")
+
+
+def ddpg_loss(q, ldq, y, mean, std, B, dq, lddq, losses):
+    for t, nm in ((q, "q"), (y, "y"), (mean, "mean"), (std, "std"), (losses, "losses")):
+        _chk(t, torch.float32, nm)
+    _chk(dq, torch.float16, "dq")
+    _lib.call("b200rl_ddpg_loss", _ptr(q), int(ldq), _ptr(y), _ptr(mean), _ptr(std), int(B), _ptr(dq), int(lddq),
+              _ptr(losses), _stream(), label="ddpg_loss")
+
+
+def ddpg_actor_dz(g, ldg, mu, B, nA, dz, lddz):
+    _chk(g, torch.float32, "g")
+    _chk(mu, torch.float32, "mu")
+    _chk(dz, torch.float16, "dz")
+    _lib.call("b200rl_ddpg_actor_dz", _ptr(g), int(ldg), _ptr(mu), int(B), int(nA), _ptr(dz), int(lddz), _stream(),
+              label="ddpg_actor_dz")
+
+
+def ddpg_l2(w, g, segs, reg, loss):
+    """segs: int64 device [nseg, 2] of (offset, length) into the flat w / g."""
+    for t, nm in ((w, "w"), (g, "g"), (loss, "loss")):
+        _chk(t, torch.float32, nm)
+    _chk(segs, torch.int64, "segs")
+    _lib.call("b200rl_ddpg_l2", _ptr(w), _ptr(g), _ptr(segs), int(segs.shape[0]), float(reg), _ptr(loss), _stream(),
+              label="ddpg_l2")
+
+
+def ddpg_polyak(t0, s0, tau, t1=None, s1=None, init=False):
+    for t, nm in ((t0, "t0"), (s0, "s0"), (t1, "t1"), (s1, "s1")):
+        _chk(t, torch.float32, nm)
+    if s0.numel() != t0.numel() or (t1 is not None and s1.numel() != t1.numel()):
+        raise RuntimeError("ddpg_polyak: source and target sizes differ")
+    _lib.call("b200rl_ddpg_polyak", _ptr(t0), _ptr(s0), t0.numel(), _ptr(t1), _ptr(s1),
+              0 if t1 is None else t1.numel(), float(tau), int(bool(init)), _stream(), label="ddpg_polyak",
+              nbytes=12.0 * (t0.numel() + (0 if t1 is None else t1.numel())))
+
+
+def ddpg_obs_rms(x, pos0, limit, n, D, st, mean, std):
+    _chk(x, torch.float32, "x")
+    _chk(st, torch.float64, "st")
+    _chk(mean, torch.float32, "mean")
+    _chk(std, torch.float32, "std")
+    _lib.call("b200rl_ddpg_obs_rms", _ptr(x), int(pos0), int(limit), int(n), int(D), _ptr(st), _ptr(mean), _ptr(std),
+              _stream(), label="ddpg_obs_rms")
+
+
+def ddpg_ret_rms(y, B, st, mean, std, popart=None):
+    """popart: (w0, b0, w1, b1) float32 device views of the critic's and the target critic's output layers, or None."""
+    _chk(y, torch.float32, "y")
+    _chk(st, torch.float64, "st")
+    w0 = b0 = w1 = b1 = None
+    if popart is not None:
+        w0, b0, w1, b1 = popart
+        for t, nm in ((w0, "w0"), (b0, "b0"), (w1, "w1"), (b1, "b1")):
+            _chk(t, torch.float32, nm)
+    _lib.call("b200rl_ddpg_ret_rms", _ptr(y), int(B), _ptr(st), _ptr(mean), _ptr(std), _ptr(w0), _ptr(b0), _ptr(w1),
+              _ptr(b1), 0 if w0 is None else w0.numel(), _stream(), label="ddpg_ret_rms")
+
+
+def ddpg_pn_adapt(mu, mu_adapt, n, desired, stddev, stddev32, dist):
+    _chk(mu, torch.float32, "mu")
+    _chk(mu_adapt, torch.float32, "mu_adapt")
+    _chk(stddev, torch.float64, "stddev")
+    _chk(stddev32, torch.float32, "stddev32")
+    _chk(dist, torch.float32, "dist")
+    _lib.call("b200rl_ddpg_pn_adapt", _ptr(mu), _ptr(mu_adapt), int(n), float(desired), _ptr(stddev), _ptr(stddev32),
+              _ptr(dist), _stream(), label="ddpg_pn_adapt")

@@ -311,6 +311,52 @@ int b200rl_vecnorm_rewards(const void* rew, int rew_f64, const uint8_t* news, lo
  * out[0] = SM cycles per add.  out[1] seeds the chain (and receives its end). */
 int b200rl_vecnorm_add_latency(int f64, long long n, double* out, void* stream);
 
+/* DDPG (ddpg/ddpg_learner.py, ddpg/models.py), csrc/ddpg.cu.  The replay ring (ddpg/memory.py RingBuffer) holds float32
+ * rows obs [limit, obs_dim], actions [limit, nA], rewards [limit], terminals [limit]; a ring selection `sel` is the
+ * int64 device vector [start, idx_0 .. idx_{B-1}], sample b reads ring row (start + idx_b) % limit.
+ * encode: fp16 [hi | lo] operand rows out [B, 2*in_pad] of [clip(normalize(obs), +-clip) | action] (:17-20, :108-111,
+ *   models.py:43); normalize is (x - mean) / (std + 1e-8) when mean/std are given; act (may be NULL: obs-only rows)
+ *   holds [*, nA] float32 rows read at the ring row (act_sel = 1) or at row b (act_sel = 0).  sel NULL: row b.
+ *   overflow as in b200rl_obs_encode.
+ * tanh: mu [B, nA] = tanhf(z[b * ldz + j]).  denorm: out[b] = q[b * ldq] * std + mean (mean NULL: q).
+ * target: y[b] = r + (1 - d) * gamma * (Q'[b] * std + mean) (:134-135; mean NULL: Q'), r and d read at the ring row.
+ * loss: one CTA; rows [0, B) of q are Q(s, a), rows [B, 2B) Q(s, mu(s)).  losses[0] = mean((Q - (y - mean) / (std +
+ *   1e-8))^2), losses[1] = -mean(Q_mu * std + mean); dq (fp16, column 0 of row pitch lddq) = 2 (Q - y_n) on the first
+ *   B rows and -std (-1 when mean is NULL) on the second: gradients of the sums, the backward scales by 1/B.
+ * actor_dz: dz[b, j] = fp16(g[b, j] * (1 - mu[b, j]^2)).
+ * l2: one CTA; segs = nseg int64 pairs {offset, len} into w / g; g += reg * w and *loss += sum_s reg * sum(w_s^2) / 2.
+ * polyak: t <- float32(1 - tau) * t + float32(tau) * s over (t0, s0, n0) and (t1, s1, n1) (t1 may be NULL), or t <- s
+ *   when init.
+ * obs_rms: one CTA; RunningMeanStd state st float64 [sum(D) | sumsq(D) | count] updated by each of the n rows x[(pos0 +
+ *   i) % limit] in order, then mean = float32(sum / count), std = sqrtf(max(float32(sumsq / count) - mean^2, 1e-2f))
+ *   (common/mpi_running_mean_std.py:29-48).
+ * ret_rms: one CTA; the same state with D = 1 updated once by the B values y (numpy's pairwise sums in float64), then
+ *   with w0 given Pop-Art (:205-221) on the K-element output kernels w0, w1 and biases b0, b1.
+ * pn_adapt: one CTA; *dist = sqrtf(mean((mu - mu_adapt)^2)) over n elements; *stddev (float64) /= 1.01 when dist >
+ *   desired, else *= 1.01; *stddev32 = float32(*stddev) (noise.py:12-18). */
+int b200rl_ddpg_encode(const float* obs, const long long* sel, long long limit, long long B, int obs_dim,
+                       const float* mean, const float* std, float clip, const float* act, int act_sel, int nA,
+                       int in_pad, void* out, int* overflow, void* stream);
+int b200rl_ddpg_tanh(const float* z, long long ldz, float* mu, long long B, int nA, void* stream);
+int b200rl_ddpg_denorm(const float* q, long long ldq, const float* mean, const float* std, float* out, long long B,
+                       void* stream);
+int b200rl_ddpg_target(const float* q1, long long ldq, const long long* sel, long long limit, const float* rewards,
+                       const float* terminals, const float* mean, const float* std, float gamma, float* y, long long B,
+                       void* stream);
+int b200rl_ddpg_loss(const float* q, long long ldq, const float* y, const float* mean, const float* std, int B,
+                     void* dq, long long lddq, float* losses, void* stream);
+int b200rl_ddpg_actor_dz(const float* g, long long ldg, const float* mu, long long B, int nA, void* dz,
+                         long long lddz, void* stream);
+int b200rl_ddpg_l2(const float* w, float* g, const long long* segs, int nseg, float reg, float* loss, void* stream);
+int b200rl_ddpg_polyak(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1, double tau,
+                       int init, void* stream);
+int b200rl_ddpg_obs_rms(const float* x, long long pos0, long long limit, long long n, int D, double* st, float* mean,
+                        float* std, void* stream);
+int b200rl_ddpg_ret_rms(const float* y, long long B, double* st, float* mean, float* std, float* w0, float* b0,
+                        float* w1, float* b1, int K, void* stream);
+int b200rl_ddpg_pn_adapt(const float* mu, const float* mu_adapt, long long n, double desired, double* stddev,
+                         float* stddev32, float* dist, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
