@@ -8,7 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200rl.so")
 SOURCES = ["api.cu", "gemm_wgmma.cu", "conv_shift.cu", "gae.cu", "conv_lowering.cu", "policy_heads.cu", "optim.cu", "replay.cu", "obs_encode.cu",
-           "lstm.cu", "layer_norm.cu", "param_noise.cu", "vec_normalize.cu", "ddpg.cu"]
+           "lstm.cu", "layer_norm.cu", "param_noise.cu", "vec_normalize.cu", "ddpg.cu",
+           "her.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

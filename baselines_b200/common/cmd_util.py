@@ -6,9 +6,12 @@ Ids registered in baselines_b200.envs are built without gym; any other id goes t
 import argparse
 import os
 
+import numpy as np
+
 from .. import logger
 from ..bench import Monitor
 from .misc_util import set_global_seeds
+from . import spaces
 from .vec_env import DummyVecEnv, SubprocVecEnv
 
 
@@ -39,6 +42,32 @@ class ClipActionsWrapper:
 
     def reset(self, **kwargs):
         return self.env.reset(**kwargs)
+
+
+class FlattenObservation:
+    """gym.wrappers.FlattenObservation: a Dict observation as the concatenation of its parts in key order."""
+
+    def __init__(self, env):
+        self.env = env
+        parts = env.observation_space.spaces
+        n = sum(int(np.prod(s.shape)) for s in parts.values())
+        self.observation_space = spaces.Box(-np.inf, np.inf, (n,), np.float32)
+        self.action_space = env.action_space
+
+    def __getattr__(self, name):
+        if name.startswith('_'):
+            raise AttributeError(name)
+        return getattr(self.env, name)
+
+    def _flat(self, ob):
+        return np.concatenate([np.asarray(ob[k], np.float32).ravel() for k in self.env.observation_space.spaces])
+
+    def step(self, action):
+        ob, rew, done, info = self.env.step(action)
+        return self._flat(ob), rew, done, info
+
+    def reset(self, **kwargs):
+        return self._flat(self.env.reset(**kwargs))
 
 
 class RewardScaler:
@@ -84,6 +113,8 @@ def make_env(env_id, env_type, mpi_rank=0, subrank=0, seed=None, reward_scale=1.
             raise NotImplementedError("gym atari / retro ids need the reference's emulator wrappers (out of scope)")
         env = gym.make(env_id, **env_kwargs)
     env.seed(seed + subrank if seed is not None else None)
+    if flatten_dict_observations and spaces.is_dict(env.observation_space):
+        env = FlattenObservation(env)
     env = Monitor(env, logger_dir and os.path.join(logger_dir, str(mpi_rank) + '.' + str(subrank)),
                   allow_early_resets=True)
     if hasattr(env.action_space, "low") and hasattr(env.action_space, "high"):

@@ -103,6 +103,35 @@ class MultiBinary:
         return f"MultiBinary({self.n})"
 
 
+class Dict:
+    """gym.spaces.Dict: a mapping of named spaces (goal environments: observation / achieved_goal / desired_goal)."""
+
+    def __init__(self, spaces):
+        from collections import OrderedDict
+        items = spaces.items() if isinstance(spaces, dict) else spaces
+        self.spaces = OrderedDict(sorted(items) if isinstance(spaces, dict) and
+                                  not isinstance(spaces, OrderedDict) else items)
+        self.shape, self.dtype = None, None
+
+    def seed(self, seed=None):
+        for s in self.spaces.values():
+            s.seed(seed)
+
+    def sample(self):
+        from collections import OrderedDict
+        return OrderedDict((k, s.sample()) for k, s in self.spaces.items())
+
+    def contains(self, x):
+        return isinstance(x, dict) and x.keys() == self.spaces.keys() and \
+            all(s.contains(x[k]) for k, s in self.spaces.items())
+
+    def __getitem__(self, key):
+        return self.spaces[key]
+
+    def __repr__(self):
+        return "Dict(" + ", ".join(f"{k}:{s}" for k, s in self.spaces.items()) + ")"
+
+
 def is_discrete(space):
     """Discrete: `.n` and a scalar shape (gym's MultiBinary also has `.n`, with shape (n,))."""
     return hasattr(space, "n") and not hasattr(space, "nvec") and tuple(getattr(space, "shape", ())) == ()
@@ -118,3 +147,7 @@ def is_multi_binary(space):
 
 def is_box(space):
     return hasattr(space, "low") and hasattr(space, "high")
+
+
+def is_dict(space):
+    return hasattr(space, "spaces") and isinstance(space.spaces, dict)

@@ -12,6 +12,28 @@ import torch
 from . import spaces
 
 
+def obs_space_info(obs_space):
+    """vec_env/util.py:obs_space_info: (keys, shapes, dtypes) of the observation's parts; a non-Dict space is the
+    single part None."""
+    if spaces.is_dict(obs_space):
+        subspaces = obs_space.spaces
+    else:
+        subspaces = {None: obs_space}
+    keys = list(subspaces.keys())
+    return keys, {k: tuple(subspaces[k].shape) for k in keys}, {k: np.dtype(subspaces[k].dtype) for k in keys}
+
+
+def dict_to_obs(obs_dict):
+    """vec_env/util.py:dict_to_obs: {None: array} -> array, any other dict as it is."""
+    if set(obs_dict.keys()) == {None}:
+        return obs_dict[None]
+    return obs_dict
+
+
+def _copy_obs_dict(obs):
+    return {k: np.copy(v) for k, v in obs.items()}
+
+
 class VecEnv(ABC):
     """vec_env.py:29-138: batched env; reset() -> obs[N,...]; step(a[N]) -> (obs, rews f32[N], dones bool[N], infos)."""
     closed = False
@@ -49,8 +71,9 @@ class DummyVecEnv(VecEnv):
         self.envs = [fn() for fn in env_fns]
         env = self.envs[0]
         super().__init__(len(self.envs), env.observation_space, env.action_space)
-        shp, dt = tuple(env.observation_space.shape), env.observation_space.dtype
-        self.buf_obs = np.zeros((self.num_envs,) + shp, dtype=dt)
+        self.spec = getattr(env, "spec", None)
+        self.keys, shapes, dtypes = obs_space_info(env.observation_space)
+        self.buf_obs = {k: np.zeros((self.num_envs,) + shapes[k], dtype=dtypes[k]) for k in self.keys}
         self.buf_dones = np.zeros((self.num_envs,), dtype=np.bool_)
         self.buf_rews = np.zeros((self.num_envs,), dtype=np.float32)
         self.buf_infos = [{} for _ in range(self.num_envs)]
@@ -65,13 +88,20 @@ class DummyVecEnv(VecEnv):
             obs, self.buf_rews[e], self.buf_dones[e], self.buf_infos[e] = self.envs[e].step(a)
             if self.buf_dones[e]:
                 obs = self.envs[e].reset()
-            self.buf_obs[e] = obs
-        return self.buf_obs.copy(), self.buf_rews.copy(), self.buf_dones.copy(), list(self.buf_infos)
+            self._save_obs(e, obs)
+        return self._obs_from_buf(), self.buf_rews.copy(), self.buf_dones.copy(), list(self.buf_infos)
 
     def reset(self):
         for e in range(self.num_envs):
-            self.buf_obs[e] = self.envs[e].reset()
-        return self.buf_obs.copy()
+            self._save_obs(e, self.envs[e].reset())
+        return self._obs_from_buf()
+
+    def _save_obs(self, e, obs):
+        for k in self.keys:
+            self.buf_obs[k][e] = obs if k is None else obs[k]
+
+    def _obs_from_buf(self):
+        return dict_to_obs(_copy_obs_dict(self.buf_obs))
 
 
 def _subproc_worker(remote, parent_remote, fns_pickled, obs_buf, first):
@@ -81,7 +111,11 @@ def _subproc_worker(remote, parent_remote, fns_pickled, obs_buf, first):
     parent_remote.close()
     fns = pickle.loads(fns_pickled) if isinstance(fns_pickled, bytes) else fns_pickled
     envs = [fn() for fn in fns]
-    view = obs_buf.numpy()
+    views = {k: b.numpy() for k, b in obs_buf.items()}
+
+    def put(i, ob):
+        for k, v in views.items():
+            v[i] = ob if k is None else ob[k]
     try:
         while True:
             cmd, data = remote.recv()
@@ -91,12 +125,12 @@ def _subproc_worker(remote, parent_remote, fns_pickled, obs_buf, first):
                     ob, rew, done, info = env.step(a)
                     if done:
                         ob = env.reset()                          # subproc_vec_env.py:8-12: auto-reset
-                    view[first + k] = ob
+                    put(first + k, ob)
                     out.append((rew, done, info))
                 remote.send(out)
             elif cmd == 'reset':
                 for k, env in enumerate(envs):
-                    view[first + k] = env.reset()
+                    put(first + k, env.reset())
                 remote.send(None)
             elif cmd == 'get_spaces_spec':
                 remote.send((envs[0].observation_space, envs[0].action_space, getattr(envs[0], "spec", None)))
@@ -136,10 +170,12 @@ class SubprocVecEnv(VecEnv):
                 probe.close()
         ob_space, ac_space = spaces
         super().__init__(nenvs, ob_space, ac_space)
-        dt = torch.from_numpy(np.zeros(1, dtype=ob_space.dtype)).dtype
-        self._obs = torch.zeros((nenvs,) + tuple(ob_space.shape), dtype=dt).share_memory_()
+        self.keys, shapes, dtypes = obs_space_info(ob_space)
+        self._bufs = {k: torch.zeros((nenvs,) + shapes[k], dtype=torch.from_numpy(np.zeros(1, dtypes[k])).dtype)
+                      .share_memory_() for k in self.keys}
+        self._obs = self._bufs[None] if self.keys == [None] else None
         self._pinned = False
-        if torch.cuda.is_available():
+        if torch.cuda.is_available() and self._obs is not None:
             try:
                 rc = torch.cuda.cudart().cudaHostRegister(self._obs.data_ptr(), self._obs.numel() * self._obs.element_size(), 0)
                 self._pinned = int(rc) == 0
@@ -152,7 +188,7 @@ class SubprocVecEnv(VecEnv):
             if context != 'fork':
                 import cloudpickle
                 payload = cloudpickle.dumps(fns)
-            proc = ctx.Process(target=_subproc_worker, args=(work_remote, remote, payload, self._obs, k * in_series),
+            proc = ctx.Process(target=_subproc_worker, args=(work_remote, remote, payload, self._bufs, k * in_series),
                                daemon=True)                  # a crashed parent must not leave workers behind
             proc.start()
             self.ps.append(proc)
@@ -171,7 +207,7 @@ class SubprocVecEnv(VecEnv):
         results = [r for remote in self.remotes for r in remote.recv()]
         self.waiting = False
         rews, dones, infos = zip(*results)
-        return self._obs.numpy(), np.asarray(rews, dtype=np.float32), np.asarray(dones, dtype=np.bool_), list(infos)
+        return self._obs_out(), np.asarray(rews, dtype=np.float32), np.asarray(dones, dtype=np.bool_), list(infos)
 
     def reset(self):
         assert not self.closed
@@ -179,7 +215,13 @@ class SubprocVecEnv(VecEnv):
             remote.send(('reset', None))
         for remote in self.remotes:
             remote.recv()
-        return self._obs.numpy()
+        return self._obs_out()
+
+    def _obs_out(self):
+        """The shared observation array itself, or a dict of copies of the parts of a Dict observation."""
+        if self._obs is not None:
+            return self._obs.numpy()
+        return {k: b.numpy().copy() for k, b in self._bufs.items()}
 
     def close(self):
         if self.closed:

@@ -9,6 +9,8 @@ reference's plumbing tests and the benchmark workload:
   CartPole-v0 / CartPole-v1              classic cart-pole of common/tests/test_cartpole.py:14 (gym's dynamics: Barto,
                                          Sutton & Anderson 1983, Euler step, tau = 0.02)
   SyntheticAtari-v0                      84x84x1 uint8 frames, 6 actions: the bench.py workload as a steppable env
+  PointReach-v0 / PointReachDense-v0     a goal environment (env type `robotics`) with the gym robotics interface:
+                                         a 2-D point reaching a goal, sparse / dense compute_reward (for her)
 """
 import math
 from collections import deque
@@ -63,6 +65,10 @@ class Env:
     def close(self):
         pass
 
+    @property
+    def unwrapped(self):
+        return self
+
 
 class TimeLimit(Env):
     """Episode cap (gym.wrappers.TimeLimit): done after max_episode_steps, flagged in info['TimeLimit.truncated']."""
@@ -93,6 +99,20 @@ class TimeLimit(Env):
 
     def close(self):
         self.env.close()
+
+    @property
+    def _max_episode_steps(self):
+        return self.max_episode_steps
+
+    @property
+    def unwrapped(self):
+        return self.env.unwrapped
+
+    def __getattr__(self, name):
+        # goal environments' compute_reward (gym.Wrapper forwards it); every other missing attribute stays missing
+        if name == 'compute_reward':
+            return getattr(self.env, name)
+        raise AttributeError(name)
 
 
 # ------------------------------------------------------------------------------------------------ identity envs
@@ -250,9 +270,64 @@ class SyntheticAtariEnv(Env):
                 bool(self.np_random.rand() < self.p_done), {})
 
 
+# ------------------------------------------------------------------------------------------------ goal envs
+class PointReachEnv(Env):
+    """A point in [-1, 1]^2 moved by actions in [-1, 1]^2 (step 0.1 per unit) towards a goal drawn uniformly in the
+    square, with the gym robotics goal interface (gym/envs/robotics/fetch_env.py): the observation is the dict of
+    `observation` (position, last action), `achieved_goal` (position) and `desired_goal`; compute_reward(achieved_goal,
+    desired_goal, info) is -(|ag - g| > distance_threshold) (sparse) or -|ag - g| (dense); info['is_success'] is 1 within
+    the threshold.  Episodes start at the origin.  With the sparse reward a random policy almost never sees a success,
+    so replay without relabelling learns little."""
+
+    def __init__(self, reward_type='sparse', distance_threshold=0.1, step_size=0.1):
+        self.reward_type, self.distance_threshold, self.step_size = reward_type, float(distance_threshold), step_size
+        box = lambda lo, hi, n: spaces.Box(lo, hi, (n,), np.float32)
+        self.observation_space = spaces.Dict([('achieved_goal', box(-1, 1, 2)), ('desired_goal', box(-1, 1, 2)),
+                                              ('observation', box(-1, 1, 4))])
+        self.action_space = box(-1, 1, 2)
+        self.action_space.seed(None)                  # space samples never draw from numpy's global stream
+        self.np_random = np.random.RandomState()
+        self.pos = np.zeros(2, np.float32)
+        self.vel = np.zeros(2, np.float32)
+        self.goal = np.zeros(2, np.float32)
+
+    def seed(self, seed=None):
+        self.np_random = np.random.RandomState(seed)
+        self.action_space.seed(seed)
+        return [seed]
+
+    def _obs(self):
+        return {'observation': np.concatenate([self.pos, self.vel]).astype(np.float32),
+                'achieved_goal': self.pos.copy(), 'desired_goal': self.goal.copy()}
+
+    def reset(self):
+        self.pos[:] = 0.0
+        self.vel[:] = 0.0
+        self.goal = self.np_random.uniform(-1, 1, 2).astype(np.float32)
+        return self._obs()
+
+    def step(self, action):
+        a = np.clip(np.asarray(action, np.float32).reshape(2), -1, 1)
+        self.vel = (self.step_size * a).astype(np.float32)
+        self.pos = np.clip(self.pos + self.vel, -1, 1).astype(np.float32)
+        obs = self._obs()
+        d = np.linalg.norm(obs['achieved_goal'] - self.goal, axis=-1)
+        info = {'is_success': np.float32(d < self.distance_threshold)}
+        reward = self.compute_reward(obs['achieved_goal'], self.goal, info)
+        return obs, reward, False, info
+
+    def compute_reward(self, achieved_goal, desired_goal, info):
+        d = np.linalg.norm(np.asarray(achieved_goal) - np.asarray(desired_goal), axis=-1)
+        if self.reward_type == 'sparse':
+            return -(d > self.distance_threshold).astype(np.float32)
+        return -d
+
+
 register("DiscreteIdentity-v0", DiscreteIdentityEnv, "identity", dim=10, episode_len=100)
 register("MultiDiscreteIdentity-v0", MultiDiscreteIdentityEnv, "identity", dims=(3, 3), episode_len=100)
 register("BoxIdentity-v0", BoxIdentityEnv, "identity", shape=(1,), episode_len=100)
 register("CartPole-v0", CartPoleEnv, "classic_control", max_episode_steps=200)
 register("CartPole-v1", CartPoleEnv, "classic_control", max_episode_steps=500)
 register("SyntheticAtari-v0", SyntheticAtariEnv, "atari")
+register("PointReach-v0", PointReachEnv, "robotics", max_episode_steps=50)
+register("PointReachDense-v0", PointReachEnv, "robotics", max_episode_steps=50, reward_type='dense')

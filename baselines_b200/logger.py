@@ -182,6 +182,10 @@ def info(*args):
 log = info
 
 
+def warn(*args):
+    info(*args)
+
+
 def dumpkvs():
     d = OrderedDict(_kvs)
     if d:
@@ -192,3 +196,8 @@ def dumpkvs():
     _kvs.clear()
     _counts.clear()
     return d
+
+
+# the names her.py and its config use (logger.py:461-463 of the reference)
+record_tabular = logkv
+dump_tabular = dumpkvs

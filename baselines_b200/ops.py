@@ -717,3 +717,89 @@ def ddpg_pn_adapt(mu, mu_adapt, n, desired, stddev, stddev32, dist):
     _chk(dist, torch.float32, "dist")
     _lib.call("b200rl_ddpg_pn_adapt", _ptr(mu), _ptr(mu_adapt), int(n), float(desired), _ptr(stddev), _ptr(stddev32),
               _ptr(dist), _stream(), label="ddpg_pn_adapt")
+
+
+# ---- HER (csrc/her.cu) ----------------------------------------------------------------------------------------------
+def her_sample(ring, sel, B, relative, clip_obs, o_mean, o_std, g_mean, g_std, norm_clip, max_u, reward_type,
+               threshold, r, xa, xta, pad_a, xc, xtc, pad_c, ag2_out=None, g_out=None, info_out=None):
+    """ring: (o, ag, g, u, info) float64 device tensors [S, T+1 or T, dim]; sel: int64 [B, 3] (episode, t, future_t)."""
+    o, ag, g, u, info = ring
+    for t, nm in ((o, "o"), (ag, "ag"), (g, "g"), (u, "u"), (info, "info"), (ag2_out, "ag2_out"), (g_out, "g_out"),
+                  (info_out, "info_out")):
+        _chk(t, torch.float64, nm)
+    for t, nm in ((o_mean, "o_mean"), (o_std, "o_std"), (g_mean, "g_mean"), (g_std, "g_std"), (max_u, "max_u"),
+                  (r, "r")):
+        _chk(t, torch.float32, nm)
+    for t, nm in ((xa, "xa"), (xta, "xta"), (xc, "xc"), (xtc, "xtc")):
+        _chk(t, torch.float16, nm)
+    _chk(sel, torch.int64, "sel")
+    T, ninfo = g.shape[1], (0 if info is None else info.shape[2])
+    _lib.call("b200rl_her_sample", _ptr(o), _ptr(ag), _ptr(g), _ptr(u), _ptr(info), int(T), int(o.shape[2]),
+              int(g.shape[2]), int(u.shape[2]), int(ninfo), _ptr(sel), int(B), int(bool(relative)), float(clip_obs),
+              _ptr(o_mean), _ptr(o_std), _ptr(g_mean), _ptr(g_std), float(norm_clip), _ptr(max_u), int(reward_type),
+              float(threshold), _ptr(r), _ptr(xa), _ptr(xta), int(pad_a), _ptr(xc), _ptr(xtc), int(pad_c),
+              _ptr(ag2_out), _ptr(g_out), _ptr(info_out), _stream(), label="her_sample")
+
+
+def her_obs_encode(o, g, n, o_mean, o_std, g_mean, g_std, norm_clip, xa, pad_a, xc=None, pad_c=0):
+    for t, nm in ((o, "o"), (g, "g"), (o_mean, "o_mean"), (o_std, "o_std"), (g_mean, "g_mean"), (g_std, "g_std")):
+        _chk(t, torch.float32, nm)
+    _chk(xa, torch.float16, "xa")
+    _chk(xc, torch.float16, "xc")
+    _lib.call("b200rl_her_obs_encode", _ptr(o), _ptr(g), int(n), int(o.shape[1]), int(g.shape[1]), _ptr(o_mean),
+              _ptr(o_std), _ptr(g_mean), _ptr(g_std), float(norm_clip), _ptr(xa), int(pad_a), _ptr(xc), int(pad_c),
+              _stream(), label="her_obs_encode")
+
+
+def her_pi(z, ldz, B, dimu, max_u, pi, xc=None, pad_c=0, col0=0):
+    for t, nm in ((z, "z"), (max_u, "max_u"), (pi, "pi")):
+        _chk(t, torch.float32, nm)
+    _chk(xc, torch.float16, "xc")
+    _lib.call("b200rl_her_pi", _ptr(z), int(ldz), int(B), int(dimu), _ptr(max_u), _ptr(pi), _ptr(xc), int(pad_c),
+              int(col0), _stream(), label="her_pi")
+
+
+def her_target(q, ldq, r, B, gamma, lo, hi, y):
+    for t, nm in ((q, "q"), (r, "r"), (y, "y")):
+        _chk(t, torch.float32, nm)
+    _lib.call("b200rl_her_target", _ptr(q), int(ldq), _ptr(r), int(B), float(gamma), float(lo), float(hi), _ptr(y),
+              _stream(), label="her_target")
+
+
+def her_loss(q, ldq, y, B, dq, lddq, loss, q_pi):
+    for t, nm in ((q, "q"), (y, "y"), (loss, "loss"), (q_pi, "q_pi")):
+        _chk(t, torch.float32, nm)
+    _chk(dq, torch.float16, "dq")
+    _lib.call("b200rl_her_loss", _ptr(q), int(ldq), _ptr(y), int(B), _ptr(dq), int(lddq), _ptr(loss), _ptr(q_pi),
+              _stream(), label="her_loss")
+
+
+def her_actor_dz(g, ldg, z, ldz, pi, B, dimu, max_u, action_l2, dz, lddz):
+    for t, nm in ((g, "g"), (z, "z"), (pi, "pi"), (max_u, "max_u")):
+        _chk(t, torch.float32, nm)
+    _chk(dz, torch.float16, "dz")
+    _lib.call("b200rl_her_actor_dz", _ptr(g), int(ldg), _ptr(z), int(ldz), _ptr(pi), int(B), int(dimu), _ptr(max_u),
+              float(action_l2), _ptr(dz), int(lddz), _stream(), label="her_actor_dz")
+
+
+def her_norm(o, ag, g, sel, N, relative, clip_obs, f32_o, f32_g, o_stats, g_stats, eps):
+    """o / ag / g: float64 episode arrays [S, T+1 or T, dim]; *_stats: (state [2D + 1], mean [D], std [D]) float32."""
+    for t, nm in ((o, "o"), (ag, "ag"), (g, "g")):
+        _chk(t, torch.float64, nm)
+    for t in tuple(o_stats) + tuple(g_stats):
+        _chk(t, torch.float32, "stats")
+    _chk(sel, torch.int64, "sel")
+    _lib.call("b200rl_her_norm", _ptr(o), _ptr(ag), _ptr(g), int(g.shape[1]), int(o.shape[2]), int(g.shape[2]),
+              _ptr(sel), int(N), int(bool(relative)), float(clip_obs), int(bool(f32_o)), int(bool(f32_g)),
+              _ptr(o_stats[0]), _ptr(o_stats[1]), _ptr(o_stats[2]), _ptr(g_stats[0]), _ptr(g_stats[1]),
+              _ptr(g_stats[2]), float(eps), _stream(), label="her_norm")
+
+
+def her_polyak(t0, s0, polyak, t1=None, s1=None):
+    for t, nm in ((t0, "t0"), (s0, "s0"), (t1, "t1"), (s1, "s1")):
+        _chk(t, torch.float32, nm)
+    if s0.numel() != t0.numel() or (t1 is not None and s1.numel() != t1.numel()):
+        raise RuntimeError("her_polyak: source and target sizes differ")
+    _lib.call("b200rl_her_polyak", _ptr(t0), _ptr(s0), t0.numel(), _ptr(t1), _ptr(s1),
+              0 if t1 is None else t1.numel(), float(polyak), _stream(), label="her_polyak",
+              nbytes=12.0 * (t0.numel() + (0 if t1 is None else t1.numel())))

@@ -3,7 +3,7 @@
 
 Command-line front end with the flags, defaults lookup and control flow of the reference's baselines/run.py:52-247
 (train / build_env / get_env_type / get_learn_function(_defaults) / parse_cmdline_kwargs / main).  Algorithms: the
-ones this package accelerates (ppo2, deepq).  Under `torchrun` every rank runs the same command (the reference's
+ones this package accelerates (ppo2, deepq, ddpg, her).  Under `torchrun` every rank runs the same command (the reference's
 `mpirun -np K python -m baselines.run ...`); only rank 0 logs and saves.
 """
 import multiprocessing
@@ -102,7 +102,9 @@ def build_env(args):
         return VecFrameStack(venv, 4)
     if args.alg == 'deepq':
         return make_env(env_id, env_type, seed=args.seed, reward_scale=args.reward_scale, logger_dir=logger.get_dir())
-    venv = make_vec_env(env_id, env_type, args.num_env or 1, args.seed, reward_scale=args.reward_scale)
+    flatten_dict_observations = args.alg not in {'her'}
+    venv = make_vec_env(env_id, env_type, args.num_env or 1, args.seed, reward_scale=args.reward_scale,
+                        flatten_dict_observations=flatten_dict_observations)
     if env_type == 'mujoco':
         venv = VecNormalize(venv)
     return venv

@@ -357,6 +357,50 @@ int b200rl_ddpg_ret_rms(const float* y, long long B, double* st, float* mean, fl
 int b200rl_ddpg_pn_adapt(const float* mu, const float* mu_adapt, long long n, double desired, double* stddev,
                          float* stddev32, float* dist, void* stream);
 
+/* HER (her/ddpg.py, her/her_sampler.py, her/normalizer.py, her/actor_critic.py), csrc/her.cu.  The episode ring
+ * (her/replay_buffer.py) holds float64 o [S, T+1, dimo], ag [S, T+1, dimg], g [S, T, dimg], u [S, T, dimu] and info
+ * [S, T, ninfo]; a sample `sel` is the int64 device array [B, 3] of (episode slot, t, future_t), future_t = -1 keeping
+ * the stored goal.
+ * sample: g = future_t >= 0 ? ag[ep, future_t] : g[ep, t]; reward_type 1 (sparse) r = -(|ag[ep, t+1] - g| >
+ *   threshold), 2 (dense) r = -|ag[ep, t+1] - g|, the norm in float64 with numpy's summation order; 0: r untouched.
+ *   Then o, o_2 = o[ep, t], o[ep, t+1] and g, g_2 (minus ag[ep, t], ag[ep, t+1] when relative) are clipped to
+ *   +-clip_obs in float64, rounded to float32, normalised as clip((x - mean) / std, +-norm_clip) and written as fp16
+ *   [hi | lo] rows: xa [B, 2*pad_a] = [o | g], xta = [o_2 | g_2], xc rows [0, B) = [o | g | u / max_u] and rows [B, 2B)
+ *   = [o | g] (action columns untouched), xtc [B, 2*pad_c] = [o_2 | g_2].  ag2_out / g_out (float64 [B, dimg]) and
+ *   info_out ([B, ninfo]) receive ag[ep, t+1], the relabelled g and info[ep, t] when given.
+ * obs_encode: xa (and xc when given) rows of [normalize(o) | normalize(g)] for n preprocessed float32 rows.
+ * pi: pi[b, j] = max_u[j] * tanhf(z[b * ldz + j]); with xc, pi / max_u into columns col0 + j of its rows.
+ * target: y = min(max(r + gamma * q, lo), hi).
+ * loss: one CTA; *loss = mean((y - Q)^2) over rows [0, B) of q; dq column 0 = -2 (y - Q) there and -1 on rows [B, 2B);
+ *   q_pi[b] = q[B + b].  Gradients of sums: the backward scales by 1/B.
+ * actor_dz: dz = fp16((g / max_u + 2 action_l2 (pi / max_u) / (max_u dimu)) * max_u * (1 - tanh(z)^2)).
+ * norm: two CTAs (o, g statistics, float32 state [sum(D) | sumsq(D) | count]); Normalizer.update over the N samples
+ *   of sel (float32 sums when f32_o / f32_g, else float64 sums rounded to float32), then recompute_stats: count += N,
+ *   sum += local, sumsq += local_sq, mean = sum / count, std = sqrt(max(eps^2, sumsq / count - mean^2)).
+ * polyak: t <- float32(polyak) * t + float32(1 - polyak) * s over (t0, s0, n0) and (t1, s1, n1) (t1 may be NULL). */
+int b200rl_her_sample(const double* o, const double* ag, const double* g, const double* u, const double* info, int T,
+                      int dimo, int dimg, int dimu, int ninfo, const long long* sel, int B, int relative,
+                      double clip_obs, const float* o_mean, const float* o_std, const float* g_mean,
+                      const float* g_std, float norm_clip, const float* max_u, int reward_type, double threshold,
+                      float* r, void* xa, void* xta, int pad_a, void* xc, void* xtc, int pad_c, double* ag2_out,
+                      double* g_out, double* info_out, void* stream);
+int b200rl_her_obs_encode(const float* o, const float* g, int n, int dimo, int dimg, const float* o_mean,
+                          const float* o_std, const float* g_mean, const float* g_std, float norm_clip, void* xa,
+                          int pad_a, void* xc, int pad_c, void* stream);
+int b200rl_her_pi(const float* z, long long ldz, int B, int dimu, const float* max_u, float* pi, void* xc, int pad_c,
+                  int col0, void* stream);
+int b200rl_her_target(const float* q, long long ldq, const float* r, int B, float gamma, float lo, float hi, float* y,
+                      void* stream);
+int b200rl_her_loss(const float* q, long long ldq, const float* y, int B, void* dq, long long lddq, float* loss,
+                    float* q_pi, void* stream);
+int b200rl_her_actor_dz(const float* g, long long ldg, const float* z, long long ldz, const float* pi, int B, int dimu,
+                        const float* max_u, float action_l2, void* dz, long long lddz, void* stream);
+int b200rl_her_norm(const double* o, const double* ag, const double* g, int T, int dimo, int dimg,
+                    const long long* sel, int N, int relative, double clip_obs, int f32_o, int f32_g, float* o_st,
+                    float* o_mean, float* o_std, float* g_st, float* g_mean, float* g_std, float eps, void* stream);
+int b200rl_her_polyak(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1, double polyak,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
