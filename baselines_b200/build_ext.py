@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200rl.so")
 SOURCES = ["api.cu", "gemm_wgmma.cu", "conv_shift.cu", "gae.cu", "conv_lowering.cu", "policy_heads.cu", "optim.cu", "replay.cu", "obs_encode.cu",
            "lstm.cu", "layer_norm.cu", "param_noise.cu", "vec_normalize.cu", "ddpg.cu",
-           "her.cu"]
+           "her.cu", "acer.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -20,7 +20,7 @@ class PolicyBuilder:
     policies.py:126).  Carries the architecture; `Model` instantiates it on a device."""
 
     def __init__(self, ob_space, ac_space, network, value_network=None, normalize_observations=False,
-                 **network_kwargs):
+                 estimate_q=False, **network_kwargs):
         if callable(network) and not isinstance(network, str):
             raise NotImplementedError("custom network callables build TF graphs in the reference; this learner "
                                       "supports the registry names 'cnn', 'mlp', 'conv_only', 'lstm', 'cnn_lstm'")
@@ -38,16 +38,18 @@ class PolicyBuilder:
         self.network = network
         self.value_network = "copy" if value_network == "copy" else None
         self.normalize_observations = bool(normalize_observations)
+        # policies.py:58-61: ACER's policy replaces the scalar value head 'vf' by a Q head 'q' of width nA
+        if estimate_q and not spaces.is_discrete(ac_space):
+            raise NotImplementedError("estimate_q=True needs a Discrete action space (policies.py:59)")
+        self.estimate_q = bool(estimate_q)
         self.network_kwargs = network_kwargs
 
 
 def build_policy(env, policy_network, value_network=None, normalize_observations=False, estimate_q=False,
                  **policy_kwargs):
     """Same call signature as the reference's build_policy (policies.py:121)."""
-    if estimate_q:
-        raise NotImplementedError("estimate_q is only used by ACER in the reference (out of scope)")
     return PolicyBuilder(env.observation_space, env.action_space, policy_network, value_network,
-                         normalize_observations, **policy_kwargs)
+                         normalize_observations, estimate_q, **policy_kwargs)
 
 
 def _pad(n, m):
@@ -119,23 +121,28 @@ class PolicyNet:
             store.add("pi/logstd", np.zeros((1, self.nout), np.float32))         # distributions.py:104
             store.map_tf(f"{scope}/pi/logstd:0", "pi/logstd", (1, self.nout))
         Lv = self.tower_vf.latent_dim if self.copy_vf else L
-        w_vf = nn.ortho_init((Lv, 1), 1.0, rng)                                # policies.py:63
+        # the value head: 'vf' [Lv, 1] (policies.py:63), or with estimate_q the Q head 'q' [Lv, nA] (:60); both fc()
+        # with init_scale 1, created after the 'pi' head
+        self.nv = self.nout if builder.estimate_q else 1
+        vname = "q" if builder.estimate_q else "vf"
+        w_vf = nn.ortho_init((Lv, self.nv), 1.0, rng)
+        nv = self.nv
         if self.copy_vf:
             self.head_pi = nn.Linear(store, "head_pi", L, self.nout, None, w_pi,
                                      tf_w=None if self.pi_identity else f"{scope}/pi/w:0",
                                      tf_b=None if self.pi_identity else f"{scope}/pi/b:0")
-            self.head_vf = nn.Linear(store, "head_vf", Lv, 1, None, w_vf,
-                                     tf_w=f"{scope}/vf/w:0", tf_b=f"{scope}/vf/b:0")
+            self.head_vf = nn.Linear(store, "head_vf", Lv, nv, None, w_vf,
+                                     tf_w=f"{scope}/{vname}/w:0", tf_b=f"{scope}/{vname}/b:0")
             self.head = None
         else:
             # fused [pi | vf] head: one skinny GEMM; TF variables are column slices of it
             n = self.nout
-            self.head = nn.Linear(store, "head", L, n + 1, None, np.concatenate([w_pi, w_vf], axis=1))
+            self.head = nn.Linear(store, "head", L, n + nv, None, np.concatenate([w_pi, w_vf], axis=1))
             if not self.pi_identity:
                 store.map_tf(f"{scope}/pi/w:0", "head/w", (L, n), col_slice=slice(0, n))
                 store.map_tf(f"{scope}/pi/b:0", "head/b", (n,), col_slice=slice(0, n))
-            store.map_tf(f"{scope}/vf/w:0", "head/w", (L, 1), col_slice=slice(n, n + 1))
-            store.map_tf(f"{scope}/vf/b:0", "head/b", (1,), col_slice=slice(n, n + 1))
+            store.map_tf(f"{scope}/{vname}/w:0", "head/w", (L, nv), col_slice=slice(n, n + nv))
+            store.map_tf(f"{scope}/{vname}/b:0", "head/b", (nv,), col_slice=slice(n, n + nv))
         # policies.py:133-137,182-185: float observations pass through clip((x - mean) / std, -5, 5) of a
         # RunningMeanStd (mpi_running_mean_std.py:11-33: float64 sum / sumsq / count variables, epsilon 1e-2).  Nothing
         # in ppo2 ever updates those statistics, so they stay at their initial values (mean 0, std 1) unless a
@@ -189,11 +196,11 @@ class PolicyNet:
             self.g0cat = torch.zeros(a.K, 2 * N, **f32)
         if self.head is not None:
             self.head.materialize()
-            self.ld_ho = _pad(self.nout + 1, 16)
+            self.ld_ho = _pad(self.nout + self.nv, 16)
             self.headout = torch.zeros(cap, self.ld_ho, **f32)
             self.pi_out, self.ld_pi = self.headout, self.ld_ho
             self.v_out, self.ld_v = self.headout[:, self.nout:], self.ld_ho
-            self.ld_dh = _pad(self.nout + 1, 64)
+            self.ld_dh = _pad(self.nout + self.nv, 64)
             self.dhead = torch.zeros(cap, self.ld_dh, **f16)                  # padding columns stay zero
             self.dpi, self.ld_dpi = self.dhead, self.ld_dh
             self.dv, self.ld_dv = self.dhead[:, self.nout:], self.ld_dh
@@ -202,12 +209,12 @@ class PolicyNet:
             self.head_vf.materialize()
             self.ld_pi = _pad(self.nout, 16)
             self.pi_out = torch.zeros(cap, self.ld_pi, **f32)
-            self.ld_v = 16
-            self.v_out = torch.zeros(cap, 16, **f32)
+            self.ld_v = _pad(self.nv, 16)
+            self.v_out = torch.zeros(cap, self.ld_v, **f32)
             self.ld_dpi = _pad(self.nout, 64)
             self.dpi = torch.zeros(cap, self.ld_dpi, **f16)
-            self.ld_dv = 64
-            self.dv = torch.zeros(cap, 64, **f16)
+            self.ld_dv = _pad(self.nv, 64)
+            self.dv = torch.zeros(cap, self.ld_dv, **f16)
         if self.pd == "gauss":
             self.logstd = self.store.views["pi/logstd"].view(-1)
             self.g_logstd = self.store.gviews["pi/logstd"].view(-1)
@@ -381,21 +388,26 @@ class PolicyNet:
                            returns, old_values, old_neglogp, self.adv_st, cliprange, ent_coef, vf_coef, self.dpi,
                            self.ld_dpi, self.dv, self.ld_dv, self.g_logstd, inv_M, self.stats, B,
                            cliprange_dev=clip_dev)
+        self.backward(B, inv_M)
+
+    def backward(self, B, alpha):
+        """Backward of the last forward from the head-output gradients in dpi / dv: every weight gradient accumulates
+        alpha * (its gradient of the sum over the B rows) into store.grads."""
         tp = self.tower_pi
         if self.head is not None:
-            self.head.wgrad(self._lat_pi, self._ld_lat_pi, self.dhead, self.ld_dh, B, inv_M)
+            self.head.wgrad(self._lat_pi, self._ld_lat_pi, self.dhead, self.ld_dh, B, alpha)
             self.head.dgrad(self.dhead, self.ld_dh, B, tp.dlatent, tp.ld_dlatent, saved=self._lat_pi,
                             ld_saved=self._ld_lat_pi, act=tp.latent_act)
-            tp.backward(B, inv_M)
+            tp.backward(B, alpha)
         else:
             tv = self.tower_vf
-            self.head_pi.wgrad(self._lat_pi, self._ld_lat_pi, self.dpi, self.ld_dpi, B, inv_M)
+            self.head_pi.wgrad(self._lat_pi, self._ld_lat_pi, self.dpi, self.ld_dpi, B, alpha)
             self.head_pi.dgrad(self.dpi, self.ld_dpi, B, tp.dlatent, tp.ld_dlatent, saved=self._lat_pi,
                                ld_saved=self._ld_lat_pi, act=tp.latent_act)
-            tp.backward(B, inv_M, skip_first_wgrad=self.fuse0)
-            self.head_vf.wgrad(self._lat_vf, self._ld_lat_vf, self.dv, self.ld_dv, B, inv_M)
+            tp.backward(B, alpha, skip_first_wgrad=self.fuse0)
+            self.head_vf.wgrad(self._lat_vf, self._ld_lat_vf, self.dv, self.ld_dv, B, alpha)
             self.head_vf.dgrad(self.dv, self.ld_dv, B, tv.dlatent, tv.ld_dlatent, saved=self._lat_vf,
                                ld_saved=self._ld_lat_vf, act=tv.latent_act)
-            tv.backward(B, inv_M, skip_first_wgrad=self.fuse0)
+            tv.backward(B, alpha, skip_first_wgrad=self.fuse0)
             if self.fuse0:
-                self._fused_first_wgrad(B, inv_M)
+                self._fused_first_wgrad(B, alpha)

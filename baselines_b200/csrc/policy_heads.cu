@@ -9,7 +9,7 @@
 //   * per-minibatch advantage moments (ppo2/model.py:136-139)
 // The rollout arrays are gathered in place through src_idx (no materialised minibatch, ppo2.py:165).
 #include "common.cuh"
-#include "philox.cuh"
+#include "cat_sample.cuh"
 
 namespace b200rl {
 
@@ -59,22 +59,7 @@ cat_step_kernel(const float* __restrict__ logits, long long ld, int nA, const in
     for (int j = lo; j < hi; ++j) m = fmaxf(m, l[j]);
     float z = 0.0f;
     for (int j = lo; j < hi; ++j) z += expf(l[j] - m);
-    float best = -INFINITY;
-    int a = lo;
-    for (int j = lo; j < hi; ++j) {
-      float u;
-      if (uniforms) {
-        u = uniforms[b * nA + j];
-      } else {
-        if ((j >> 2) != held) {
-          held = j >> 2;
-          philox4(seed, (uint64_t)b, (uint32_t)held, (uint32_t)offset, rnd);
-        }
-        u = u01_open(rnd[j & 3]);
-      }
-      const float sc = l[j] - logf(-logf(u));
-      if (sc > best) { best = sc; a = j; }   // first max wins (tf.argmax)
-    }
+    const int a = cat_gumbel_argmax(l, lo, hi, nA, uniforms, seed, b, offset, rnd, held);
     actions[b * nseg + s] = a - lo;
     nlp += (m + logf(z)) - l[a];             // sum of the components' neglogp (distributions.py:86-87)
   }

@@ -803,3 +803,68 @@ def her_polyak(t0, s0, polyak, t1=None, s1=None):
     _lib.call("b200rl_her_polyak", _ptr(t0), _ptr(s0), t0.numel(), _ptr(t1), _ptr(s1),
               0 if t1 is None else t1.numel(), float(polyak), _stream(), label="her_polyak",
               nbytes=12.0 * (t0.numel() + (0 if t1 is None else t1.numel())))
+
+
+def acer_step(logits, ld, nA, actions, mu, B, seed=0, offset=0, offset_dev=None):
+    """ACER act: actions int64 [B] (the cat_step sampler's bits) and mu float32 [B, nA] = softmax(logits)."""
+    _chk(logits, torch.float32, "logits")
+    _chk(actions, torch.int64, "actions")
+    _chk(mu, torch.float32, "mu")
+    _chk(offset_dev, torch.int64, "offset_dev")
+    _lib.call("b200rl_acer_step", _ptr(logits), int(ld), int(nA), int(seed), int(offset), _ptr(offset_dev),
+              _ptr(actions), _ptr(mu), int(B), _stream(), label="acer_step", nbytes=float(B) * (8.0 * nA + 8.0))
+
+
+def acer_stack_obs(ring, idx, nenv, nsteps, nstack, dones_ring, out):
+    """_stack_obs of ring slot idx[e] of every env e (idx None: slot 0).  ring [slots, nenv, nsteps+nstack, *frame, nc]
+    uint8 / float32, dones_ring uint8 [slots, nenv, nsteps], out [nenv * (nsteps + 1), *frame, nstack * nc]."""
+    if ring.dtype not in (torch.uint8, torch.float32) or out.dtype != ring.dtype:
+        raise RuntimeError("acer_stack_obs: uint8 or float32 frames, and out of the same dtype")
+    _chk(dones_ring, torch.uint8, "dones_ring")
+    _chk(idx, torch.int64, "idx")
+    nc = int(ring.shape[-1])
+    F = int(ring[0, 0, 0].numel()) // nc
+    if ring.shape[1] != nenv or ring.shape[2] != nsteps + nstack or out.numel() != nenv * (nsteps + 1) * F * nstack * nc:
+        raise RuntimeError("acer_stack_obs: ring / out shapes do not match nenv, nsteps, nstack")
+    _lib.call("b200rl_acer_stack_obs", _ptr(ring), int(ring.dtype == torch.float32), int(ring[0].numel()), _ptr(idx),
+              int(nenv), int(nsteps), int(nstack), F, nc, _ptr(dones_ring), _ptr(out), _stream(),
+              label="acer_stack_obs", nbytes=float(out.numel() * out.element_size()) * 2.0)
+
+
+def acer_take(idx, nenv, nsteps, nA, rings, outs):
+    """Buffer.take of the per-step arrays: rings / outs = (actions int64, rewards f32, mus f32, dones u8, masks u8)."""
+    for ts in (rings, outs):
+        for t, dt, nm in zip(ts, (torch.int64, torch.float32, torch.float32, torch.uint8, torch.uint8),
+                             ("actions", "rewards", "mus", "dones", "masks")):
+            _chk(t, dt, nm)
+    _chk(idx, torch.int64, "idx")
+    _lib.call("b200rl_acer_take", _ptr(idx), int(nenv), int(nsteps), int(nA), *[_ptr(t) for t in rings],
+              *[_ptr(t) for t in outs], _stream(), label="acer_take")
+
+
+def acer_loss(pi, ldpi, q, ldq, pol, ldpol, actions, rewards, dones, mus, nenv, nsteps, nA, gamma, c, delta, q_coef,
+              ent_coef, trust_region, dpi, lddpi, dq, lddq, stats, f_out=None, v_out=None, qret_out=None):
+    """acer.py:103-178 for nenv * (nsteps + 1) head rows; see include/b200rl.h."""
+    for t, nm in ((pi, "pi"), (q, "q"), (pol, "pol"), (rewards, "rewards"), (mus, "mus"), (f_out, "f_out"),
+                  (v_out, "v_out"), (qret_out, "qret_out")):
+        _chk(t, torch.float32, nm)
+    _chk(actions, torch.int64, "actions")
+    _chk(dones, torch.uint8, "dones")
+    _chk(dpi, torch.float16, "dpi")
+    _chk(dq, torch.float16, "dq")
+    _chk(stats, torch.float64, "stats")
+    _lib.call("b200rl_acer_loss", _ptr(pi), int(ldpi), _ptr(q), int(ldq), _ptr(pol), int(ldpol), _ptr(actions),
+              _ptr(rewards), _ptr(dones), _ptr(mus), int(nenv), int(nsteps), int(nA), float(gamma), float(c),
+              float(delta), float(q_coef), float(ent_coef), int(bool(trust_region)), _ptr(dpi), int(lddpi), _ptr(dq),
+              int(lddq), _ptr(stats), _ptr(f_out), _ptr(v_out), _ptr(qret_out), _stream(), label="acer_loss")
+
+
+def clip_rmsprop_ema(p, g, ms, shadow, lr_dev, clip, sumsq_buf, decay, eps, alpha):
+    """Global-norm clip + TF RMSProp (momentum 0) + Polyak moving average of the updated parameters, one pass."""
+    for t, nm in ((p, "p"), (g, "g"), (ms, "ms"), (shadow, "shadow"), (lr_dev, "lr_dev")):
+        _chk(t, torch.float32, nm)
+    if not (p.numel() == g.numel() == ms.numel() == shadow.numel()):
+        raise RuntimeError("clip_rmsprop_ema: buffer sizes differ")
+    _lib.call("b200rl_clip_rmsprop_ema", _ptr(p), _ptr(g), _ptr(ms), _ptr(shadow), p.numel(), _ptr(lr_dev),
+              float(clip if clip else 0.0), _ptr(sumsq_buf), float(decay), float(eps), float(alpha), _stream(),
+              label="clip_rmsprop_ema", nbytes=20.0 * p.numel())

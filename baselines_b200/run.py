@@ -3,7 +3,7 @@
 
 Command-line front end with the flags, defaults lookup and control flow of the reference's baselines/run.py:52-247
 (train / build_env / get_env_type / get_learn_function(_defaults) / parse_cmdline_kwargs / main).  Algorithms: the
-ones this package accelerates (ppo2, deepq, ddpg, her).  Under `torchrun` every rank runs the same command (the reference's
+ones this package accelerates (ppo2, deepq, ddpg, her, acer).  Under `torchrun` every rank runs the same command (the reference's
 `mpirun -np K python -m baselines.run ...`); only rank 0 logs and saves.
 """
 import multiprocessing

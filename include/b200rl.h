@@ -401,6 +401,40 @@ int b200rl_her_norm(const double* o, const double* ag, const double* g, int T, i
 int b200rl_her_polyak(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1, double polyak,
                       void* stream);
 
+/* ACER (acer/acer.py, acer/buffer.py), csrc/acer.cu.
+ * step: actions int64 [B] = the Gumbel-max sample of b200rl_cat_step (same bits for the same seed / offset) and
+ *   mu float32 [B, nA] = softmax(logits) (acer.py:105,214).
+ * stack_obs: the replay ring holds frames [slots, nenv, nsteps + nstack, F, nc] (uint8, or float32 when f32) and
+ *   dones uint8 [slots, nenv, nsteps]; for env e it reads slot idx[e] (idx NULL: slot 0) and writes the stacked
+ *   observations of _stack_obs (buffer.py:124-140) to out [nenv * (nsteps + 1), F, nstack * nc], row e*(nsteps+1)+t.
+ * take: the slot's actions int64 / rewards float32 / dones uint8 [nenv, nsteps], mus [nenv, nsteps, nA] and masks uint8
+ *   [nenv, nsteps + 1], gathered like Buffer.take.
+ * loss: acer.py:103-178 over rows e*(nsteps+1)+t of the train head outputs pi / q and the Polyak logits pol; actions,
+ *   rewards, dones, mus are step rows e*nsteps+t.  dpi / dq (fp16, nA columns) get N * d loss / d [logits | q],
+ *   N = nenv * nsteps, zero on each env's last row.  stats float64 [12]: loss, loss_q, entropy, loss_policy, loss_f,
+ *   loss_bc, explained_variance, avg_norm_k, avg_norm_g, avg_norm_k_dot_g, avg_norm_adj, avg_norm_grads_f (the last
+ *   five use adj = 0 when trust_region is 0).  f_out [rows, nA], v_out [rows], qret_out [N] may be NULL.
+ *   The statistics are reduced through one device-wide scratch and completion counter, like b200rl_sumsq's: at most
+ *   one acer_loss launch may be in flight per device (issue them on one stream).
+ * clip_rmsprop_ema: g *= clip / max(sqrt(sumsq[0]), clip) (clip <= 0: none); TF RMSProp with momentum 0
+ *   ms += (g^2 - ms) (1 - decay), p -= lr g / sqrt(ms + eps), lr read from lr_dev; then the moving average
+ *   shadow -= (shadow - p) (1 - alpha) of the updated parameters. */
+int b200rl_acer_step(const float* logits, long long ld, int nA, unsigned long long seed, unsigned long long offset,
+                     const unsigned long long* offset_dev, long long* actions, float* mu, long long B, void* stream);
+int b200rl_acer_stack_obs(const void* ring, int f32, long long slot_stride, const long long* idx, int nenv, int nsteps,
+                          int nstack, long long F, int nc, const uint8_t* dones_ring, void* out, void* stream);
+int b200rl_acer_take(const long long* idx, int nenv, int nsteps, int nA, const long long* actions_ring,
+                     const float* rewards_ring, const float* mus_ring, const uint8_t* dones_ring,
+                     const uint8_t* masks_ring, long long* actions, float* rewards, float* mus, uint8_t* dones,
+                     uint8_t* masks, void* stream);
+int b200rl_acer_loss(const float* pi, long long ldpi, const float* q, long long ldq, const float* pol, long long ldpol,
+                     const long long* actions, const float* rewards, const uint8_t* dones, const float* mus, int nenv,
+                     int nsteps, int nA, float gamma, float c, float delta, float q_coef, float ent_coef,
+                     int trust_region, void* dpi, long long lddpi, void* dq, long long lddq, double* stats,
+                     float* f_out, float* v_out, float* qret_out, void* stream);
+int b200rl_clip_rmsprop_ema(float* p, const float* g, float* ms, float* shadow, long long n, const float* lr_dev,
+                            float clip, const double* sumsq, float decay, float eps, float alpha, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
