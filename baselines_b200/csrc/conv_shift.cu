@@ -76,17 +76,6 @@ static constexpr int SH_WABYTES = SH_WROWS_K * 128;
 // N = 64 over 64 channels: QW = 3, so that a 3x3 conv's 9 chunks fit one 2-CTA cluster and X / dY are read once.
 __host__ __device__ constexpr int sh_wgrad_qw(int BN, int KH, bool u8) { return u8 ? 2 : BN == 32 ? 4 : KH == 1 ? 3 : 2; }
 
-// Ordered MMA issue of the two consumer warpgroups (barrier 0 is __syncthreads, 1 joins the consumer warps in the
-// wgrad).  Group g waits on barrier SH_ORDER_BAR + g for its turn and hands the turn over with an arrive on the other
-// group's barrier: every wait is matched by exactly one arrive, so neither group may skip one while the other waits.
-static constexpr int SH_ORDER_BAR = 2;
-__device__ __forceinline__ void order_wait(int wg) {
-  asm volatile("bar.sync %0, %1;" ::"r"(SH_ORDER_BAR + wg), "n"(SH_CONSUMER_WARPS * 32) : "memory");
-}
-__device__ __forceinline__ void order_pass(int wg) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(SH_ORDER_BAR + 1 - wg), "n"(SH_CONSUMER_WARPS * 32) : "memory");
-}
-
 // address map of an output / saved tensor: grid position (n, y, x) + column -> element offset
 struct AddrMap {
   int mode;              // 0: n*sN + y*sY + x*sX + col
@@ -187,9 +176,6 @@ __device__ __forceinline__ uint4 ldg_stream_v4(const void* p) {
                : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
                : "l"(p));
   return v;
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
 template <int TR, int STAGES>
@@ -300,31 +286,6 @@ struct ShiftParams {
 };
 
 // ------------------------------------------------------------------------------------------------ forward / dgrad
-// Epilogue transpose: the accumulator fragment of one warp (16 rows; thread t holds 2 columns of rows t/4 and t/4 + 8 per
-// 8-column block) goes through a per-warp scratch of 16 rows x 64 B so that each lane then holds 8 consecutive columns
-// of one row.  16-byte piece p of scratch row r lives at slot p ^ ((r >> 1) & 3): the 8 rows of one stmatrix matrix,
-// and the 8 lanes of a quarter-warp load, hit 8 distinct 16-byte slots of 128 B (no bank conflict).
-__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
-  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3])
-               : "memory");
-}
-__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-// (a plain uint4 store is split into four 4-byte stores by the compiler here)
-__device__ __forceinline__ void st_global_v4(void* p, const uint4& v) {
-  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
-// bits 2k, 2k + 1 of b8 -> 0xffff in the low / high half of the word (the mask of fp16 elements 2k, 2k + 1)
-__device__ __forceinline__ uint32_t mask_pair(uint32_t b8, int k) {
-  const uint32_t b = b8 >> (2 * k);
-  return ((b & 1u) | ((b & 2u) << 15)) * 0xffffu;
-}
-
 // Weights: [BN rows, taps*KH*64 columns (t, h, c)], all resident in shared memory as (t, h) sub-tiles of BN rows x 128 B.
 template <int BN, int KH, bool DACT, bool U8>
 __global__ void __launch_bounds__(sh_threads(U8), 1)

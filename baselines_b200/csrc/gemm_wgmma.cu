@@ -7,6 +7,14 @@
 //                from the accumulator registers
 //   warp 8     : TMA producer (tiled or IM2COL-mode cp.async.bulk.tensor -> swizzled smem ring, mbarrier tx)
 //
+// K-major plain GEMMs with the f16 / f32-store epilogue (forward and data gradient of fc layers) instead stage their
+// epilogue as conv_shift.cu does: the bias of a tile is read once into shared memory, each warp's fp16 fragment leaves
+// through a per-warp swizzled scratch (stmatrix) as 16-byte row pieces, the column remap is computed once per 16-column
+// chunk, a ReLU bit mask is staged by the producer warp with the tile's last k-block, and the fp16 saved activation is
+// read as 16-byte pieces (ldmatrix hands it back in the accumulator layout).  Where the accumulators fit (BN <= 128,
+// not the fp32 store at 128) they run the ping-pong schedule: each warpgroup takes whole tiles, even / odd, as two
+// m64 accumulators, and named barriers order the groups' MMA issue, so one group's epilogue overlaps the other's MMAs.
+//
 // The reduction dimension is processed in stages of 64 elements made of 64/CPT "taps" of CPT elements
 // (CPT = 64, 32 or 16 -> 128 B / 64 B / 32 B swizzled smem rows):
 //   plain GEMM      : a tap is a 64-wide K chunk                                 (CPT = 64)
@@ -23,6 +31,7 @@
 #include <stdlib.h>
 
 #include <map>
+#include <type_traits>
 #include <mutex>
 
 #include "common.cuh"
@@ -62,6 +71,8 @@ struct GemmParams {
   ConvCoords cv;
   ShuffleOut sh;
   bool vec32;               // f16 outputs: rows / columns aligned so that a column pair is one 4-byte store
+  bool vec16;               // staged epilogue: C and ldc allow 16-byte row pieces (8 fp16 / 4 fp32 columns)
+  bool saved16;             // staged epilogue: `saved` and ld_saved allow 16-byte row pieces
   int rm_C, rm_OW, rm_Wg;   // rm_C > 0: output column (pix*rm_C + c) is stored at ((pix/rm_OW)*rm_Wg + pix%rm_OW)*rm_C + c
   float* ws;                // MODE_F32_ATOMIC with splits > 1: split s stores its partial [M, N] at ws + s*M*N
 };
@@ -76,11 +87,43 @@ struct Cfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
+// Staged epilogue of the K-major plain instances (TMODE = MODE_F16_ACT, MODE_F16_DACT or MODE_F32_STORE), after the
+// barrier block: the ReLU bit mask of each stage (DACT: 128 rows x BN bits, filled with a tile's last k-block), then one
+// 16-row x 32-column fp16 transpose scratch per consumer warp (as in conv_shift.cu).
+__host__ __device__ constexpr bool staged_epi(bool mn_major, bool im2col, int tmode) {
+  return !mn_major && !im2col && (tmode == MODE_F16_ACT || tmode == MODE_F16_DACT || tmode == MODE_F32_STORE);
+}
+static constexpr int EPI_WARP_BYTES = 16 * 64;
+__host__ __device__ constexpr int staged_mask_bytes(int BN, int tmode) { return tmode == MODE_F16_DACT ? BM * BN / 8 : 0; }
+template <int BN, int TMODE>
+__host__ __device__ constexpr int staged_smem_bytes() {
+  return Cfg<BN>::STAGES * staged_mask_bytes(BN, TMODE) + CONSUMER_WARPS * EPI_WARP_BYTES;
+}
+// Ping-pong (each consumer warpgroup takes whole 128 x BN tiles, two m64 accumulators) where BN/2 * 2 accumulator
+// registers fit under the 168-register cap of 9 warps next to the epilogue's: BN = 256, and the fp32 store at BN = 128
+// (which would spill), keep the cooperative schedule (each group 64 rows of every tile).
+__host__ __device__ constexpr bool gemm_pingpong(int BN, int tmode) {
+  return BN <= 64 || (BN == 128 && tmode != MODE_F32_STORE);
+}
+
 // CPT: channels per tap (64 / 32 / 16); MN_MAJOR: wgrad layout; IM2COL: A operand through TMA im2col mode
 // BRES (K-major implicit conv only): the whole weight matrix (taps x [BN x CPT]) is loaded ONCE per CTA and
 // stays resident in shared memory; the ring then carries only the A (activation patch) tiles.
 static constexpr int BRES_STAGES = 7;
 static constexpr int BRES_B_BYTES = 80 * 1024;
+
+// Read-only global loads as volatile asm: the compiler keeps them in program order next to the epilogue's stmatrix /
+// ldmatrix instead of hoisting every chunk's load, whose registers the ping-pong accumulators cannot spare.
+__device__ __forceinline__ uint4 ld_nc_v4(const void* p) {
+  uint4 v;
+  asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ unsigned short ld_nc_u16(const void* p) {
+  unsigned short v;
+  asm volatile("ld.global.nc.u16 %0, [%1];" : "=h"(v) : "l"(p));
+  return v;
+}
 
 // Epilogue of one accumulator column pair (col, col + 1) of one row; `two`: col + 1 < N.
 __device__ __forceinline__ void gemm_epi_pair(const GemmParams& p, int mode, int split, int row, int col, float v0,
@@ -182,6 +225,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint64_t* full_bar = bars;                  // [STAGES]
   uint64_t* empty_bar = bars + STAGES;        // [STAGES]
   uint64_t* bres_bar = bars + 2 * STAGES;     // [1]
+  constexpr bool STAGED = staged_epi(MN_MAJOR, IM2COL, TMODE);
+  constexpr bool PINGPONG = STAGED && gemm_pingpong(BN, TMODE);
+  constexpr int MASK_STAGE = STAGED ? staged_mask_bytes(BN, TMODE) : 0;
+  uint8_t* smask = reinterpret_cast<uint8_t*>(bars) + 256;      // STAGED DACT: the mask rows of stage s's tile
+  uint8_t* sepi = smask + STAGES * MASK_STAGE;                  // STAGED: epilogue scratch, one per consumer warp
+  __shared__ float s_bias[2][STAGED ? BN : 1];                  // STAGED: each group's copy of its tile's bias
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -190,7 +239,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CONSUMER_WARPS);
+      // a stage is released by the warps that read it: one group's 4 under ping-pong, both groups' 8 otherwise
+      mbar_init(&empty_bar[s], PINGPONG ? 4 : CONSUMER_WARPS);
     }
     mbar_init(bres_bar, 1);
     fence_barrier_init();
@@ -227,12 +277,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&empty_bar[s], ph ^ 1);
+        // STAGED DACT with the bit mask: the tile's mask rows travel with its last k-block (see below)
+        const bool mstage = MASK_STAGE > 0 && p.saved_bits != nullptr && kb + 1 == kb1;
         if (elect_one()) {
           uint8_t* sa = smem + s * STAGE_BYTES;
           uint8_t* sb = sa + C_::A_BYTES;
           if (!MN_MAJOR) {
             const int ntap = IM2COL ? min(TPS, p.cv.taps - kb * TPS) : TPS;
-            mbar_arrive_expect_tx(&full_bar[s], (uint32_t)ntap * (A_SUB + (BRES ? 0 : B_SUB)));
+            const uint32_t tx = (uint32_t)ntap * (A_SUB + (BRES ? 0 : B_SUB));
+            if (mstage) mbar_expect_tx(&full_bar[s], tx);
+            else mbar_arrive_expect_tx(&full_bar[s], tx);
 #pragma unroll
             for (int t = 0; t < TPS; ++t) {
               if (t < ntap) {
@@ -274,7 +328,238 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
         }
         __syncwarp();
+        if (mstage) {
+          // 128 rows x BN/16 words at row pitch ld_saved/16 words.  That pitch is a multiple of 2 bytes only (fc1 of
+          // NatureCNN: 392 B), which no tensor map or bulk copy takes, so the warp copies the words itself after issuing
+          // the stage's TMA loads, and arrives once they are in shared memory.  Rows >= M and words >= N/16 read 0.
+          constexpr int WPR = BN / 16;
+          uint16_t* dst = reinterpret_cast<uint16_t*>(smask + s * MASK_STAGE);
+          const int m0 = m_tile * BM, w0 = n_tile * WPR, nw = p.N >> 4;
+          const long long pitch = p.ld_saved >> 4;
+#pragma unroll 4
+          for (int i = lane; i < BM * WPR; i += 32) {
+            const int r = i / WPR, j = i % WPR;
+            dst[i] = (m0 + r < p.M && w0 + j < nw) ? __ldg(p.saved_bits + (long long)(m0 + r) * pitch + w0 + j)
+                                                   : (uint16_t)0;
+          }
+          __threadfence_block();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&full_bar[s]);
+        }
         if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+    }
+  } else if constexpr (STAGED) {
+    // ------------------------------------------------------------------ consumer warpgroups, staged epilogue
+    // Ping-pong: group wg takes the CTA's tiles i = wg, wg + 2, ... whole, as two m64 accumulators (tile rows [0, 64)
+    // and [64, 128)), and issues a tile's MMAs only after the other group has issued the previous tile's (order_wait /
+    // order_pass), so each group's epilogue runs while the tensor cores work on the other group's tile.  Cooperative:
+    // both groups take every tile, rows [64*wg, 64*wg + 64).  Thread t holds rows r0 and r0 + 8 of each accumulator.
+    constexpr int MH = PINGPONG ? 2 : 1;
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), t = threadIdx.x & 127;
+    const int row0 = PINGPONG ? 0 : wg * 64;
+    const int kbt = p.kb_total;                                      // one split: every tile runs all k-blocks
+    const int tile_count =
+        (int)blockIdx.x < total_work ? (total_work - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+    // After the transpose lane l holds columns 8 * (l >> 4) .. + 7 of each 16-column chunk of row er = l & 15 of the
+    // warp's 16 rows; that is also the row and piece whose address lane l hands to stmatrix / ldmatrix.
+    const int er = lane & 15, ep = lane >> 4;
+    const int erow = row0 + 16 * (warp & 3) + er;                    // tile row of accumulator 0 after the transpose
+    uint32_t epi_addr[2];
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj)
+      epi_addr[jj] = smem_u32(sepi + warp * EPI_WARP_BYTES) + er * 64 + (((2 * jj + ep) ^ ((er >> 1) & 3)) << 4);
+    const bool masked = TMODE == MODE_F16_DACT && p.saved_bits != nullptr;
+    const bool has_bias = TMODE != MODE_F16_DACT && p.bias != nullptr;
+    __half* Ch = reinterpret_cast<__half*>(p.C);
+    float acc[MH][BN / 2];
+    auto release = [&](int st) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[st]);
+    };
+    for (int i = PINGPONG ? wg : 0; i < tile_count; i += PINGPONG ? 2 : 1) {
+      const int work = (int)blockIdx.x + i * (int)gridDim.x;
+      const int n_tile = work % p.n_tiles, m_tile = work / p.n_tiles;
+      const int col0 = n_tile * BN;
+      if (has_bias) {                                                // the bias of the tile's columns, read once
+        asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");  // the group's previous epilogue is done with it
+        for (int c = t; c < BN; c += 128) s_bias[wg][c] = col0 + c < p.N ? __ldg(p.bias + col0 + c) : 0.0f;
+        asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");
+      }
+      const long long q0 = (long long)i * kbt;                       // stage sequence number of the tile's first k-block
+      int s = (int)(q0 % STAGES);
+      uint32_t ph = (uint32_t)(q0 / STAGES) & 1u;
+      if (PINGPONG && i > 0) order_wait(wg);                         // the other group has issued tile i - 1
+      int prev = -1;
+      for (int kb = 0; kb < kbt; ++kb) {
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t st = smem_u32(smem + s * STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int tp = 0; tp < TPS; ++tp) {
+#pragma unroll
+          for (int k = 0; k < CPT / MMA_K; ++k) {
+            const uint64_t bdesc = make_sdesc(st + C_::A_BYTES + tp * B_SUB + k * (MMA_K * 2), 16, 8 * ROWB, LAYOUT_A);
+#pragma unroll
+            for (int mh = 0; mh < MH; ++mh) {
+              const uint64_t adesc =
+                  make_sdesc(st + tp * A_SUB + (row0 + mh * 64) * ROWB + k * (MMA_K * 2), 16, 8 * ROWB, LAYOUT_A);
+              wgmma_f16<BN, 0, 0>(acc[mh], adesc, bdesc, (kb > 0 || tp > 0 || k > 0) ? 1u : 0u);
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0) release(prev);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      if (PINGPONG && i + 1 < tile_count) order_pass(wg);           // the other group may issue tile i + 1
+      wgmma_wait<0>();
+      if constexpr (TMODE == MODE_F32_STORE) {
+        release(prev);
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) {
+          // fp32: lanes q and q ^ 1 of a row quad swap pairs, so that each holds 4 consecutive columns of one row
+          const int q = t & 3;
+          const bool odd = q & 1;
+          const int orow = m_tile * BM + row0 + mh * 64 + 16 * (warp & 3) + (lane >> 2) + (odd ? 8 : 0);
+          float* Cf = reinterpret_cast<float*>(p.C) + (long long)orow * p.ldc;
+#pragma unroll
+          for (int b = 0; b < BN / 8; ++b) {
+            const int c = 8 * b + 2 * q;
+            const float b0 = has_bias ? s_bias[wg][c] : 0.0f, b1 = has_bias ? s_bias[wg][c + 1] : 0.0f;
+            const float f0 = fmaf(acc[mh][4 * b], p.alpha, b0), f1 = fmaf(acc[mh][4 * b + 1], p.alpha, b1);
+            const float f2 = fmaf(acc[mh][4 * b + 2], p.alpha, b0), f3 = fmaf(acc[mh][4 * b + 3], p.alpha, b1);
+            const float s0 = __shfl_xor_sync(0xffffffffu, odd ? f0 : f2, 1);
+            const float s1 = __shfl_xor_sync(0xffffffffu, odd ? f1 : f3, 1);
+            const float o[4] = {odd ? s0 : f0, odd ? s1 : f1, odd ? f2 : s0, odd ? f3 : s1};
+            const int oc = col0 + 8 * b + 2 * (q & ~1);
+            if (orow < p.M && oc < p.N) {
+              if (p.vec16 && oc + 4 <= p.N) {
+                st_global_v4(Cf + oc, make_uint4(__float_as_uint(o[0]), __float_as_uint(o[1]), __float_as_uint(o[2]),
+                                                 __float_as_uint(o[3])));
+              } else {
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                  if (oc + k < p.N) Cf[oc + k] = o[k];
+              }
+            }
+          }
+        }
+      } else {
+        // fp16 epilogue; the DACT mask and saved-activation variants are separate instantiations (MASKED), so that the
+        // registers of one are not live in the other
+        auto epi16 = [&](auto masked_c) {
+        constexpr bool MASKED = decltype(masked_c)::value;
+        // DACT with the bit mask: this lane's mask rows, staged with the last k-block.  The fence makes the loads
+        // complete before the stage is released (an arrive alone does not wait for another lane's shared-memory load
+        // in flight).
+        uint32_t mrow[MH][MASKED ? (BN + 31) / 32 : 1];
+        if constexpr (MASKED) {
+#pragma unroll
+          for (int mh = 0; mh < MH; ++mh) {
+            const uint32_t r = smem_u32(smask + prev * MASK_STAGE) + (uint32_t)((erow + mh * 64) * (BN / 8));
+#pragma unroll
+            for (int w = 0; w < BN / 32; ++w)
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(mrow[mh][w]) : "r"(r + 4 * w));
+          }
+          __threadfence_block();
+        }
+        release(prev);
+#pragma unroll
+        for (int mh = 0; mh < MH; ++mh) {
+          const int grow = m_tile * BM + erow + mh * 64;             // this lane's output row after the transpose
+          const bool rok = grow < p.M;
+#pragma unroll
+          for (int ps = 0; ps < BN / 32; ++ps) {                     // passes of 32 columns = two 16-column chunks
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj) {
+              // chunk 2 * ps + jj = 8-column blocks b, b + 1; stmatrix matrices (b, row t/4), (b, + 8), (b + 1, ...)
+              const int b = 2 * (2 * ps + jj);
+              // DACT with the fp16 saved activation: each lane reads its 16-byte piece of the chunk into the scratch,
+              // and ldmatrix hands every thread the values of its accumulator columns
+              uint32_t hs[4];
+              if constexpr (TMODE == MODE_F16_DACT && !MASKED) {
+                const int gc = col0 + 16 * (2 * ps + jj) + 8 * ep;
+                uint4 sv = make_uint4(0u, 0u, 0u, 0u);
+                if (rok && gc < p.N) {
+                  const __half* sp = p.saved + (long long)grow * p.ld_saved + gc;
+                  if (p.saved16 && gc + 8 <= p.N) {
+                    sv = ld_nc_v4(sp);
+                  } else {
+                    uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+                    for (int k = 0; k < 8; ++k)
+                      if (gc + k < p.N) w[k >> 1] |= (uint32_t)ld_nc_u16(sp + k) << (16 * (k & 1));
+                    sv = make_uint4(w[0], w[1], w[2], w[3]);
+                  }
+                }
+                st_shared_v4(epi_addr[jj], sv);
+                __syncwarp();
+                ldmatrix_x4(epi_addr[jj], hs);
+                __syncwarp();
+              }
+              uint32_t r[4];
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const int e = 4 * (b + (k >> 1)) + 2 * (k & 1);
+                const int c = 8 * (b + (k >> 1)) + 2 * (t & 3);
+                // per element and in the order of the unstaged epilogue: product with alpha, then bias and activation
+                // (ACT) or the activation's derivative (DACT), then one rounding to fp16
+                float v0 = __fmul_rn(acc[mh][e], p.alpha), v1 = __fmul_rn(acc[mh][e + 1], p.alpha);
+                if (TMODE == MODE_F16_ACT) {
+                  if (has_bias) {
+                    v0 = __fadd_rn(v0, s_bias[wg][c]);
+                    v1 = __fadd_rn(v1, s_bias[wg][c + 1]);
+                  }
+                  v0 = apply_act(v0, p.act);
+                  v1 = apply_act(v1, p.act);
+                } else if constexpr (!MASKED) {
+                  const __half2 h = *reinterpret_cast<const __half2*>(&hs[k]);
+                  v0 = __fmul_rn(v0, act_grad_from_saved(__low2float(h), p.act));
+                  v1 = __fmul_rn(v1, act_grad_from_saved(__high2float(h), p.act));
+                }
+                r[k] = h2_bits(__floats2half2_rn(v0, v1));
+              }
+              stmatrix_x4(epi_addr[jj], r);
+            }
+            __syncwarp();
+#pragma unroll
+            for (int jj = 0; jj < 2; ++jj) {
+              const int j = 2 * ps + jj;
+              uint4 v = ld_shared_v4(epi_addr[jj]);                 // columns 16 * j + 8 * ep .. + 7 of row er
+              if constexpr (MASKED) {                                // zeroing the rounded value gives what rounding
+                const uint32_t b8 = (mrow[mh][j >> 1] >> (16 * (j & 1) + 8 * ep)) & 0xffu;   // 0.0f gives: +0
+                v.x &= mask_pair(b8, 0);
+                v.y &= mask_pair(b8, 1);
+                v.z &= mask_pair(b8, 2);
+                v.w &= mask_pair(b8, 3);
+              }
+              const int gc = col0 + 16 * j + 8 * ep;
+              if (rok && gc < p.N) {
+                long long oc = gc;
+                if (p.rm_C > 0) {              // rm_C % 16 == 0: the chunk's 16 columns lie in one pixel, in order
+                  const int c16 = col0 + 16 * j, pix = c16 / p.rm_C;
+                  oc = (long long)((pix / p.rm_OW) * p.rm_Wg + pix % p.rm_OW) * p.rm_C + (c16 - pix * p.rm_C) + 8 * ep;
+                }
+                __half* out = Ch + (long long)grow * p.ldc + oc;
+                if (p.vec16 && gc + 8 <= p.N) {
+                  st_global_v4(out, v);
+                } else {
+                  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                  for (int k = 0; k < 8; ++k)
+                    if (gc + k < p.N) out[k] = __ushort_as_half((unsigned short)(w[k >> 1] >> (16 * (k & 1))));
+                }
+              }
+            }
+            __syncwarp();                                            // the scratch is rewritten by the next pass
+          }
+        }
+        };
+        if (TMODE == MODE_F16_DACT && masked) epi16(std::integral_constant<bool, TMODE == MODE_F16_DACT>{});
+        else epi16(std::false_type{});
       }
     }
   } else {
@@ -520,7 +805,8 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmPara
                   cudaStream_t stream) {
   using C_ = Cfg<BN>;
   constexpr int ZT = (IM2COL && !MN) ? BN * CPT * 2 : 0;    // zero weight tile of the implicit conv
-  constexpr int SMEM = (BRES ? (BRES_STAGES * C_::A_BYTES + BRES_B_BYTES + 1024 + 256) : C_::SMEM_BYTES) + ZT;
+  constexpr int SMEM = (BRES ? (BRES_STAGES * C_::A_BYTES + BRES_B_BYTES + 1024 + 256) : C_::SMEM_BYTES) + ZT +
+                       (staged_epi(MN, IM2COL, TMODE) ? staged_smem_bytes<BN, TMODE>() : 0);
   static_assert(SMEM <= 227 * 1024, "gemm: shared memory budget");
   static bool attr_set = false;
   auto kern = gemm_wgmma_kernel<BN, CPT, MN, IM2COL, BRES, TMODE>;
@@ -641,6 +927,8 @@ extern "C" int b200rl_gemm_f16(const void* A, const void* B, void* C, const floa
   p.vec32 = ((ldc & 15) == 0) && ((reinterpret_cast<uintptr_t>(C) & 31) == 0) && (rm_C == 0 || (rm_C & 15) == 0) &&
             (!saved || (((ld_saved & 15) == 0) && ((reinterpret_cast<uintptr_t>(saved) & 31) == 0)));
   B200RL_REQUIRE(saved_bits == nullptr || p.vec32, "gemm: saved_bits needs 32-byte aligned 16-column output chunks");
+  p.vec16 = ((reinterpret_cast<uintptr_t>(C) & 15) == 0) && (ldc % (mode == MODE_F32_STORE ? 4 : 8)) == 0;
+  p.saved16 = saved && ((reinterpret_cast<uintptr_t>(saved) & 15) == 0) && (ld_saved % 8) == 0;
 
   CUtensorMap tmA, tmB;
   int rc;
