@@ -366,9 +366,7 @@ extern "C" int b200rl_clip_rmsprop_ema(float* p, const float* g, float* ms, floa
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(p && g && ms && shadow && lr_dev && n > 0, "clip_rmsprop_ema: bad args");
   B200RL_REQUIRE(clip <= 0.0f || sumsq != nullptr, "clip_rmsprop_ema: clipping needs the device sumsq");
-  long long blocks = ceil_div_ll(n, 256);
-  if (blocks > 8LL * device_num_sms()) blocks = 8LL * device_num_sms();
-  clip_rmsprop_ema_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p, g, ms, shadow, n, lr_dev, clip, sumsq,
-                                                                1.0f - decay, eps, 1.0f - alpha);
+  clip_rmsprop_ema_kernel<<<grid_blocks(n, 256, 8), 256, 0, stream>>>(p, g, ms, shadow, n, lr_dev, clip, sumsq,
+                                                                      1.0f - decay, eps, 1.0f - alpha);
   return check_launch("clip_rmsprop_ema_kernel");
 }

@@ -42,6 +42,11 @@ float* det_workspace(size_t floats, cudaStream_t stream);
 // out[r * ldo + c] += sum_{p < parts} ws[(p * rows + r) * cols + c], parts summed in order
 int sum_partials(const float* ws, int parts, long long rows, int cols, float* out, long long ldo, cudaStream_t stream);
 int device_num_sms();   // streaming multiprocessors of the current device (grid sizing)
+// grid of a grid-stride kernel over `work` items: one thread per item, at most per_sm CTAs per SM, at least one CTA
+inline int grid_blocks(long long work, int threads, int per_sm) {
+  const long long blocks = ceil_div_ll(work, threads), cap = (long long)per_sm * device_num_sms();
+  return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
+}
 
 #ifdef __CUDACC__
 // ------------------------------------------------------------------ mbarrier / TMA / wgmma PTX
@@ -169,6 +174,41 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+// One CTA of N threads: thread 0 returns the N values v added in thread order from +0 (the others return 0).  red: N
+// floats of shared memory, free for reuse when the call returns.
+template <int N>
+__device__ __forceinline__ float cta_sum_in_order(float v, float* red) {
+  red[threadIdx.x] = v;
+  __syncthreads();
+  float t = 0.0f;
+  if (threadIdx.x == 0)
+    for (int k = 0; k < N; ++k) t = __fadd_rn(t, red[k]);
+  __syncthreads();
+  return t;
+}
+
+// ------------------------------------------------------------------ fp16 [hi | lo] operand rows (obs_encode.cu)
+// v = hi + lo with hi = fp16(v), lo = fp16(v - hi): v - hi is exact in fp32
+__device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {
+  const __half h = __float2half_rn(v);
+  hi = h;
+  lo = __float2half_rn(v - __half2float(h));
+}
+// some |v[j]| >= 65520, which rounds hi to +-inf (a NaN compares false: it passes through)
+__device__ __forceinline__ bool f16_overflow8(const float (&v)[8]) {
+  bool over = false;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) over |= fabsf(v[j]) >= 65520.0f;
+  return over;
+}
+// eight columns of an operand row [hi(0..in_pad) | lo(0..in_pad)]: o points at the first (16-byte aligned) hi column
+__device__ __forceinline__ void store_split_f16x8(__half* o, int in_pad, const float (&v)[8]) {
+  __align__(16) __half hi[8], lo[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) split_f16(v[j], hi[j], lo[j]);
+  *reinterpret_cast<uint4*>(o) = *reinterpret_cast<const uint4*>(hi);
+  *reinterpret_cast<uint4*>(o + in_pad) = *reinterpret_cast<const uint4*>(lo);
 }
 #endif  // __CUDACC__
 

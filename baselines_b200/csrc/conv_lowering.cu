@@ -7,7 +7,6 @@
 //             the activation derivative of the layer below
 //   colsum  : bias gradients
 // All HBM-bound: 16-byte vector accesses, consecutive lanes on consecutive 16 B chunks.
-#include <algorithm>
 #include "common.cuh"
 
 namespace b200rl {
@@ -248,12 +247,6 @@ colsum_vec_kernel(const __half* __restrict__ dz, float* __restrict__ part, long 
   }
 }
 
-static int grid_for(long long total, int threads) {
-  long long blocks = (total + threads - 1) / threads;
-  const long long cap = (long long)device_num_sms() * 32;
-  return (int)(blocks < cap ? (blocks < 1 ? 1 : blocks) : cap);
-}
-
 static int fill_geom(ConvGeom& g, int H, int W, int C, int rf, int stride, int same_pad) {
   g.H = H; g.W = W; g.C = C; g.rf = rf; g.stride = stride;
   if (same_pad) {
@@ -328,7 +321,7 @@ extern "C" int b200rl_im2col(const void* x, int src_is_u8, const long long* src_
   else
     B200RL_REQUIRE(C % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0, "im2col(f16): C must be a multiple of 8");
   const long long total = B * g.OH * g.OW * rf * ((rf * C) / 8);
-  const int grid = grid_for(total, 256);
+  const int grid = grid_blocks(total, 256, 32);
   if (src_is_u8)
     im2col_kernel<uint8_t><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(x), src_idx,
                                                      reinterpret_cast<__half*>(cols), B, g);
@@ -349,7 +342,7 @@ extern "C" int b200rl_frame_stack(const void* prev, const void* frame, const voi
                     (reinterpret_cast<uintptr_t>(frame) & 3) == 0;
   if (K == 4 && c == 1) {
     if (al16 && pixels % 4 == 0) {
-      const int grid = (int)std::min<long long>((total / 4 + 255) / 256, (long long)device_num_sms() * 16);
+      const int grid = grid_blocks(total / 4, 256, 16);
       frame_stack_k4_kernel<4><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint32_t*>(prev),
                                                         reinterpret_cast<const uint8_t*>(frame),
                                                         reinterpret_cast<const uint8_t*>(news),
@@ -357,14 +350,14 @@ extern "C" int b200rl_frame_stack(const void* prev, const void* frame, const voi
     } else {
       B200RL_REQUIRE(((reinterpret_cast<uintptr_t>(prev) | reinterpret_cast<uintptr_t>(out)) & 3) == 0,
                      "frame_stack: stacked buffers must be 4-byte aligned");
-      const int grid = (int)std::min<long long>((total + 255) / 256, (long long)device_num_sms() * 16);
+      const int grid = grid_blocks(total, 256, 16);
       frame_stack_k4_kernel<1><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint32_t*>(prev),
                                                         reinterpret_cast<const uint8_t*>(frame),
                                                         reinterpret_cast<const uint8_t*>(news),
                                                         reinterpret_cast<uint32_t*>(out), pixels, total);
     }
   } else {
-    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)device_num_sms() * 16);
+    const int grid = grid_blocks(total, 256, 16);
     frame_stack_generic_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(prev),
                                                         reinterpret_cast<const uint8_t*>(frame),
                                                         reinterpret_cast<const uint8_t*>(news),
@@ -382,7 +375,7 @@ extern "C" int b200rl_s2d_gather(const void* x, const long long* src_idx, void* 
                  "s2d_gather: need H,W multiples of s and s*C, W*C multiples of 8");
   const bool wide = ((s * C) % 16 == 0) && ((W * C) % 16 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0);
   const long long total = B * (H / s) * (W / s) * s * ((s * C) / (wide ? 16 : 8));
-  const int grid = grid_for((total + 3) / 4, 256);
+  const int grid = grid_blocks((total + 3) / 4, 256, 32);
   if (wide)
     s2d_gather_kernel<16><<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(x), src_idx,
                                                     reinterpret_cast<__half*>(out), B, H, W, C, s);
@@ -400,9 +393,9 @@ extern "C" int b200rl_col2im(const void* dcols, const void* saved, void* dx, lon
   B200RL_REQUIRE(fill_geom(g, H, W, C, rf, stride, same_pad) == 0, "col2im: empty output");
   B200RL_REQUIRE(C % 8 == 0, "col2im: C must be a multiple of 8");
   const long long total = B * H * W * (C / 8);
-  col2im_kernel<<<grid_for(total, 256), 256, 0, stream>>>(reinterpret_cast<const __half*>(dcols),
-                                                          reinterpret_cast<const __half*>(saved),
-                                                          reinterpret_cast<__half*>(dx), B, g, act);
+  col2im_kernel<<<grid_blocks(total, 256, 32), 256, 0, stream>>>(reinterpret_cast<const __half*>(dcols),
+                                                                  reinterpret_cast<const __half*>(saved),
+                                                                  reinterpret_cast<__half*>(dx), B, g, act);
   return check_launch("col2im_kernel");
 }
 

@@ -9,13 +9,13 @@
 //                      mu(s)))) (:174) with their head gradients
 //   ddpg_actor_dz      the actor's head gradient: dQ/dmu through tanh'
 //   ddpg_l2            the critic's L2 term over the `/w:0` variables outside `output` (:187-196)
-//   ddpg_polyak        target <- (1 - tau) target + tau online (:36-47)
 //   ddpg_obs_rms       mpi_running_mean_std RunningMeanStd.update once per stored row (:281-287) + mean / std
 //   ddpg_ret_rms       the same update over a target batch (:299), then Pop-Art on the critics' output layers (:205-221)
 //   ddpg_pn_adapt      sqrt(mean((mu - mu_adapt)^2)) (:170) and AdaptiveParamNoiseSpec.adapt (noise.py:12-18)
 // Every reduction runs in one CTA in a fixed order, so a step is deterministic run to run.  All of them are a few
-// thousand elements: the step is latency bound, and one launch per stage is what matters.
-#include "common.cuh"
+// thousand elements: the step is latency bound, and one launch per stage is what matters.  The soft target update
+// (:36-47) is b200rl_soft_update (optim.cu).
+#include "np_sum.cuh"
 
 namespace b200rl {
 
@@ -74,21 +74,8 @@ __global__ void __launch_bounds__(DD_THREADS) ddpg_encode_kernel(const DdpgEncod
       }
       v[j] = t;
     }
-    if (p.overflow) {
-      bool over = false;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) over |= fabsf(v[j]) >= 65520.0f;
-      if (over) *p.overflow = 1;
-    }
-    __align__(16) __half hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      hi[j] = __float2half_rn(v[j]);
-      lo[j] = __float2half_rn(v[j] - __half2float(hi[j]));
-    }
-    __half* o = p.out + b * (2LL * p.in_pad) + c0;
-    *reinterpret_cast<uint4*>(o) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(o + p.in_pad) = *reinterpret_cast<const uint4*>(lo);
+    if (p.overflow && f16_overflow8(v)) *p.overflow = 1;
+    store_split_f16x8(p.out + b * (2LL * p.in_pad) + c0, p.in_pad, v);
   }
 }
 
@@ -131,7 +118,7 @@ ddpg_target_kernel(const float* __restrict__ q1, long long ldq, const long long*
 __global__ void __launch_bounds__(DD_THREADS)
 ddpg_loss_kernel(const float* __restrict__ q, long long ldq, const float* __restrict__ y, const float* __restrict__ mean,
                  const float* __restrict__ std, int B, __half* __restrict__ dq, long long lddq, float* __restrict__ losses) {
-  __shared__ float red_c[DD_THREADS], red_a[DD_THREADS];
+  __shared__ float red[DD_THREADS];
   const float m = mean ? *mean : 0.0f, s = mean ? *std : 1.0f;
   float sc = 0.0f, sa = 0.0f;
   for (int b = threadIdx.x; b < B; b += DD_THREADS) {
@@ -143,15 +130,9 @@ ddpg_loss_kernel(const float* __restrict__ q, long long ldq, const float* __rest
     sa = __fadd_rn(sa, mean ? dd_denormalize(qa, m, s) : qa);
     dq[(long long)(B + b) * lddq] = __float2half_rn(-s);
   }
-  red_c[threadIdx.x] = sc;
-  red_a[threadIdx.x] = sa;
-  __syncthreads();
+  const float tc = cta_sum_in_order<DD_THREADS>(sc, red);
+  const float ta = cta_sum_in_order<DD_THREADS>(sa, red);
   if (threadIdx.x == 0) {
-    float tc = 0.0f, ta = 0.0f;
-    for (int k = 0; k < DD_THREADS; ++k) {
-      tc = __fadd_rn(tc, red_c[k]);
-      ta = __fadd_rn(ta, red_a[k]);
-    }
     losses[0] = __fdiv_rn(tc, (float)B);
     losses[1] = -__fdiv_rn(ta, (float)B);
   }
@@ -186,26 +167,10 @@ ddpg_l2_kernel(const float* __restrict__ w, float* __restrict__ g, const DdpgSeg
       acc = __fadd_rn(acc, __fmul_rn(v, v));
       g[sg.off + i] = __fadd_rn(g[sg.off + i], __fmul_rn(reg, v));
     }
-    red[threadIdx.x] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float t = 0.0f;
-      for (int k = 0; k < (int)blockDim.x; ++k) t = __fadd_rn(t, red[k]);
-      total = __fadd_rn(total, __fmul_rn(reg, __fmul_rn(t, 0.5f)));
-    }
-    __syncthreads();
+    const float t = cta_sum_in_order<1024>(acc, red);
+    if (threadIdx.x == 0) total = __fadd_rn(total, __fmul_rn(reg, __fmul_rn(t, 0.5f)));
   }
   if (threadIdx.x == 0) *loss = __fadd_rn(*loss, total);
-}
-
-__global__ void __launch_bounds__(DD_THREADS)
-ddpg_polyak_kernel(float* __restrict__ t0, const float* __restrict__ s0, long long n0, float* __restrict__ t1,
-                   const float* __restrict__ s1, long long n1, float keep, float tau, int init) {
-  float* t = blockIdx.y ? t1 : t0;
-  const float* s = blockIdx.y ? s1 : s0;
-  const long long n = blockIdx.y ? n1 : n0;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    t[i] = init ? s[i] : __fadd_rn(__fmul_rn(keep, t[i]), __fmul_rn(tau, s[i]));
 }
 
 // RunningMeanStd state: float64 [sum(D) | sumsq(D) | count]; mean = float32(sum / count), std = sqrt(max(float32(sumsq /
@@ -242,31 +207,6 @@ ddpg_obs_rms_kernel(const float* __restrict__ x, long long pos0, long long limit
   for (int c = threadIdx.x; c < D; c += blockDim.x) dd_rms_publish(st, D, c, mean, std);
 }
 
-// numpy's pairwise_sum (np.add.reduce of a contiguous float64 vector) of f(y[0..n)), from +0
-template <bool SQ>
-__device__ double dd_pairwise(const float* y, long long n) {
-  auto f = [](float v) { const double d = (double)v; return SQ ? __dmul_rn(d, d) : d; };
-  if (n < 8) {
-    double r = 0.0;
-    for (long long i = 0; i < n; ++i) r = __dadd_rn(r, f(y[i]));
-    return r;
-  }
-  if (n <= 128) {
-    double r[8];
-    for (int j = 0; j < 8; ++j) r[j] = f(y[j]);
-    const long long m = n - n % 8;
-    for (long long i = 8; i < m; i += 8)
-      for (int j = 0; j < 8; ++j) r[j] = __dadd_rn(r[j], f(y[i + j]));
-    double res = __dadd_rn(__dadd_rn(__dadd_rn(r[0], r[1]), __dadd_rn(r[2], r[3])),
-                           __dadd_rn(__dadd_rn(r[4], r[5]), __dadd_rn(r[6], r[7])));
-    for (long long i = m; i < n; ++i) res = __dadd_rn(res, f(y[i]));
-    return res;
-  }
-  long long n2 = n / 2;
-  n2 -= n2 % 8;
-  return __dadd_rn(dd_pairwise<SQ>(y, n2), dd_pairwise<SQ>(y + n2, n - n2));
-}
-
 // One CTA.  ret_rms.update(y) over the B targets, then (Pop-Art, w0 given) the output layers [K] + [1] of the critic and
 // the target critic: M <- M * old_std / new_std, b <- (b * old_std + old_mean - new_mean) / new_std.
 __global__ void __launch_bounds__(DD_THREADS)
@@ -277,8 +217,11 @@ ddpg_ret_rms_kernel(const float* __restrict__ y, long long B, double* __restrict
   if (threadIdx.x == 0) {
     old[0] = *mean;
     old[1] = *std;
-    st[0] = __dadd_rn(st[0], __dadd_rn(0.0, dd_pairwise<false>(y, B)));
-    st[1] = __dadd_rn(st[1], __dadd_rn(0.0, dd_pairwise<true>(y, B)));
+    // numpy's pairwise sums of the float64 vector y and of its squares
+    const double s = np_pairwise<double>([y](long long i) { return (double)y[i]; }, 0LL, B);
+    const double q = np_pairwise<double>([y](long long i) { const double v = y[i]; return __dmul_rn(v, v); }, 0LL, B);
+    st[0] = __dadd_rn(st[0], __dadd_rn(0.0, s));
+    st[1] = __dadd_rn(st[1], __dadd_rn(0.0, q));
     st[2] = __dadd_rn(st[2], (double)B);
     dd_rms_publish(st, 1, 0, mean, std);
     now[0] = *mean;
@@ -308,24 +251,14 @@ ddpg_pn_adapt_kernel(const float* __restrict__ mu, const float* __restrict__ mu_
     const float d = __fsub_rn(mu[i], mu_adapt[i]);
     s = __fadd_rn(s, __fmul_rn(d, d));
   }
-  red[threadIdx.x] = s;
-  __syncthreads();
+  const float t = cta_sum_in_order<DD_THREADS>(s, red);
   if (threadIdx.x == 0) {
-    float t = 0.0f;
-    for (int k = 0; k < DD_THREADS; ++k) t = __fadd_rn(t, red[k]);
     const float dv = sqrtf(__fdiv_rn(t, (float)n));
     *dist = dv;
     const double sd = (double)dv > desired ? __ddiv_rn(*stddev, 1.01) : __dmul_rn(*stddev, 1.01);
     *stddev = sd;
     *stddev32 = (float)sd;
   }
-}
-
-inline unsigned dd_blocks(long long work) {
-  long long blocks = (work + DD_THREADS - 1) / DD_THREADS;
-  if (blocks < 1) blocks = 1;
-  if (blocks > 16LL * device_num_sms()) blocks = 16LL * device_num_sms();
-  return (unsigned)blocks;
 }
 
 }  // namespace b200rl
@@ -345,14 +278,14 @@ extern "C" int b200rl_ddpg_encode(const float* obs, const long long* sel, long l
   B200RL_REQUIRE(!act_sel || sel, "ddpg_encode: ring actions need the ring selection");
   DdpgEncodeParams p{obs, sel, limit, B, obs_dim, mean, std, clip, act, act_sel, act ? nA : 0, in_pad,
                      reinterpret_cast<__half*>(out), overflow};
-  ddpg_encode_kernel<<<dd_blocks(B * (in_pad / 8)), DD_THREADS, 0, stream>>>(p);
+  ddpg_encode_kernel<<<grid_blocks(B * (in_pad / 8), DD_THREADS, 16), DD_THREADS, 0, stream>>>(p);
   return check_launch("ddpg_encode_kernel");
 }
 
 extern "C" int b200rl_ddpg_tanh(const float* z, long long ldz, float* mu, long long B, int nA, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(z && mu && B > 0 && nA > 0 && ldz >= nA, "ddpg_tanh: bad args");
-  ddpg_tanh_kernel<<<dd_blocks(B * nA), DD_THREADS, 0, stream>>>(z, ldz, mu, B, nA);
+  ddpg_tanh_kernel<<<grid_blocks(B * nA, DD_THREADS, 16), DD_THREADS, 0, stream>>>(z, ldz, mu, B, nA);
   return check_launch("ddpg_tanh_kernel");
 }
 
@@ -360,7 +293,7 @@ extern "C" int b200rl_ddpg_denorm(const float* q, long long ldq, const float* me
                                   long long B, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(q && out && B > 0 && ldq >= 1 && (mean == nullptr) == (std == nullptr), "ddpg_denorm: bad args");
-  ddpg_denorm_kernel<<<dd_blocks(B), DD_THREADS, 0, stream>>>(q, ldq, mean, std, out, B);
+  ddpg_denorm_kernel<<<grid_blocks(B, DD_THREADS, 16), DD_THREADS, 0, stream>>>(q, ldq, mean, std, out, B);
   return check_launch("ddpg_denorm_kernel");
 }
 
@@ -371,8 +304,8 @@ extern "C" int b200rl_ddpg_target(const float* q1, long long ldq, const long lon
   B200RL_REQUIRE(q1 && rewards && terminals && y && B > 0 && ldq >= 1, "ddpg_target: bad args");
   B200RL_REQUIRE(sel == nullptr || limit > 0, "ddpg_target: a ring selection needs limit > 0");
   B200RL_REQUIRE((mean == nullptr) == (std == nullptr), "ddpg_target: mean and std come together");
-  ddpg_target_kernel<<<dd_blocks(B), DD_THREADS, 0, stream>>>(q1, ldq, sel, limit, rewards, terminals, mean, std, gamma,
-                                                              y, B);
+  ddpg_target_kernel<<<grid_blocks(B, DD_THREADS, 16), DD_THREADS, 0, stream>>>(q1, ldq, sel, limit, rewards,
+                                                                                 terminals, mean, std, gamma, y, B);
   return check_launch("ddpg_target_kernel");
 }
 
@@ -389,8 +322,8 @@ extern "C" int b200rl_ddpg_actor_dz(const float* g, long long ldg, const float* 
                                     long long lddz, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(g && mu && dz && B > 0 && nA > 0 && ldg >= nA && lddz >= nA, "ddpg_actor_dz: bad args");
-  ddpg_actor_dz_kernel<<<dd_blocks(B * nA), DD_THREADS, 0, stream>>>(g, ldg, mu, B, nA, reinterpret_cast<__half*>(dz),
-                                                                     lddz);
+  ddpg_actor_dz_kernel<<<grid_blocks(B * nA, DD_THREADS, 16), DD_THREADS, 0, stream>>>(
+      g, ldg, mu, B, nA, reinterpret_cast<__half*>(dz), lddz);
   return check_launch("ddpg_actor_dz_kernel");
 }
 
@@ -400,18 +333,6 @@ extern "C" int b200rl_ddpg_l2(const float* w, float* g, const long long* segs, i
   B200RL_REQUIRE(w && g && segs && loss && nseg > 0, "ddpg_l2: bad args");
   ddpg_l2_kernel<<<1, 1024, 0, stream>>>(w, g, reinterpret_cast<const DdpgSeg*>(segs), nseg, reg, loss);
   return check_launch("ddpg_l2_kernel");
-}
-
-extern "C" int b200rl_ddpg_polyak(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1,
-                                  double tau, int init, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  B200RL_REQUIRE(t0 && s0 && n0 > 0 && (t1 == nullptr || (s1 && n1 > 0)), "ddpg_polyak: bad args");
-  const long long n = n0 > n1 ? n0 : n1;
-  const dim3 grid(dd_blocks(n), t1 ? 2u : 1u);
-  // (1. - tau) and tau are python floats turned into float32 constants
-  ddpg_polyak_kernel<<<grid, DD_THREADS, 0, stream>>>(t0, s0, n0, t1, s1, t1 ? n1 : 0, (float)(1.0 - tau), (float)tau,
-                                                      init);
-  return check_launch("ddpg_polyak_kernel");
 }
 
 extern "C" int b200rl_ddpg_obs_rms(const float* x, long long pos0, long long limit, long long n, int D, double* st,

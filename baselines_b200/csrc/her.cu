@@ -11,44 +11,13 @@
 //   her_loss           Q_loss = mean((y - Q)^2) and the critic head gradients; the -mean(Q_pi) head gradient
 //   her_actor_dz       the actor's head gradient: dQ/du_in / max_u + action_l2's term, through max_u * tanh'
 //   her_norm           Normalizer.update over a sample of new episodes + recompute_stats (normalizer.py:64-118)
-//   her_polyak         target <- polyak * target + (1 - polyak) * main (ddpg.py:398-399)
-// Every reduction runs in one CTA in a fixed order, so a step is deterministic run to run.
-#include "common.cuh"
+// Every reduction runs in one CTA in a fixed order, so a step is deterministic run to run.  The target update
+// (ddpg.py:398-399) is b200rl_soft_update (optim.cu).
+#include "np_sum.cuh"
 
 namespace b200rl {
 
 constexpr int HER_THREADS = 256;
-
-__device__ __forceinline__ double her_add(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float her_add(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double her_sub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float her_sub(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double her_sq(double a) { return __dmul_rn(a, a); }
-__device__ __forceinline__ float her_sq(float a) { return __fmul_rn(a, a); }
-
-// numpy's pairwise_sum of f(lo..lo+n) in the accumulator type R, from +0 (np.add.reduce along a contiguous axis, and
-// along axis 0 of an [N, 1] array): what np.linalg.norm and a one-column v.sum(axis=0) add
-template <typename R, typename F>
-__device__ R her_pairwise(F f, int lo, int n) {
-  if (n < 8) {
-    R r = R(0);
-    for (int i = 0; i < n; ++i) r = her_add(r, f(lo + i));
-    return r;
-  }
-  if (n <= 128) {
-    R r[8];
-    for (int j = 0; j < 8; ++j) r[j] = f(lo + j);
-    const int m = n - n % 8;
-    for (int i = 8; i < m; i += 8)
-      for (int j = 0; j < 8; ++j) r[j] = her_add(r[j], f(lo + i + j));
-    R res = her_add(her_add(her_add(r[0], r[1]), her_add(r[2], r[3])), her_add(her_add(r[4], r[5]), her_add(r[6], r[7])));
-    for (int i = m; i < n; ++i) res = her_add(res, f(lo + i));
-    return res;
-  }
-  int n2 = n / 2;
-  n2 -= n2 % 8;
-  return her_add(her_pairwise<R>(f, lo, n2), her_pairwise<R>(f, lo + n2, n - n2));
-}
 
 __device__ __forceinline__ double her_clip64(double x, double c) { return fmin(fmax(x, -c), c); }
 
@@ -56,12 +25,6 @@ __device__ __forceinline__ double her_clip64(double x, double c) { return fmin(f
 __device__ __forceinline__ float her_normalize(float x, const float* mean, const float* std, int c, float clip) {
   const float v = __fdiv_rn(__fsub_rn(x, mean[c]), std[c]);
   return fminf(fmaxf(v, -clip), clip);
-}
-
-__device__ __forceinline__ void her_put(__half* row, int pad, int c, float v) {
-  const __half hi = __float2half_rn(v);
-  row[c] = hi;
-  row[pad + c] = __float2half_rn(v - __half2float(hi));
 }
 
 struct HerSampleParams {
@@ -93,8 +56,9 @@ __global__ void __launch_bounds__(HER_THREADS) her_sample_kernel(const HerSample
     const double* ag1 = ag0 + p.dimg;
     const double* gs = ft >= 0 ? p.ag + (ep * T1 + ft) * p.dimg : p.g + (ep * p.T + t) * p.dimg;
     if (p.reward_type) {
-      const double d2 = her_pairwise<double>([&](int i) { const double d = __dsub_rn(ag1[i], gs[i]); return __dmul_rn(d, d); },
-                                     0, p.dimg);
+      // np.linalg.norm: numpy's pairwise sum of the squares
+      const double d2 = np_pairwise<double>([&](int i) { const double d = __dsub_rn(ag1[i], gs[i]); return __dmul_rn(d, d); },
+                                            0, p.dimg);
       const double d = __dsqrt_rn(__dadd_rn(0.0, d2));
       p.r[b] = p.reward_type == 1 ? (d > p.threshold ? -1.0f : -0.0f) : (float)(-d);
     }
@@ -114,11 +78,11 @@ __global__ void __launch_bounds__(HER_THREADS) her_sample_kernel(const HerSample
     for (int c = 0; c < p.dimo; ++c) {
       const float v0 = her_normalize((float)her_clip64(o0[c], p.clip_obs), p.o_mean, p.o_std, c, p.norm_clip);
       const float v1 = her_normalize((float)her_clip64(o1[c], p.clip_obs), p.o_mean, p.o_std, c, p.norm_clip);
-      her_put(ra, p.pad_a, c, v0);
-      her_put(rc, p.pad_c, c, v0);
-      her_put(rc2, p.pad_c, c, v0);
-      her_put(rta, p.pad_a, c, v1);
-      her_put(rtc, p.pad_c, c, v1);
+      split_f16(v0, ra[c], ra[p.pad_a + c]);
+      split_f16(v0, rc[c], rc[p.pad_c + c]);
+      split_f16(v0, rc2[c], rc2[p.pad_c + c]);
+      split_f16(v1, rta[c], rta[p.pad_a + c]);
+      split_f16(v1, rtc[c], rtc[p.pad_c + c]);
     }
     for (int i = 0; i < p.dimg; ++i) {
       const double g0 = p.relative ? __dsub_rn(gs[i], ag0[i]) : gs[i];
@@ -126,14 +90,17 @@ __global__ void __launch_bounds__(HER_THREADS) her_sample_kernel(const HerSample
       const float v0 = her_normalize((float)her_clip64(g0, p.clip_obs), p.g_mean, p.g_std, i, p.norm_clip);
       const float v1 = her_normalize((float)her_clip64(g1, p.clip_obs), p.g_mean, p.g_std, i, p.norm_clip);
       const int c = p.dimo + i;
-      her_put(ra, p.pad_a, c, v0);
-      her_put(rc, p.pad_c, c, v0);
-      her_put(rc2, p.pad_c, c, v0);
-      her_put(rta, p.pad_a, c, v1);
-      her_put(rtc, p.pad_c, c, v1);
+      split_f16(v0, ra[c], ra[p.pad_a + c]);
+      split_f16(v0, rc[c], rc[p.pad_c + c]);
+      split_f16(v0, rc2[c], rc2[p.pad_c + c]);
+      split_f16(v1, rta[c], rta[p.pad_a + c]);
+      split_f16(v1, rtc[c], rtc[p.pad_c + c]);
     }
     const double* us = p.u + (ep * p.T + t) * p.dimu;
-    for (int j = 0; j < p.dimu; ++j) her_put(rc, p.pad_c, p.dimo + p.dimg + j, __fdiv_rn((float)us[j], p.max_u[j]));
+    for (int j = 0; j < p.dimu; ++j) {
+      const int c = p.dimo + p.dimg + j;
+      split_f16(__fdiv_rn((float)us[j], p.max_u[j]), rc[c], rc[p.pad_c + c]);
+    }
   }
 }
 
@@ -149,8 +116,12 @@ her_obs_encode_kernel(const float* __restrict__ o, const float* __restrict__ g, 
     const int c = (int)(i - b * w);
     const float v = c < dimo ? her_normalize(o[b * dimo + c], o_mean, o_std, c, norm_clip)
                              : her_normalize(g[b * dimg + c - dimo], g_mean, g_std, c - dimo, norm_clip);
-    her_put(xa + b * 2 * pad_a, pad_a, c, v);
-    if (xc) her_put(xc + b * 2 * pad_c, pad_c, c, v);
+    __half* ra = xa + b * 2 * pad_a;
+    split_f16(v, ra[c], ra[pad_a + c]);
+    if (xc) {
+      __half* rc = xc + b * 2 * pad_c;
+      split_f16(v, rc[c], rc[pad_c + c]);
+    }
   }
 }
 
@@ -163,7 +134,10 @@ her_pi_kernel(const float* __restrict__ z, long long ldz, int B, int dimu, const
     const int j = (int)(i - b * dimu);
     const float v = __fmul_rn(max_u[j], tanhf(z[b * ldz + j]));
     pi[i] = v;
-    if (xc) her_put(xc + b * 2 * pad_c, pad_c, col0 + j, __fdiv_rn(v, max_u[j]));
+    if (xc) {
+      __half* rc = xc + b * 2 * pad_c;
+      split_f16(__fdiv_rn(v, max_u[j]), rc[col0 + j], rc[pad_c + col0 + j]);
+    }
   }
 }
 
@@ -189,13 +163,8 @@ her_loss_kernel(const float* __restrict__ q, long long ldq, const float* __restr
     dq[(long long)(B + b) * lddq] = __float2half_rn(-1.0f);
     q_pi[b] = q[(long long)(B + b) * ldq];
   }
-  red[threadIdx.x] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.0f;
-    for (int k = 0; k < HER_THREADS; ++k) t = __fadd_rn(t, red[k]);
-    *loss = __fdiv_rn(t, (float)B);
-  }
+  const float t = cta_sum_in_order<HER_THREADS>(s, red);
+  if (threadIdx.x == 0) *loss = __fdiv_rn(t, (float)B);
 }
 
 // dz = (g / max_u + 2 action_l2 (pi / max_u) / (max_u dimu)) * max_u * (1 - tanh(z)^2), sum scaling over the batch:
@@ -234,20 +203,20 @@ __device__ void her_norm_sums(const double* o, const double* ag, const double* g
       v = (R)o[(ep * T1 + t) * dimo + c];
     } else {
       v = (R)(ft >= 0 ? ag[(ep * T1 + ft) * dimg + c] : g[(ep * T + t) * dimg + c]);
-      if (relative) v = her_sub(v, (R)ag[(ep * T1 + t) * dimg + c]);
+      if (relative) v = sub_rn(v, (R)ag[(ep * T1 + t) * dimg + c]);
     }
     const R cl = (R)clip_obs;
     return v < -cl ? -cl : (v > cl ? cl : v);
   };
   R s = R(0), q = R(0);
   if (D == 1) {
-    s = her_pairwise<R>(val, 0, N);
-    q = her_pairwise<R>([&](int i) { return her_sq(val(i)); }, 0, N);
+    s = np_pairwise<R>(val, 0, N);
+    q = np_pairwise<R>([&](int i) { const R v = val(i); return mul_rn(v, v); }, 0, N);
   } else {
     for (int i = 0; i < N; ++i) {
       const R x = val(i);
-      s = her_add(s, x);
-      q = her_add(q, her_sq(x));
+      s = add_rn(s, x);
+      q = add_rn(q, mul_rn(x, x));
     }
   }
   *ls = (float)s;
@@ -284,23 +253,6 @@ her_norm_kernel(const double* __restrict__ o, const double* __restrict__ ag, con
   if (threadIdx.x == 0) st[2 * D] = cnt;
 }
 
-__global__ void __launch_bounds__(HER_THREADS)
-her_polyak_kernel(float* __restrict__ t0, const float* __restrict__ s0, long long n0, float* __restrict__ t1,
-                  const float* __restrict__ s1, long long n1, float keep, float mix) {
-  float* t = blockIdx.y ? t1 : t0;
-  const float* s = blockIdx.y ? s1 : s0;
-  const long long n = blockIdx.y ? n1 : n0;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    t[i] = __fadd_rn(__fmul_rn(keep, t[i]), __fmul_rn(mix, s[i]));
-}
-
-inline unsigned her_blocks(long long work) {
-  long long blocks = (work + HER_THREADS - 1) / HER_THREADS;
-  if (blocks < 1) blocks = 1;
-  if (blocks > 16LL * device_num_sms()) blocks = 16LL * device_num_sms();
-  return (unsigned)blocks;
-}
-
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -324,7 +276,7 @@ extern "C" int b200rl_her_sample(const double* o, const double* ag, const double
                     g_std, norm_clip, max_u, reward_type, threshold, r, reinterpret_cast<__half*>(xa),
                     reinterpret_cast<__half*>(xta), reinterpret_cast<__half*>(xc), reinterpret_cast<__half*>(xtc),
                     pad_a, pad_c, ag2_out, g_out, ninfo ? info_out : nullptr};
-  her_sample_kernel<<<her_blocks(B), HER_THREADS, 0, stream>>>(p);
+  her_sample_kernel<<<grid_blocks(B, HER_THREADS, 16), HER_THREADS, 0, stream>>>(p);
   return check_launch("her_sample_kernel");
 }
 
@@ -335,7 +287,7 @@ extern "C" int b200rl_her_obs_encode(const float* o, const float* g, int n, int 
   B200RL_REQUIRE(o && g && xa && o_mean && o_std && g_mean && g_std && n > 0 && dimo > 0 && dimg > 0,
                  "her_obs_encode: bad args");
   B200RL_REQUIRE(pad_a >= dimo + dimg && (xc == nullptr || pad_c >= dimo + dimg), "her_obs_encode: rows too narrow");
-  her_obs_encode_kernel<<<her_blocks((long long)n * (dimo + dimg)), HER_THREADS, 0, stream>>>(
+  her_obs_encode_kernel<<<grid_blocks((long long)n * (dimo + dimg), HER_THREADS, 16), HER_THREADS, 0, stream>>>(
       o, g, n, dimo, dimg, o_mean, o_std, g_mean, g_std, norm_clip, reinterpret_cast<__half*>(xa), pad_a,
       reinterpret_cast<__half*>(xc), pad_c);
   return check_launch("her_obs_encode_kernel");
@@ -346,8 +298,8 @@ extern "C" int b200rl_her_pi(const float* z, long long ldz, int B, int dimu, con
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(z && max_u && pi && B > 0 && dimu > 0 && ldz >= dimu, "her_pi: bad args");
   B200RL_REQUIRE(xc == nullptr || (col0 >= 0 && pad_c >= col0 + dimu), "her_pi: action columns outside the row");
-  her_pi_kernel<<<her_blocks((long long)B * dimu), HER_THREADS, 0, stream>>>(z, ldz, B, dimu, max_u, pi,
-                                                                             reinterpret_cast<__half*>(xc), pad_c, col0);
+  her_pi_kernel<<<grid_blocks((long long)B * dimu, HER_THREADS, 16), HER_THREADS, 0, stream>>>(
+      z, ldz, B, dimu, max_u, pi, reinterpret_cast<__half*>(xc), pad_c, col0);
   return check_launch("her_pi_kernel");
 }
 
@@ -355,7 +307,7 @@ extern "C" int b200rl_her_target(const float* q, long long ldq, const float* r, 
                                  float* y, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(q && r && y && B > 0 && ldq >= 1, "her_target: bad args");
-  her_target_kernel<<<her_blocks(B), HER_THREADS, 0, stream>>>(q, ldq, r, B, gamma, lo, hi, y);
+  her_target_kernel<<<grid_blocks(B, HER_THREADS, 16), HER_THREADS, 0, stream>>>(q, ldq, r, B, gamma, lo, hi, y);
   return check_launch("her_target_kernel");
 }
 
@@ -373,7 +325,7 @@ extern "C" int b200rl_her_actor_dz(const float* g, long long ldg, const float* z
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(g && z && pi && max_u && dz && B > 0 && dimu > 0 && ldg >= dimu && ldz >= dimu && lddz >= dimu,
                  "her_actor_dz: bad args");
-  her_actor_dz_kernel<<<her_blocks((long long)B * dimu), HER_THREADS, 0, stream>>>(
+  her_actor_dz_kernel<<<grid_blocks((long long)B * dimu, HER_THREADS, 16), HER_THREADS, 0, stream>>>(
       g, ldg, z, ldz, pi, B, dimu, max_u, action_l2, reinterpret_cast<__half*>(dz), lddz);
   return check_launch("her_actor_dz_kernel");
 }
@@ -388,16 +340,4 @@ extern "C" int b200rl_her_norm(const double* o, const double* ag, const double* 
   her_norm_kernel<<<2, HER_THREADS, 0, stream>>>(o, ag, g, T, dimo, dimg, sel, N, relative, clip_obs, f32_o, f32_g, o_st,
                                                  o_mean, o_std, g_st, g_mean, g_std, eps);
   return check_launch("her_norm_kernel");
-}
-
-extern "C" int b200rl_her_polyak(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1,
-                                 double polyak, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  B200RL_REQUIRE(t0 && s0 && n0 > 0 && (t1 == nullptr || (s1 && n1 > 0)), "her_polyak: bad args");
-  const long long n = n0 > n1 ? n0 : n1;
-  const dim3 grid(her_blocks(n), t1 ? 2u : 1u);
-  // polyak * v[0] + (1. - polyak) * v[1]: both python floats become float32 constants
-  her_polyak_kernel<<<grid, HER_THREADS, 0, stream>>>(t0, s0, n0, t1, s1, t1 ? n1 : 0, (float)polyak,
-                                                      (float)(1.0 - polyak));
-  return check_launch("her_polyak_kernel");
 }

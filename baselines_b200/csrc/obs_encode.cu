@@ -72,22 +72,9 @@ __global__ void __launch_bounds__(256) obs_encode_kernel(const ObsEncodeParams p
         }
         v[j] = t;
       }
-      if (p.overflow) {
-        bool over = false;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) over |= fabsf(v[j]) >= 65520.0f;    // NaN compares false: it passes through
-        if (over) *p.overflow = 1;
-      }
+      if (p.overflow && f16_overflow8(v)) *p.overflow = 1;
     }
-    __align__(16) __half hi[8], lo[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      hi[j] = __float2half_rn(v[j]);
-      lo[j] = __float2half_rn(v[j] - __half2float(hi[j]));
-    }
-    __half* o = p.out + b * (2LL * p.in_pad) + c0;
-    *reinterpret_cast<uint4*>(o) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(o + p.in_pad) = *reinterpret_cast<const uint4*>(lo);
+    store_split_f16x8(p.out + b * (2LL * p.in_pad) + c0, p.in_pad, v);
   }
 }
 
@@ -112,9 +99,6 @@ extern "C" int b200rl_obs_encode(const float* x, const long long* src_idx, long 
     B200RL_REQUIRE(raw_dim == in_dim, "obs_encode: raw_dim != in_dim");
   ObsEncodeParams p{x, src_idx, B, raw_dim, in_dim, in_pad, mean, inv_std, clip_lo, clip_hi, onehot_n,
                     onehot_n > 0 ? seg_off : nullptr, nseg, reinterpret_cast<__half*>(out), overflow};
-  const long long total = B * (in_pad / 8);
-  long long blocks = (total + 255) / 256;
-  if (blocks > 16LL * device_num_sms()) blocks = 16LL * device_num_sms();
-  obs_encode_kernel<<<(int)blocks, 256, 0, stream>>>(p);
+  obs_encode_kernel<<<grid_blocks(B * (in_pad / 8), 256, 16), 256, 0, stream>>>(p);
   return check_launch("obs_encode_kernel");
 }

@@ -219,10 +219,15 @@ dgrad_weights_kernel(const float* __restrict__ w, __half* __restrict__ out, int 
   }
 }
 
-static int grid_for(long long n, int threads, int per_sm) {
-  long long blocks = (n + threads - 1) / threads;
-  const long long cap = (long long)device_num_sms() * per_sm;
-  return (int)(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
+// Soft target update t <- keep * t + mix * s, unfused, of (t0, s0, n0) and, in grid row 1, (t1, s1, n1)
+__global__ void __launch_bounds__(256)
+soft_update_kernel(float* __restrict__ t0, const float* __restrict__ s0, long long n0, float* __restrict__ t1,
+                   const float* __restrict__ s1, long long n1, float keep, float mix) {
+  float* t = blockIdx.y ? t1 : t0;
+  const float* s = blockIdx.y ? s1 : s0;
+  const long long n = blockIdx.y ? n1 : n0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    t[i] = __fadd_rn(__fmul_rn(keep, t[i]), __fmul_rn(mix, s[i]));
 }
 
 __global__ void set_scalars_kernel(float* dst, float a, float b, float c, float d, int n) {
@@ -277,7 +282,7 @@ extern "C" int b200rl_sumsq(const float* g, long long n, double* out, void* stre
   B200RL_REQUIRE(g && out && n > 0, "sumsq: bad args");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "sumsq: gradient buffer must be 16 B aligned");
   cudaMemsetAsync(out, 0, sizeof(double), stream);
-  const int grid = grid_for(n / 4 + 1, 256, 4);
+  const int grid = grid_blocks(n / 4 + 1, 256, 4);
   B200RL_REQUIRE(grid <= SUMSQ_MAX_BLOCKS, "sumsq: %d blocks exceed the partial-sum slots", grid);
   sumsq_kernel<<<grid, 256, 0, stream>>>(g, n, out);
   return check_launch("sumsq_kernel");
@@ -301,7 +306,7 @@ extern "C" int b200rl_clip_adam(float* p, const float* g, float* m, float* v, lo
   B200RL_REQUIRE(p && g && m && v && n > 0, "clip_adam: bad args");
   B200RL_REQUIRE(clip <= 0.0f || sumsq != nullptr, "clip_adam: clipping needs the device sumsq");
   AdamArgs a{lr_t, beta1, beta2, eps, clip};
-  clip_adam_kernel<<<grid_for(n, 256, 8), 256, 0, stream>>>(p, g, m, v, n, a, sumsq, seg_off, nseg, lr_t_dev);
+  clip_adam_kernel<<<grid_blocks(n, 256, 8), 256, 0, stream>>>(p, g, m, v, n, a, sumsq, seg_off, nseg, lr_t_dev);
   return check_launch("clip_adam_kernel");
 }
 
@@ -328,7 +333,7 @@ extern "C" int b200rl_shuffle_indices(long long* out, long long n, unsigned long
   B200RL_REQUIRE(T == 0 || T * N == n, "shuffle_indices: T*N must equal n");
   int half_bits = 1;
   while ((1LL << (2 * half_bits)) < n) ++half_bits;  // domain 4^half_bits >= n: at most 4x the range (<= 4 walks expected)
-  shuffle_indices_kernel<<<grid_for(n, 256, 8), 256, 0, stream>>>(out, n, key, half_bits, T, N);
+  shuffle_indices_kernel<<<grid_blocks(n, 256, 8), 256, 0, stream>>>(out, n, key, half_bits, T, N);
   return check_launch("shuffle_indices_kernel");
 }
 
@@ -337,8 +342,19 @@ extern "C" int b200rl_clip_accumulate(const float* g, float* acc, long long n, f
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(g && acc && n > 0, "clip_accumulate: bad args");
   B200RL_REQUIRE(clip <= 0.0f || sumsq != nullptr, "clip_accumulate: clipping needs the device sumsq");
-  clip_accumulate_kernel<<<grid_for(n, 256, 8), 256, 0, stream>>>(g, acc, n, clip, weight, sumsq);
+  clip_accumulate_kernel<<<grid_blocks(n, 256, 8), 256, 0, stream>>>(g, acc, n, clip, weight, sumsq);
   return check_launch("clip_accumulate_kernel");
+}
+
+extern "C" int b200rl_soft_update(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1,
+                                  double keep, double mix, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  B200RL_REQUIRE(t0 && s0 && n0 > 0 && (t1 == nullptr || (s1 && n1 > 0)), "soft_update: bad args");
+  const long long n = n0 > n1 ? n0 : n1;
+  const dim3 grid(grid_blocks(n, 256, 16), t1 ? 2u : 1u);
+  // keep and mix are python floats; the reference's graph holds them as float32 constants
+  soft_update_kernel<<<grid, 256, 0, stream>>>(t0, s0, n0, t1, s1, t1 ? n1 : 0, (float)keep, (float)mix);
+  return check_launch("soft_update_kernel");
 }
 
 extern "C" int b200rl_cast_transpose(const float* src, int R, int C, void* dst, long long ld_dst, void* dstT,
@@ -366,8 +382,8 @@ extern "C" int b200rl_dgrad_weights(const float* w, void* out, int R, int S, int
   B200RL_REQUIRE(w && out && R > 0 && S > 0 && s > 0, "dgrad_weights: bad args");
   const int An = (R + s - 1) / s;
   const long long total = (long long)s * s * Cin * An * An * Cout;
-  dgrad_weights_kernel<<<grid_for(total, 256, 8), 256, 0, stream>>>(w, reinterpret_cast<__half*>(out), R, S, Cin,
-                                                                     Cout, s, An, ld);
+  dgrad_weights_kernel<<<grid_blocks(total, 256, 8), 256, 0, stream>>>(w, reinterpret_cast<__half*>(out), R, S, Cin,
+                                                                        Cout, s, An, ld);
   return check_launch("dgrad_weights_kernel");
 }
 
@@ -375,7 +391,7 @@ extern "C" int b200rl_cast_f32_f16(const float* src, void* dst, long long rows, 
                                    long long ld_dst, float scale, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   B200RL_REQUIRE(src && dst && rows > 0 && cols > 0, "cast: bad args");
-  cast_f32_f16_kernel<<<grid_for(rows * cols, 256, 8), 256, 0, stream>>>(src, reinterpret_cast<__half*>(dst), rows,
-                                                                         cols, ld_src, ld_dst, scale);
+  cast_f32_f16_kernel<<<grid_blocks(rows * cols, 256, 8), 256, 0, stream>>>(src, reinterpret_cast<__half*>(dst), rows,
+                                                                            cols, ld_src, ld_dst, scale);
   return check_launch("cast_f32_f16_kernel");
 }

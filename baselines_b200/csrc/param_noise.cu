@@ -85,11 +85,8 @@ dqn_param_noise_adapt_kernel(const float* __restrict__ q, const float* __restric
     }
     s += kl;
   }
-  red[threadIdx.x] = s;
-  __syncthreads();
+  const float t = cta_sum_in_order<256>(s, red);
   if (threadIdx.x == 0) {
-    float t = 0.0f;
-    for (int k = 0; k < 256; ++k) t += red[k];
     const float mean_kl = t / (float)B;
     *mean_kl_dev = mean_kl;
     const float sc = *scale_dev;

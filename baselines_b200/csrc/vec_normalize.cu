@@ -27,20 +27,11 @@
 //   vn_normalize_kernel    float32 rows clip((x - mean) / std, +-clip) computed in float64, NaN propagating.
 //   vn_rewards_kernel      one CTA: ret = ret * gamma + rew, the pairwise moments of ret, the update of the return
 //       statistics, rew = clip(rew / std, +-cliprew) rounded to float32, ret = 0 where news.
-#include "common.cuh"
+#include "np_sum.cuh"
 
 namespace b200rl {
 
 namespace {
-
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
-__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
 
 // np.clip(v, -c, c) = minimum(maximum(v, -c), c): a NaN stays NaN (fminf / fmaxf would drop it)
 __device__ __forceinline__ double clip_nan(double v, double c) {
@@ -197,22 +188,7 @@ __device__ void pw_leaves(PairwiseSmem<T>& sm, long long N) {
 // pairwise_sum of one block of n <= 128 elements f(a[0..n))
 template <typename T, typename F>
 __device__ __forceinline__ T pw_leaf(const T* a, int n, F f) {
-  if (n < 8) {
-    T res = T(0);
-    for (int i = 0; i < n; ++i) res = add_rn(res, f(a[i]));
-    return res;
-  }
-  T r[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) r[j] = f(a[j]);
-  const int m = n - n % 8;
-  for (int i = 8; i < m; i += 8) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) r[j] = add_rn(r[j], f(a[i + j]));
-  }
-  T res = add_rn(add_rn(add_rn(r[0], r[1]), add_rn(r[2], r[3])), add_rn(add_rn(r[4], r[5]), add_rn(r[6], r[7])));
-  for (int i = m; i < n; ++i) res = add_rn(res, f(a[i]));
-  return res;
+  return np_pairwise_block<T>([&](int i) { return f(a[i]); }, 0, n);
 }
 
 // thread 0: combine the leaf sums along the split tree (post-order), then add to the +0 the reduction starts from
@@ -402,12 +378,11 @@ extern "C" int b200rl_vecnorm_normalize(const void* x, int x_f64, long long N, i
   B200RL_REQUIRE(x && out && N > 0 && D > 0, "vecnorm_normalize: bad operands");
   B200RL_REQUIRE((reinterpret_cast<uintptr_t>(x) & (x_f64 ? 7 : 3)) == 0, "vecnorm_normalize: x must be aligned to its dtype");
   const long long total = N * D;
-  long long blocks = (total + 255) / 256;
-  if (blocks > 16LL * device_num_sms()) blocks = 16LL * device_num_sms();
+  const int blocks = grid_blocks(total, 256, 16);
   if (x_f64)
-    vn_normalize_kernel<double><<<(int)blocks, 256, 0, stream>>>(static_cast<const double*>(x), total, D, rms, clip, out);
+    vn_normalize_kernel<double><<<blocks, 256, 0, stream>>>(static_cast<const double*>(x), total, D, rms, clip, out);
   else
-    vn_normalize_kernel<float><<<(int)blocks, 256, 0, stream>>>(static_cast<const float*>(x), total, D, rms, clip, out);
+    vn_normalize_kernel<float><<<blocks, 256, 0, stream>>>(static_cast<const float*>(x), total, D, rms, clip, out);
   return check_launch("vn_normalize_kernel");
 }
 

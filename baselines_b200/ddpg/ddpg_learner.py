@@ -89,8 +89,6 @@ class DDPG:
             self.y = torch.zeros(cap, dtype=torch.float32, device=dev)
             self.losses = torch.zeros(2, dtype=torch.float32, device=dev)       # critic_loss, actor_loss
             self.q_act = torch.zeros(cap, dtype=torch.float32, device=dev)
-            self._sel_host = [torch.zeros(cap + 1, dtype=torch.int64).pin_memory() for _ in range(2)]
-            self._sel_done, self._sel_slot = [None, None], 0
             if param_noise is not None:
                 st = self.actor.store
                 jobs = []
@@ -122,21 +120,6 @@ class DDPG:
                         mean=mean, std=std, clip=self.observation_range[1], act=act, act_sel=act_sel,
                         nA=self.nA if act is not None else 0)
 
-    def _upload_selection(self, idxs):
-        """The ring selection into the fixed buffer the captured steps read, through one of two pinned host buffers: the
-        copy does not wait for the stream, and a host buffer is refilled only once its copy from two uploads ago ran."""
-        B = len(idxs)
-        sel = self.graphs.home("sel", self.cap + 1, (), torch.int64, self.device)[:B + 1]
-        k = self._sel_slot = self._sel_slot ^ 1
-        if self._sel_done[k] is not None:
-            self._sel_done[k].synchronize()
-        host = self._sel_host[k][:B + 1]
-        host.copy_(torch.from_numpy(self.memory.selection(idxs)))
-        sel.copy_(host, non_blocking=True)
-        ev = self._sel_done[k] = torch.cuda.Event()
-        ev.record()
-        return sel
-
     def _critic_pass(self, obs, B, sel, act, act_sel):
         """The critic over 2B rows: [obs | act] (ring rows when act_sel) and [obs | mu(obs)] of the actor's last pass."""
         c = self.critic
@@ -155,8 +138,8 @@ class DDPG:
     def initialize(self, sess=None):
         """Target networks <- online ones (:333-338)."""
         with torch.cuda.device(self.device):
-            ops.ddpg_polyak(self.target_actor.store.params, self.actor.store.params, 1.0,
-                            self.target_critic.store.params, self.critic.store.params, init=True)
+            self.target_actor.store.params.copy_(self.actor.store.params)
+            self.target_critic.store.params.copy_(self.critic.store.params)
             self.target_actor.refresh()
             self.target_critic.refresh()
 
@@ -211,7 +194,7 @@ class DDPG:
             raise ValueError(f"batch {B} exceeds the agent's capacity {self.cap}")
         a, c, ta, tc = self.actor, self.critic, self.target_actor, self.target_critic
         with torch.cuda.device(self.device):
-            sel = self._upload_selection(idxs)
+            sel = self.graphs.upload("sel", m.selection(idxs), self.cap + 1, (), torch.int64, self.device)
             self.actor_opt.begin_step(self.actor_lr)
             self.critic_opt.begin_step(self.critic_lr)
 
@@ -255,7 +238,7 @@ class DDPG:
         ta, tc = self.target_actor, self.target_critic
 
         def body():
-            ops.ddpg_polyak(ta.store.params, self.actor.store.params, self.tau, tc.store.params,
+            ops.soft_update(ta.store.params, self.actor.store.params, 1.0 - self.tau, self.tau, tc.store.params,
                             self.critic.store.params)
             ta.refresh()
             tc.refresh()
@@ -272,7 +255,7 @@ class DDPG:
         B = len(idxs)
         a, ad = self.actor, self.adaptive_param_noise_actor
         with torch.cuda.device(self.device):
-            sel = self._upload_selection(idxs)
+            sel = self.graphs.upload("sel", m.selection(idxs), self.cap + 1, (), torch.int64, self.device)
 
             def body():
                 self._perturb(ad)

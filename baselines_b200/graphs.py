@@ -12,6 +12,7 @@ B200RL_NO_GRAPHS=1 disables replay (every call runs eagerly) -- used by tests to
 import gc
 import os
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -30,6 +31,7 @@ class GraphCache:
         self.seen = set()
         self.max_graphs = max_graphs
         self.homes = {}
+        self.pinned = {}          # name -> [two pinned host buffers, the events of their last copies, last slot used]
 
     def home(self, name, rows, trailing, dtype, device):
         """The fixed buffer `name` with at least `rows` rows of shape `trailing`: captured graphs read it, each call
@@ -42,6 +44,29 @@ class GraphCache:
                 self.clear()
             buf = self.homes[name] = torch.zeros((rows,) + tuple(trailing), dtype=dtype, device=device)
         return buf
+
+    def upload(self, name, rows, capacity, trailing, dtype, device):
+        """The host rows into the first len(rows) rows of home `name` (capacity rows of shape `trailing`); -> that device
+        view.  The copy goes through one of two pinned host buffers, so it does not wait for the stream; a host buffer is
+        refilled only once the event of its copy from two uploads earlier has completed."""
+        n = len(rows)
+        if n > capacity:
+            raise ValueError(f"{n} rows exceed the capacity {capacity} of {name!r}")
+        dev = self.home(name, capacity, trailing, dtype, device)[:n]
+        ent = self.pinned.get(name)
+        if ent is None or ent[0][0].shape != (capacity,) + tuple(trailing) or ent[0][0].dtype != dtype:
+            ent = self.pinned[name] = [[torch.zeros((capacity,) + tuple(trailing), dtype=dtype).pin_memory()
+                                        for _ in range(2)], [None, None], 0]
+        hosts, done, k = ent[0], ent[1], ent[2] ^ 1
+        ent[2] = k
+        if done[k] is not None:
+            done[k].synchronize()
+        host = hosts[k][:n]
+        host.copy_(torch.from_numpy(np.ascontiguousarray(rows)))
+        dev.copy_(host, non_blocking=True)
+        done[k] = torch.cuda.Event()
+        done[k].record()
+        return dev
 
     def run(self, key, fn, allow_fallback=False):
         if not enabled() or _lib._prof is not None:            # per-call profiling needs the eager sequence

@@ -107,31 +107,12 @@ class DDPG(object):
             self.Q_pi = torch.zeros(cap, **f32)
             self.pi_main = torch.zeros(cap, self.dimu, **f32)      # pi of the main actor's last pass
             self.pi_target = torch.zeros(cap, self.dimu, **f32)
-            self._sel_host = [torch.zeros(cap, 3, dtype=torch.int64).pin_memory() for _ in range(2)]
-            self._sel_done, self._sel_slot = [None, None], 0
             self._r_host = torch.zeros(cap, dtype=torch.float32).pin_memory()
             self._norm_host = self._norm_dev = None
             self._init_target_net()
         self.graphs = graphs.GraphCache()
 
     # ---- helpers ----------------------------------------------------------------------------------------------------
-    def _upload_sel(self, rows):
-        """The sample rows into the fixed buffer the captured steps read, through one of two pinned host buffers: a
-        host buffer is refilled only once its copy from two uploads ago ran."""
-        B = len(rows)
-        if B > self.cap:
-            raise ValueError(f"batch {B} exceeds the agent's capacity {self.cap}")
-        sel = self.graphs.home("sel", self.cap, (3,), torch.int64, self.device)[:B]
-        k = self._sel_slot = self._sel_slot ^ 1
-        if self._sel_done[k] is not None:
-            self._sel_done[k].synchronize()
-        host = self._sel_host[k][:B]
-        host.copy_(torch.from_numpy(np.ascontiguousarray(rows, np.int64)))
-        sel.copy_(host, non_blocking=True)
-        ev = self._sel_done[k] = torch.cuda.Event()
-        ev.record()
-        return sel
-
     def _upload_norm_sel(self, rows):
         """The normaliser's sample rows (rollout_batch_size * T of them) through a pinned buffer of their own."""
         n = len(rows)
@@ -228,7 +209,7 @@ class DDPG(object):
         if batch is None:
             batch = self.sample_batch()
         with torch.cuda.device(self.device):
-            self._staged = self._upload_sel(batch)
+            self._staged = self.graphs.upload("sel", batch, self.cap, (3,), torch.int64, self.device)
 
     def train_device(self, stage=True):
         """One train step on the device; -> (the float32 device scalar Q_loss, the device Q_pi [B]) without a
@@ -306,15 +287,15 @@ class DDPG(object):
         return np.float32(loss.item()), q_pi.cpu().numpy().reshape(-1, 1)
 
     def _init_target_net(self):
-        ops.her_polyak(self.target_Q.store.params, self.main_Q.store.params, 0.0, self.target_pi.store.params,
-                       self.main_pi.store.params)
+        ops.soft_update(self.target_Q.store.params, self.main_Q.store.params, 0.0, 1.0, self.target_pi.store.params,
+                        self.main_pi.store.params)
         self.target_pi.refresh()
         self.target_Q.refresh()
 
     def update_target_net(self):
         def body():
-            ops.her_polyak(self.target_Q.store.params, self.main_Q.store.params, self.polyak,
-                           self.target_pi.store.params, self.main_pi.store.params)
+            ops.soft_update(self.target_Q.store.params, self.main_Q.store.params, self.polyak, 1.0 - self.polyak,
+                            self.target_pi.store.params, self.main_pi.store.params)
             self.target_pi.refresh()
             self.target_Q.refresh()
         with torch.cuda.device(self.device):

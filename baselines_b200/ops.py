@@ -347,6 +347,17 @@ def clip_accumulate(g, acc, clip, weight, sumsq_buf):
               _ptr(sumsq_buf), _stream(), label="clip_accumulate", nbytes=12.0 * g.numel())
 
 
+def soft_update(t0, s0, keep, mix, t1=None, s1=None):
+    """Soft target update t <- float32(keep) * t + float32(mix) * s of (t0, s0) and, when given, (t1, s1), one launch."""
+    for t, nm in ((t0, "t0"), (s0, "s0"), (t1, "t1"), (s1, "s1")):
+        _chk(t, torch.float32, nm)
+    if s0.numel() != t0.numel() or (t1 is not None and s1.numel() != t1.numel()):
+        raise RuntimeError("soft_update: source and target sizes differ")
+    _lib.call("b200rl_soft_update", _ptr(t0), _ptr(s0), t0.numel(), _ptr(t1), _ptr(s1),
+              0 if t1 is None else t1.numel(), float(keep), float(mix), _stream(), label="soft_update",
+              nbytes=12.0 * (t0.numel() + (0 if t1 is None else t1.numel())))
+
+
 CastJob = namedtuple("CastJob", "src R C dst ld_dst dstT ld_t scale")
 CastJob.__doc__ = """One fp32 -> fp16 operand cast (struct CastJob of csrc/optim.cu): dst[r, c] = fp16(src[r, c] * scale)
 (row pitch ld_dst) and dstT[c, r] likewise (row pitch ld_t) for the contiguous float32 [R, C] src; dst or dstT may be
@@ -677,16 +688,6 @@ def ddpg_l2(w, g, segs, reg, loss):
               label="ddpg_l2")
 
 
-def ddpg_polyak(t0, s0, tau, t1=None, s1=None, init=False):
-    for t, nm in ((t0, "t0"), (s0, "s0"), (t1, "t1"), (s1, "s1")):
-        _chk(t, torch.float32, nm)
-    if s0.numel() != t0.numel() or (t1 is not None and s1.numel() != t1.numel()):
-        raise RuntimeError("ddpg_polyak: source and target sizes differ")
-    _lib.call("b200rl_ddpg_polyak", _ptr(t0), _ptr(s0), t0.numel(), _ptr(t1), _ptr(s1),
-              0 if t1 is None else t1.numel(), float(tau), int(bool(init)), _stream(), label="ddpg_polyak",
-              nbytes=12.0 * (t0.numel() + (0 if t1 is None else t1.numel())))
-
-
 def ddpg_obs_rms(x, pos0, limit, n, D, st, mean, std):
     _chk(x, torch.float32, "x")
     _chk(st, torch.float64, "st")
@@ -793,16 +794,6 @@ def her_norm(o, ag, g, sel, N, relative, clip_obs, f32_o, f32_g, o_stats, g_stat
               _ptr(sel), int(N), int(bool(relative)), float(clip_obs), int(bool(f32_o)), int(bool(f32_g)),
               _ptr(o_stats[0]), _ptr(o_stats[1]), _ptr(o_stats[2]), _ptr(g_stats[0]), _ptr(g_stats[1]),
               _ptr(g_stats[2]), float(eps), _stream(), label="her_norm")
-
-
-def her_polyak(t0, s0, polyak, t1=None, s1=None):
-    for t, nm in ((t0, "t0"), (s0, "s0"), (t1, "t1"), (s1, "s1")):
-        _chk(t, torch.float32, nm)
-    if s0.numel() != t0.numel() or (t1 is not None and s1.numel() != t1.numel()):
-        raise RuntimeError("her_polyak: source and target sizes differ")
-    _lib.call("b200rl_her_polyak", _ptr(t0), _ptr(s0), t0.numel(), _ptr(t1), _ptr(s1),
-              0 if t1 is None else t1.numel(), float(polyak), _stream(), label="her_polyak",
-              nbytes=12.0 * (t0.numel() + (0 if t1 is None else t1.numel())))
 
 
 def acer_step(logits, ld, nA, actions, mu, B, seed=0, offset=0, offset_dev=None):

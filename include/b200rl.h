@@ -186,6 +186,11 @@ int b200rl_clip_adam(float* p, const float* g, float* m, float* v, long long n, 
  * ppo2/microbatched_model.py:60-70 sums and averages before one apply_gradients. */
 int b200rl_clip_accumulate(const float* g, float* acc, long long n, float clip, float weight, const double* sumsq,
                            void* stream);
+/* Soft (Polyak) target update t <- float32(keep) * t + float32(mix) * s, unfused, over (t0, s0, n0) and (t1, s1, n1)
+ * (t1 may be NULL) in one launch: DDPG's (1 - tau, tau) (ddpg/ddpg_learner.py:36-47), HER's (polyak, 1 - polyak)
+ * (her/ddpg.py:398-399). */
+int b200rl_soft_update(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1, double keep,
+                       double mix, void* stream);
 int b200rl_cast_transpose(const float* src, int R, int C, void* dst, long long ld_dst, void* dstT, long long ld_t,
                           float scale, void* stream);
 /* njobs cast_transpose operations in one launch.  jobs: device array of 56-byte records
@@ -325,8 +330,6 @@ int b200rl_vecnorm_add_latency(int f64, long long n, double* out, void* stream);
  *   B rows and -std (-1 when mean is NULL) on the second: gradients of the sums, the backward scales by 1/B.
  * actor_dz: dz[b, j] = fp16(g[b, j] * (1 - mu[b, j]^2)).
  * l2: one CTA; segs = nseg int64 pairs {offset, len} into w / g; g += reg * w and *loss += sum_s reg * sum(w_s^2) / 2.
- * polyak: t <- float32(1 - tau) * t + float32(tau) * s over (t0, s0, n0) and (t1, s1, n1) (t1 may be NULL), or t <- s
- *   when init.
  * obs_rms: one CTA; RunningMeanStd state st float64 [sum(D) | sumsq(D) | count] updated by each of the n rows x[(pos0 +
  *   i) % limit] in order, then mean = float32(sum / count), std = sqrtf(max(float32(sumsq / count) - mean^2, 1e-2f))
  *   (common/mpi_running_mean_std.py:29-48).
@@ -348,8 +351,6 @@ int b200rl_ddpg_loss(const float* q, long long ldq, const float* y, const float*
 int b200rl_ddpg_actor_dz(const float* g, long long ldg, const float* mu, long long B, int nA, void* dz,
                          long long lddz, void* stream);
 int b200rl_ddpg_l2(const float* w, float* g, const long long* segs, int nseg, float reg, float* loss, void* stream);
-int b200rl_ddpg_polyak(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1, double tau,
-                       int init, void* stream);
 int b200rl_ddpg_obs_rms(const float* x, long long pos0, long long limit, long long n, int D, double* st, float* mean,
                         float* std, void* stream);
 int b200rl_ddpg_ret_rms(const float* y, long long B, double* st, float* mean, float* std, float* w0, float* b0,
@@ -376,8 +377,7 @@ int b200rl_ddpg_pn_adapt(const float* mu, const float* mu_adapt, long long n, do
  * actor_dz: dz = fp16((g / max_u + 2 action_l2 (pi / max_u) / (max_u dimu)) * max_u * (1 - tanh(z)^2)).
  * norm: two CTAs (o, g statistics, float32 state [sum(D) | sumsq(D) | count]); Normalizer.update over the N samples
  *   of sel (float32 sums when f32_o / f32_g, else float64 sums rounded to float32), then recompute_stats: count += N,
- *   sum += local, sumsq += local_sq, mean = sum / count, std = sqrt(max(eps^2, sumsq / count - mean^2)).
- * polyak: t <- float32(polyak) * t + float32(1 - polyak) * s over (t0, s0, n0) and (t1, s1, n1) (t1 may be NULL). */
+ *   sum += local, sumsq += local_sq, mean = sum / count, std = sqrt(max(eps^2, sumsq / count - mean^2)). */
 int b200rl_her_sample(const double* o, const double* ag, const double* g, const double* u, const double* info, int T,
                       int dimo, int dimg, int dimu, int ninfo, const long long* sel, int B, int relative,
                       double clip_obs, const float* o_mean, const float* o_std, const float* g_mean,
@@ -398,8 +398,6 @@ int b200rl_her_actor_dz(const float* g, long long ldg, const float* z, long long
 int b200rl_her_norm(const double* o, const double* ag, const double* g, int T, int dimo, int dimg,
                     const long long* sel, int N, int relative, double clip_obs, int f32_o, int f32_g, float* o_st,
                     float* o_mean, float* o_std, float* g_st, float* g_mean, float* g_std, float eps, void* stream);
-int b200rl_her_polyak(float* t0, const float* s0, long long n0, float* t1, const float* s1, long long n1, double polyak,
-                      void* stream);
 
 /* ACER (acer/acer.py, acer/buffer.py), csrc/acer.cu.
  * step: actions int64 [B] = the Gumbel-max sample of b200rl_cat_step (same bits for the same seed / offset) and

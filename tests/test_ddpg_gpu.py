@@ -74,17 +74,21 @@ def test_encode_normalises_clips_wraps_and_appends_actions():
     assert not (np.array_equal(got_hi, inv_hi) and np.array_equal(got_lo, inv_lo))
 
 
-def test_polyak_is_the_float32_expression_bit_for_bit():
+def test_soft_update_is_the_float32_expression_bit_for_bit():
+    """ops.soft_update in DDPG's (1 - tau, tau) and HER's (polyak, 1 - polyak) forms, over two networks in one launch."""
     from baselines_b200 import ops
     rng = np.random.RandomState(1)
     t0, s0 = rng.randn(1001).astype(np.float32), rng.randn(1001).astype(np.float32)
     t1, s1 = rng.randn(77).astype(np.float32), rng.randn(77).astype(np.float32)
     a, b = _c(t0), _c(t1)
-    ops.ddpg_polyak(a, _c(s0), 0.01, b, _c(s1))
+    ops.soft_update(a, _c(s0), 1.0 - 0.01, 0.01, b, _c(s1))
     assert np.array_equal(a.cpu().numpy(), R.polyak(t0, s0, 0.01))
     assert np.array_equal(b.cpu().numpy(), R.polyak(t1, s1, 0.01))
-    ops.ddpg_polyak(a, _c(s0), 1.0, init=True)
-    assert np.array_equal(a.cpu().numpy(), s0)
+    a, b = _c(t0), _c(t1)
+    ops.soft_update(a, _c(s0), 0.95, 1.0 - 0.95, b, _c(s1))
+    her = lambda t, s: (np.float32(0.95) * t + np.float32(1.0 - 0.95) * s).astype(np.float32)
+    assert np.array_equal(a.cpu().numpy().view(np.uint32), her(t0, s0).view(np.uint32))
+    assert np.array_equal(b.cpu().numpy().view(np.uint32), her(t1, s1).view(np.uint32))
 
 
 def test_obs_rms_is_bit_for_bit_over_thousands_of_rows():
@@ -268,6 +272,9 @@ TOL = {1: 2e-2, 64: 1e-2, 1000: 1e-2}
 def test_train_step_against_float64(case, B):
     cfg = dict(BASE, **CASES[case])
     agent = _make(cfg, B)
+    # initialize() copies the online networks into the targets, bit for bit
+    for t, s in ((agent.target_actor, agent.actor), (agent.target_critic, agent.critic)):
+        assert torch.equal(t.store.params.view(torch.int32), s.store.params.view(torch.int32))
     for _ in range(2):
         agent.train_device()
         agent.update_target_net()

@@ -77,11 +77,14 @@ def _stats(agent):
 # ---------------------------------------------------------------------------------------------------------- kernels
 @pytest.mark.parametrize("relative", [False, True])
 @pytest.mark.parametrize("rtype", ["sparse", "dense"])
-def test_sample_relabels_rewards_and_encodes_bit_for_bit(relative, rtype):
+def test_cache_uploaded_sample_relabels_rewards_and_encodes_bit_for_bit(relative, rtype):
     from baselines_b200 import ops
     rng = np.random.RandomState(1)
     thr = 0.0625
     agent = _agent(relative_goals=relative, reward=(rtype, thr), max_u=[1.0, 0.5, 2.0, 1.5], buffer_episodes=8)
+    # the constructor's 0 * target + 1 * main leaves the targets equal to the main networks, bit for bit
+    for t, m in ((agent.target_pi, agent.main_pi), (agent.target_Q, agent.main_Q)):
+        assert torch.equal(t.store.params.view(torch.int32), m.store.params.view(torch.int32))
     np.random.seed(3)
     for _ in range(7):                            # 14 episodes into 8 slots: the ring fills, then random replacement
         agent.store_episode(_episodes(agent, rng, 2))
@@ -95,7 +98,7 @@ def test_sample_relabels_rewards_and_encodes_bit_for_bit(relative, rtype):
     B = agent.cap
     sel = agent.buffer.draw(B)
     sel[:4] = [[0, 3, -1], [0, 3, 4], [1, T - 1, T], [2, 0, T]]   # at the threshold, relabelled, future_t = T
-    S = agent._upload_sel(sel)
+    S = agent.graphs.upload("sel", sel, agent.cap, (3,), torch.int64, agent.device)
     pi, Q, tpi, tQ = agent.main_pi, agent.main_Q, agent.target_pi, agent.target_Q
     st = _stats(agent)
     ops.her_sample(agent.buffer.ring, S, B, relative, 200., agent.o_stats.mean, agent.o_stats.std, agent.g_stats.mean, agent.g_stats.std, 5.0,
